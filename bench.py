@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- SDS train-steps/sec (NeRF render + SD U-Net) @128x128 on N B200s (BASELINE.json metric).
+"""bench.py -- SDS train-steps/sec (NeRF render + SD U-Net) @128x128 on N H100s (BASELINE.json metric).
 
 One step == the SDS branch of Trainer.train_step (nerf/utils.py:461-574) restricted to the hot path (SURVEY.md 8d):
     model.render(128x128 rays, perturb, force_all_rays, max_steps 512, k = 13 field evaluations / sample)
@@ -13,6 +13,7 @@ Excluded like SURVEY 8d says: CLIP losses, PNG dumps, the Adan update.  Syntheti
   python bench.py --gpus 1 --steps 10 --warmup 3            # one JSON line
   torchrun ... bench.py --gpus N ...                        # one rank per GPU, weak scaling (one view per GPU per step)
   python bench.py --impl reference ...                      # the reference algorithm on the host CPU cores (oracle port)
+  python bench.py ... --dump-outputs DIR                    # also write what the last timed step computed, as DIR/<name>.npy
 """
 import argparse
 import importlib
@@ -21,6 +22,7 @@ import math
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -34,6 +36,9 @@ METRIC = "SDS train-steps/sec (NeRF render+SD U-Net) @128x128"
 UNIT = "view-steps/s"
 HW = 128
 SPHERE_R = 0.2
+# NVIDIA H100 SXM data sheet (700 W card): dense FP16 / BF16 tensor rate and HBM3 bandwidth.  The fractions below are of these figures.
+H100_FP16_DENSE_TFLOPS, H100_HBM_GBS = 989.0, 3350.0
+PEAK_SOURCE = "NVIDIA H100 SXM data sheet (dense fp16 989 TFLOP/s, HBM3 3.35 TB/s; not a measured peak)"
 WORKLOAD = ("coarse stage 128x128, SD-2.0-base architecture (random-init weights) SDS, hash-grid L=16 F=2 T=2^19 fp32, "
             "solid-sphere occupancy r=0.2, max_steps 512, k=13 field evals/sample (reference defaults lambda_orient/lambda_smooth on)")
 
@@ -211,6 +216,7 @@ def run_ours(args):
         reducer()
         if marks is not None:
             marks.append(_ev())
+        state["last"] = out, loss
         if e2e:
             result_dev[0] = loss.detach(); result_dev[1] = out['loss_orient'].detach(); result_dev[2] = out['loss_smooth'].detach()
             result_dev[3] = out['weights_sum'].mean().detach()
@@ -308,6 +314,8 @@ def run_ours(args):
     time.sleep(0.3)
     i_first = state["i"]
     ms = timed(args.steps, False, args.warmup)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, model, *state["last"])
     m_timed = m_log[[(i_first + k) % m_log.numel() for k in range(args.steps)]].cpu().numpy().astype(np.int64)
     # ---- per-kernel live timing of the dominant kernels (CUDA events on the launching stream) ----
     import ctypes as C
@@ -332,19 +340,22 @@ def run_ours(args):
             step(args.warmup + s, False)
         torch.cuda.synchronize()
     gemm_ms, gemm_n = C.c_float(0), C.c_int(0)
-    dump_path = os.path.join(ROOT, "gpurun_out", f"sd_launches_rank{rank}.txt")
-    os.makedirs(os.path.dirname(dump_path), exist_ok=True)
-    # one line per timed launch: M N K block_n splits conv batch epi ms
-    L.check(L.lib().mi3d_sd_profile_dump(guidance.engine.h, C.c_int(0), C.byref(gemm_ms), C.byref(gemm_n), dump_path.encode()), "sd_profile_dump")
-    tile_flops = attn_flops = attn_ms = 0.0
+    # one line per timed launch: M N K block_n splits conv batch epi ms (to a temporary directory: the tree may be read-only)
+    with tempfile.TemporaryDirectory(prefix="mi3d_bench_") as tmp:
+        dump_path = os.path.join(tmp, f"sd_launches_rank{rank}.txt")
+        L.check(L.lib().mi3d_sd_profile_dump(guidance.engine.h, C.c_int(0), C.byref(gemm_ms), C.byref(gemm_n), dump_path.encode()), "sd_profile_dump")
+        with open(dump_path) as fh:
+            launches = fh.read().splitlines()
+    tile_flops = tile_bytes = attn_flops = attn_ms = 0.0
     attn_n = 0
-    for ln in open(dump_path):
+    for ln in launches:
         f = ln.split()
         Mm, Nn, Kk, conv, batch, ms_l = int(f[0]), int(f[1]), int(f[2]), int(f[5]), int(f[6]), float(f[8])
         if conv == 2:
             attn_flops += 4.0 * Mm * Nn * Kk * batch; attn_ms += ms_l; attn_n += 1
         else:
             tile_flops += 2.0 * Mm * Nn * Kk * batch
+            tile_bytes += 2.0 * (Mm * Kk + Nn * Kk + Mm * Nn) * batch        # fp16 A, B and D once each
     for s in range(2):                      # untimed: first-use allocations of the host-input staging path
         step(s, True)
     ms_e2e = timed(args.steps, True, args.warmup)
@@ -372,30 +383,19 @@ def run_ours(args):
         "gpu_launches": (launches_per_step * args.steps) if launches_per_step is not None else None,
         "clocks": clock_info,
     }
-    # roofline of the dominant kernel = the tcgen05 tile kernel k_tc_gemm (every conv / linear product of the U-Net and the VAE: the
+    # roofline of the dominant kernel = the wgmma tile kernel k_tc_gemm (every conv / linear product of the U-Net and the VAE: the
     # largest share of the step).  achieved = 2*M*N*K over the engine's own launch list of the profiled steps / summed duration of
     # those launches, timed live with CUDA events around each launch (plain launches: graph replay is suspended while profiling).
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    tf_peak = float(peaks.get("bf16_tflops_sustained", 1400.0))
-    hbm = float(peaks.get("hbm_gbs", 6650.0))
-    summary = {}
-    try:
-        summary = json.load(open(os.path.join(ROOT, "profiles", "r2_summary.json")))
-    except Exception:
-        pass
+    tf_peak, hbm = H100_FP16_DENSE_TFLOPS, H100_HBM_GBS
     gemm_ms_step = gemm_ms.value / n_prof
     flops = tile_flops / n_prof
     line["roofline"] = {
-        "kernel": "tc::k_tc_gemm<64|128|160|256> (tcgen05.mma/TMEM/TMA tile kernel; all launches of one step: every conv / linear of the U-Net and the VAE)", "bound": "tensor",
+        "kernel": "tc::k_tc_gemm<64|128|160|256> (wgmma/TMA tile kernel; all launches of one step: every conv / linear of the U-Net and the VAE)", "bound": "tensor",
         "achieved": round(flops / (gemm_ms_step * 1e-3) / 1e12, 1), "peak": tf_peak, "unit": "TFLOP/s",
         "frac": round(flops / (gemm_ms_step * 1e-3) / 1e12 / tf_peak, 4),
-        "traffic": summary.get("k_tc_gemm", {}).get("dram_bytes_per_launch"),
-        "traffic_source": "ncu --set full capture committed under profiles/ (per-launch mean; not measured by this run)",
-        "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (of measured; kernel timed inside a long step)" if peaks else "fallback 1400 TFLOP/s (of fallback)",
+        "peak_source": PEAK_SOURCE,
+        "traffic": {"algorithmic_bytes_per_step": int(tile_bytes / n_prof),
+                    "source": "computed from the launch shapes: fp16 operands and output read / written once per launch (not measured)"},
         "ms_per_step": round(gemm_ms_step, 3), "launches_per_step": gemm_n.value // n_prof, "algorithmic_flops_per_step": flops,
     }
     if cupti.get("k_tc_gemm"):
@@ -404,7 +404,7 @@ def run_ours(args):
                                            "frac": round(flops / (cupti["k_tc_gemm"] * 1e-3) / 1e12 / tf_peak, 4)}
         line["kernel_ms_in_pipeline"] = {k: round(v, 3) for k, v in cupti.items()}
     if attn_n:
-        line["roofline"]["attention"] = {"kernel": "attn::k_flash_attn (tcgen05, scores in TMEM)", "ms_per_step": round(attn_ms / n_prof, 3),
+        line["roofline"]["attention"] = {"kernel": "attn::k_flash_attn (wgmma, scores in registers)", "ms_per_step": round(attn_ms / n_prof, 3),
                                          "launches_per_step": attn_n // n_prof, "achieved": round(attn_flops / (attn_ms * 1e-3) / 1e12, 1), "unit": "TFLOP/s",
                                          "frac": round(attn_flops / (attn_ms * 1e-3) / 1e12 / tf_peak, 4)}
     # second roofline: the render kernels against the HBM roofline the north_star names.  Bytes and times come from the SAME profiled
@@ -418,9 +418,7 @@ def run_ours(args):
                 fb += 13 * m_pad * 1024 + N * 44 + 262144; ft += r["k_field_fwd"]
             if "k_field_bwd_full" in r:
                 bb += 13 * m_pad * 2048 + N * 16; bt += r["k_field_bwd_full"]
-        line["roofline_render"] = {"bound": "hbm", "peak": hbm, "unit": "GB/s", "profiled_steps": prof_steps,
-                                   "traffic": {k: summary.get(k, {}).get("dram_bytes_per_launch") for k in ("k_field_fwd_tc", "k_bwd_enc_scatter", "k_field_bwd_tc")},
-                                   "traffic_source": "ncu --set full capture committed under profiles/ (not measured by this run)"}
+        line["roofline_render"] = {"bound": "hbm", "peak": hbm, "unit": "GB/s", "peak_source": PEAK_SOURCE, "profiled_steps": prof_steps}
         if ft:
             line["roofline_render"]["fwd"] = {"algorithmic_bytes": int(fb), "ms": round(ft, 3), "achieved": round(fb / (ft * 1e-3) / 1e9, 1), "frac": round(fb / (ft * 1e-3) / 1e9 / hbm, 4)}
         if bt:
@@ -436,6 +434,23 @@ def run_ours(args):
                 f.write(json.dumps(tl) + "\n")
     if world > 1:
         torch.distributed.destroy_process_group()
+
+
+def dump_outputs(out_dir, model, out, loss):
+    """What the timed step handed its caller: the render outputs, the losses and the gradients the optimiser would read.  The
+    12.2 M-entry hash-table gradient is written as a fixed, seeded sample of 1 M entries (with their indices) to stay small."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"image": out["image"], "depth": out["depth"], "weights_sum": out["weights_sum"], "loss": loss,
+              "loss_orient": out["loss_orient"], "loss_smooth": out["loss_smooth"]}
+    for name, p in model.sigma_net.named_parameters():
+        arrays["grad_sigma_net." + name] = p.grad
+    g = model.encoder.params.grad
+    idx = torch.from_numpy(np.sort(np.random.default_rng(0).choice(g.numel(), size=min(g.numel(), 1 << 20), replace=False)))
+    arrays["grad_encoder_params_sample"] = g[idx.to(g.device)]
+    arrays["grad_encoder_params_sample_index"] = idx.to(torch.float64)
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy()
+        np.save(os.path.join(out_dir, name + ".npy"), a if a.dtype == np.float64 else a.astype(np.float32))
 
 
 def cpu_baseline(args, steps=1):
@@ -514,6 +529,8 @@ def main():
     ap.add_argument("--timeline-out", default=None, help="after the timed regions, also write the per-rank phase timeline of a few extra steps to this file")
     ap.add_argument("--timeline", action="store_true",
                     help="print a per-rank CUDA-event table of the step phases instead of the bench line (for profiles/)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the outputs and gradients of the last timed step as DIR/<name>.npy (float32 / float64)")
     ap.add_argument("--launch-list", action="store_true",
                     help="profiling aid: warm up, run --steps steps of the same step function and exit (use under "
                          "`ncu --metrics gpu__time_duration.sum`; numbers printed under a profiler are never bench values)")

@@ -1,5 +1,5 @@
 /*
- * mi3d.h -- C ABI of the B200-native Make-It-3D SDS-step hot path (libmi3d.so).
+ * mi3d.h -- C ABI of the H100-native (sm_90a) Make-It-3D SDS-step hot path (libmi3d.so).
  *
  * Drop-in boundary (SURVEY.md 8b): these entry points are what the reference's pybind module `_raymarching`
  * (raymarching/src/bindings.cpp:5-23, raymarching/src/raymarching.h:7-22), its third-party tiny-cuda-nn
@@ -150,7 +150,7 @@ typedef struct { const float *w1, *b1, *w2, *b2, *w3, *b3; } mi3d_mlp;
 typedef struct { float *w1, *b1, *w2, *b2, *w3, *b3; } mi3d_mlp_grad;
 
 enum { MI3D_SHADING_ALBEDO = 0, MI3D_SHADING_LAMBERTIAN = 1, MI3D_SHADING_TEXTURELESS = 2, MI3D_SHADING_NORMAL = 3 };
-/* kernel family of the fused field.  TCGEN05 (default): tcgen05 split-precision tiles; the backward chain kernel issues the
+/* kernel family of the fused field (the names are historical).  TCGEN05 (default): wgmma split-precision tiles; the backward chain kernel issues the
  * table-gradient REDs itself (LSU-bound RED stream under the latency-bound MMA chain; = _FUSED_SCATTER).  _SPLIT_SCATTER: the
  * round-1 pipeline with a separate full-occupancy scatter kernel (A/B arm).  _SINGLE_E: fused scatter, but the encoding operand of the
  * chain kernel single-buffered (the default alternates consecutive evaluations between the two column halves of its tile; A/B arm).
@@ -203,7 +203,7 @@ typedef struct {
     uint32_t enc_cache_valid;
     /* multi-view batch: DEVICE table (NULL = one view: counter / m_fixed / align above describe the rows) and its view count.
      * With segs, loss_orient / loss_smooth / grad_loss_* are [n_views] arrays and loss_partials holds
-     * 2 * n_views * mi3d_field_grid_ctas(0) floats.  tcgen05 kernels only. */
+     * 2 * n_views * mi3d_field_grid_ctas(0) floats.  Tensor-core kernels only. */
     const mi3d_view_segs* segs;
     uint32_t n_views;
     uint32_t noise_mode;       /* in-kernel smoothness perturbation keyed by 0: (seed, row)  1: (seed, sample position) */
@@ -365,7 +365,7 @@ int mi3d_adan_step(float* param, float* grad, float* exp_avg, float* exp_avg_sq,
  * B3: Stable-Diffusion guidance  (replaces the diffusers/cuDNN/cuBLAS calls behind nerf/sd.py:117-174, :212-220)
  * ------------------------------------------------------------------------------------------------------ */
 
-/* The one tensor-core tile kernel (tcgen05.mma + TMEM accumulators + TMA operand staging) exposed directly:
+/* The one tensor-core tile kernel (wgmma with register accumulators + TMA operand staging) exposed directly:
  *   out[M,N] = alpha * A[M,K] . B[N,K]^T + bias[N] (+ residual[M,N]);  A, B fp16 K-major; out fp16 or fp32.
  * Stands in for the cuBLAS GEMM under every nn.Linear of diffusers' UNet2DConditionModel / AutoencoderKL
  * (nerf/sd.py:146, :217).  M % 128 == 0, K % 64 == 0, N % block_n == 0 (block_n in {64,128,160,256}; 0 = auto).
@@ -380,7 +380,7 @@ int mi3d_gemm_f16_splitk(const void* a, const void* b, void* out, int M, int N, 
                          const float* bias, const void* residual, void* ws, mi3d_stream_t stream);
 
 /* Fused multi-head attention, head_dim 64 (stands in for diffusers' attention processor inside BasicTransformerBlock.attn1 /
- * .attn2, nerf/sd.py:146): o = softmax(q k^T / 8) v per (batch, head), scores kept in TMEM / shared memory.
+ * .attn2, nerf/sd.py:146): o = softmax(q k^T / 8) v per (batch, head), scores kept in registers.
  * q [B*T, ldq], k and v [B*Tk, ldk / ldv], o [B*T, ldo], fp16, head h at columns [64h, 64h+64); only the first Tk_valid keys of
  * every batch take part (77 of the 128 padded text rows for cross attention).  All ld % 8 == 0. */
 int mi3d_flash_attn_f16(const void* q, const void* k, const void* v, void* o, int B, int T, int Tk, int Tk_valid, int heads,
@@ -466,8 +466,8 @@ int mi3d_sd_graph_replays(mi3d_sd_t h);
 /* debug tap: device pointer + size of a named intermediate ("unet.mid", "vae.grad_in", ...) */
 int mi3d_sd_debug_tensor(mi3d_sd_t h, const char* name, void** ptr, size_t* bytes);
 
-/* unit-test entry for the hand-written kind::tf32 tiles of the field kernels (3-term split, K-major / MN-major operands):
- * mode 0: d[128,N] = a[128,K] . b[N,K]^T ; mode 1: d = a[K,128]^T . b[K,N] ; mode 2: d = a[128,K] . b[K,N].  fp32 in/out. */
+/* unit-test entry for the hand-written wgmma tf32 tiles of the field forward (3-term split, K-major operands):
+ * mode 0 (the only one): d[128,N] = a[128,K] . b[N,K]^T, N in {16, 32, 64}, K in {32, 64, 96, 128}.  fp32 in/out. */
 int mi3d_tf32_tile_test(const float* a, const float* b, float* d, int N, int K, int mode, mi3d_stream_t stream);
 
 const char* mi3d_version(void);

@@ -109,7 +109,7 @@ SYMBOLS = [
 
 
 def build(verbose=False):
-    """Compile libmi3d.so in-tree with nvcc for sm_100a (no GPU needed)."""
+    """Compile libmi3d.so in-tree with nvcc for sm_90a (no GPU needed)."""
     out = subprocess.run(["make", "-C", os.path.join(_HERE, "csrc")], capture_output=True, text=True)
     if out.returncode != 0:
         raise Mi3dError("building libmi3d.so failed:\n" + out.stdout[-4000:] + out.stderr[-4000:])
@@ -169,4 +169,4 @@ def f32c(t):
 def require_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:
-            raise Mi3dError("mi3d operators run on sm_100a only; got a CPU tensor and there is no CPU fallback")
+            raise Mi3dError("mi3d operators run on sm_90a only; got a CPU tensor and there is no CPU fallback")

@@ -1,4 +1,4 @@
-// adan.cu -- the parameter update that follows the hot path every step (SURVEY.md 8f-1), for sm_100a (C ABI: include/mi3d.h)
+// adan.cu -- the parameter update that follows the hot path every step (SURVEY.md 8f-1), for sm_90a (C ABI: include/mi3d.h)
 //
 // Replaces, in ONE elementwise pass over a (shard of a) flat parameter vector, what the reference runs as ~25 separate torch ops per
 // tensor plus two host synchronisations:
@@ -6,8 +6,8 @@
 //     Adan.step(): global-norm clip (max_grad_norm = 5.0, .item() sync)   optimizer.py:102-131
 //                  _single_tensor_adan (foreach=False, main.py:132)        optimizer.py:201-256
 // Both clip factors derive from the one global gradient norm, which stays on the device (total_sumsq): no .item().
-// HBM-bound: 6 streams in (p, g, m, n, d, prev) and 5 out per element = 44 B/element; 12.2 M parameters -> 0.54 GB -> ~0.08 ms at
-// the measured 6.5 TB/s.  With G ranks every rank updates 1/G of the table (reduce-scatter -> this kernel -> all-gather).
+// HBM-bound: 6 streams in (p, g, m, n, d, prev) and 5 out per element = 44 B/element; 12.2 M parameters -> 0.54 GB -> ~0.16 ms at
+// the H100 SXM data-sheet 3.35 TB/s.  With G ranks every rank updates 1/G of the table (reduce-scatter -> this kernel -> all-gather).
 #include "mi3d_common.cuh"
 #include "../../include/mi3d.h"
 

@@ -2,29 +2,23 @@
 //
 // Replaces the three-launch form (batched QK^T tile GEMM -> softmax over the materialised [B*heads, T, Tk] fp16 score tensor ->
 // batched PV tile GEMM) that stood in for diffusers' attention processor under nerf/sd.py:146.  At 64x64 latents one layer's
-// score tensor is 335 MB; here scores never leave the SM: S lives in TMEM, P goes registers -> swizzled shared memory -> tcgen05.
+// score tensor is 335 MB; here scores never leave the SM: S and O live in registers, P goes straight from the S accumulator
+// registers into the A operand of the second product.
 //
-// One CTA = one 128-query tile of one (batch, head).  192 threads:
-//   warps 0-3  softmax / output owners: thread r owns query row r (TMEM lane r): reference max, running sum; O row lives in TMEM
-//   warp 4     TMA producer: Q once, K double-buffered, V single-buffered (4D maps: d, token, head, batch; 128B swizzle)
-//   warp 5     tcgen05 issuer:  S = Q K_j^T (M128 N128 K64, both K-major)  ->  TMEM cols [0,128)
-//                               O += P_j V_j (M128 N64 K128, P K-major from smem, V MN-major as loaded) -> TMEM cols [128,192)
-// Per key block j:   MMA1(j) -> s_full -> softmax(j): two TMEM passes (row max, then ex2 / sum / fp16 P into smem) -> p_full
-//                    -> MMA2(j) accumulates O in TMEM, MMA1(j+1).
-// O is rescaled lazily: probabilities are taken relative to a per-row reference maximum that is only raised when a block's maximum
-// exceeds it by more than 2^8 (then the owner multiplies its O row in TMEM by alpha with tcgen05.ld / tcgen05.st); in the common
-// case there is no per-block read-back of PV and no hand-off from the MMA warp back to the softmax warps.
-// 97 KB shared memory and 256 TMEM columns per CTA: two CTAs per SM cover each other's softmax / MMA bubbles.
+// One CTA = one 128-query tile of one (batch, head).  288 threads:
+//   warpgroups 0, 1  query rows 0..63 / 64..127 of the tile: S = Q K_j^T (wgmma m64 n128 k16, both K-major from shared memory),
+//                    online softmax in registers, O += P_j V_j (wgmma m64 n64 k16, P from registers, V MN-major as loaded)
+//   warp 8           TMA producer: Q once, K and V double-buffered (4D maps: d, token, head, batch; 128B swizzle)
+// 81 KB shared memory per CTA; S (64 registers), P (32) and O (32) per thread leave room for one CTA per SM without spills.
 #pragma once
 #include "tc_host.cuh"
 
 namespace attn {
 using namespace tc;
 
-constexpr int kThreads = 192;
+constexpr int kThreads = 288;
 constexpr int kTile = 16384;                                 // 128 rows x 128 B
-constexpr size_t kSmemBytes = 1024 + 6 * (size_t)kTile + 256;   // Q, K0, K1, V, P0, P1 + barriers
-constexpr uint32_t kTmemCols = 256;
+constexpr size_t kSmemBytes = 1024 + 5 * (size_t)kTile + 256;   // Q, K0, K1, V0, V1 + barriers
 
 struct Params {
     int T;              // queries per (batch, head)
@@ -35,66 +29,42 @@ struct Params {
 };
 
 __device__ __forceinline__ float ex2(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }   // one MUFU, no range fix-up
-__device__ __forceinline__ void tmem_ld64(uint32_t taddr, uint32_t (&v)[64]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x64.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, [%64];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31]), "=r"(v[32]), "=r"(v[33]), "=r"(v[34]), "=r"(v[35]), "=r"(v[36]), "=r"(v[37]), "=r"(v[38]), "=r"(v[39]), "=r"(v[40]), "=r"(v[41]), "=r"(v[42]), "=r"(v[43]), "=r"(v[44]), "=r"(v[45]), "=r"(v[46]), "=r"(v[47]), "=r"(v[48]), "=r"(v[49]), "=r"(v[50]), "=r"(v[51]), "=r"(v[52]), "=r"(v[53]), "=r"(v[54]), "=r"(v[55]), "=r"(v[56]), "=r"(v[57]), "=r"(v[58]), "=r"(v[59]), "=r"(v[60]), "=r"(v[61]), "=r"(v[62]), "=r"(v[63])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        :: "r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-           "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]),
-           "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]),
-           "r"(v[30]), "r"(v[31]) : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+__device__ __forceinline__ uint32_t pack_h2(float lo, float hi) {
+    const __half2 h = __floats2half2_rn(lo, hi);
+    return *reinterpret_cast<const uint32_t*>(&h);
+}
 
-static __global__ void __launch_bounds__(kThreads, 2)
+static __global__ void __launch_bounds__(kThreads, 1)
 k_flash_attn(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
              const Params p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // offset arithmetic keeps the shared address space (STS / LDS, not generic ST / LD)
     uint8_t* sQ = smem;
     uint8_t* sK = sQ + kTile;            // two stages
-    uint8_t* sV = sK + 2 * kTile;
-    uint8_t* sP = sV + kTile;            // two 64-key atoms [128 rows][128 B]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * kTile);
+    uint8_t* sV = sK + 2 * kTile;        // two stages
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sV + 2 * kTile);
     uint64_t* q_full = bars + 0;
     uint64_t* k_full = bars + 1;         // [2]
     uint64_t* k_empty = bars + 3;        // [2]
-    uint64_t* v_full = bars + 5;
-    uint64_t* v_empty = bars + 6;
-    uint64_t* s_full = bars + 7;
-    uint64_t* p_full = bars + 8;
-    uint64_t* pv_full = bars + 9;
-    uint64_t* pv_empty = bars + 10;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 11);
+    uint64_t* v_full = bars + 5;         // [2]
+    uint64_t* v_empty = bars + 7;        // [2]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int q0 = blockIdx.x * 128, head = blockIdx.y, batch = blockIdx.z;
     const int nkv = (p.kv_valid + 127) >> 7;
 
-    if (warp == 4 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         prefetch_tmap(&map_q); prefetch_tmap(&map_k); prefetch_tmap(&map_v);
         mbar_init(q_full, 1);
-        for (int s = 0; s < 2; s++) { mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 1); }
-        mbar_init(v_full, 1); mbar_init(v_empty, 1); mbar_init(s_full, 1); mbar_init(p_full, 128); mbar_init(pv_full, 1); mbar_init(pv_empty, 1);
+        for (int s = 0; s < 2; s++) { mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 8); mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], 8); }
         fence_barrier_init();
     }
-    if (warp == 5) tmem_alloc(tmem_slot, kTmemCols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 4) {
+    if (warp == 8) {
         // ===================== TMA producer =====================
         // whole warp on the (uniform) loop and the barrier waits, one elected lane issues: see tc::elect_one()
         if (elect_one()) {
@@ -104,159 +74,112 @@ k_flash_attn(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ 
         __syncwarp();
         for (int j = 0; j < nkv; j++) {
             const int st = j & 1;
-            mbar_wait(&k_empty[st], (((uint32_t)j >> 1) & 1u) ^ 1u);
+            const uint32_t par = (((uint32_t)j >> 1) & 1u) ^ 1u;
+            mbar_wait(&k_empty[st], par);
             if (elect_one()) {
                 mbar_arrive_expect_tx(&k_full[st], kTile);
                 tma_load_4d(&map_k, &k_full[st], sK + st * kTile, 0, j * 128, head, batch);
             }
             __syncwarp();
-            mbar_wait(v_empty, ((uint32_t)j & 1u) ^ 1u);
+            mbar_wait(&v_empty[st], par);
             if (elect_one()) {
-                mbar_arrive_expect_tx(v_full, kTile);
-                tma_load_4d(&map_v, v_full, sV, 0, j * 128, head, batch);
+                mbar_arrive_expect_tx(&v_full[st], kTile);
+                tma_load_4d(&map_v, &v_full[st], sV + st * kTile, 0, j * 128, head, batch);
             }
             __syncwarp();
         }
-    } else if (warp == 5) {
-        // ===================== tcgen05 issuer =====================
-        // whole warp on the (uniform) loop and the barrier waits, one elected lane issues: see tc::elect_one()
-        {
-            const uint32_t idesc_s = make_idesc_f16(128, 128, 0), idesc_pv = make_idesc_f16(128, 64, 1);
-            const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-            const uint32_t sq_u = __shfl_sync(0xffffffffu, smem_u32(sQ), 0), sk_u = sq_u + (uint32_t)kTile, sv_u = sk_u + 2u * (uint32_t)kTile, sp_u = sv_u + (uint32_t)kTile;
-            const uint32_t tmem_s = tmem_u, tmem_pv = tmem_u + 128;
-            auto issue_s = [&](int j) {
-                const int st = j & 1;
-                mbar_wait(&k_full[st], ((uint32_t)j >> 1) & 1u);
-                tc_fence_after();
-                if (elect_one()) {
-                    const uint64_t dq = make_sw128_desc(sq_u), dk = make_sw128_desc(sk_u + (uint32_t)(st * kTile));
-                    #pragma unroll
-                    for (int k = 0; k < 4; k++) umma_f16(tmem_s, dq + (uint64_t)(2 * k), dk + (uint64_t)(2 * k), idesc_s, k > 0 ? 1u : 0u);
-                    umma_commit(s_full);
-                    umma_commit(&k_empty[st]);
-                }
-                __syncwarp();
-            };
-            mbar_wait(q_full, 0);
-            issue_s(0);
-            for (int j = 0; j < nkv; j++) {
-                mbar_wait(p_full, (uint32_t)j & 1u);              // S(j) drained from TMEM, P(j) in shared memory, O row rescaled if needed
-                mbar_wait(v_full, (uint32_t)j & 1u);
-                tc_fence_after();
-                if (elect_one()) {
-                    const uint64_t dv = make_sw128_desc_mn(sv_u, 8192u);
-                    #pragma unroll
-                    for (int k = 0; k < 8; k++) {
-                        const uint64_t dp = make_sw128_desc(sp_u + (uint32_t)((k >> 2) * kTile)) + (uint64_t)(2 * (k & 3));
-                        umma_f16(tmem_pv, dp, dv + (uint64_t)(128 * k), idesc_pv, (j > 0 || k > 0) ? 1u : 0u);
-                    }
-                    umma_commit(v_empty);
-                    if (j + 1 >= nkv) umma_commit(pv_full);       // O complete
-                }
-                __syncwarp();
-                if (j + 1 < nkv) issue_s(j + 1);                  // in-order pipe: s_full(j+1) also certifies that MMA2(j) has retired
-            }
-        }
     } else {
-        // ===================== softmax / output owners: thread = query row =====================
-        const int r = warp * 32 + lane;
-        const uint32_t t_row = tmem_base + ((uint32_t)(warp * 32) << 16);
+        // ===================== warpgroup g: query rows 64 g .. 64 g + 63 of the tile =====================
+        // this thread holds rows r and r + 8 (r = 16 wl + lane / 4), columns 8 j + 2 (lane % 4) + {0, 1} of every n8 block j
+        const int g = warp >> 2, wl = warp & 3;
         const float c = p.scale_log2e;
-        float m = -INFINITY, l = 0.f;
-        uint8_t* prow = sP + r * 128;
-        const int rx = r & 7;
+        const uint32_t sq_u = smem_u32(sQ) + (uint32_t)g * 8192u, sk_u = smem_u32(sK), sv_u = smem_u32(sV);
+        float o[32];
+        #pragma unroll
+        for (int i = 0; i < 32; i++) o[i] = 0.f;
+        float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+        mbar_wait(q_full, 0);
         for (int j = 0; j < nkv; j++) {
-            mbar_wait(s_full, (uint32_t)j & 1u);          // S(j) ready; every earlier MMA (incl. the O update of block j-1) has retired
-            tc_fence_after();
-            const int kbase = j * 128;
-            const bool edge = kbase + 128 > p.kv_valid;
-            float mx = -INFINITY;
-            {   // pass 1: row maximum (two 64-column TMEM reads; compact loop on purpose: the fully unrolled, software-pipelined form
-                // ran 30 % slower -- instruction fetch with 2 warps / SMSP)
-                uint32_t v[64];
-                #pragma unroll 1
-                for (int cc = 0; cc < 2; cc++) {
-                    tmem_ld64(t_row + (uint32_t)(cc * 64), v);
-                    #pragma unroll
-                    for (int i = 0; i < 64; i++) {
-                        float s = __uint_as_float(v[i]);
-                        if (edge && kbase + cc * 64 + i >= p.kv_valid) s = -INFINITY;
-                        mx = fmaxf(mx, s);
-                    }
-                }
-            }
-            if (j == 0) m = mx;
-            else {
-                // lazy rescale: keep the old reference unless this block would push P beyond 2^8 (fp16 P, fp32 sums: no overflow)
-                const bool need = (mx - m) * c > 8.f;
-                if (__any_sync(0xffffffffu, need)) {
-                    const float alpha = need ? ex2((m - mx) * c) : 1.f;
-                    if (need) m = mx;
-                    l *= alpha;
-                    uint32_t va[32], vb[32];
-                    tmem_ld32_issue(t_row + 128u, va); tmem_ld32_issue(t_row + 160u, vb); tmem_ld_wait();
-                    #pragma unroll
-                    for (int i = 0; i < 32; i++) { va[i] = __float_as_uint(__uint_as_float(va[i]) * alpha); vb[i] = __float_as_uint(__uint_as_float(vb[i]) * alpha); }
-                    tmem_st32(t_row + 128u, va); tmem_st32(t_row + 160u, vb);
-                    tmem_st_wait();
-                }
-            }
-            const float mc = m * c;
-            float rs = 0.f;
-            {   // pass 2: P = ex2(s c - m c) -> fp16 -> swizzled shared memory (A operand of the second product), row sum
-                uint32_t v[64];
-                #pragma unroll 1
-                for (int cc = 0; cc < 2; cc++) {            // cc = 64-key atom of P
-                    tmem_ld64(t_row + (uint32_t)(cc * 64), v);
-                    uint8_t* atom = prow + cc * kTile;
-                    #pragma unroll
-                    for (int g = 0; g < 8; g++) {
-                        __align__(16) __half2 h2[4];
-                        #pragma unroll
-                        for (int i = 0; i < 4; i++) {
-                            float p0 = ex2(fmaf(__uint_as_float(v[g * 8 + 2 * i]), c, -mc)), p1 = ex2(fmaf(__uint_as_float(v[g * 8 + 2 * i + 1]), c, -mc));
-                            if (edge) {
-                                const int col = kbase + cc * 64 + g * 8 + 2 * i;
-                                if (col >= p.kv_valid) p0 = 0.f;
-                                if (col + 1 >= p.kv_valid) p1 = 0.f;
-                            }
-                            h2[i] = __floats2half2_rn(p0, p1);
-                            rs += p0 + p1;
-                        }
-                        *reinterpret_cast<uint4*>(atom + ((g ^ rx) << 4)) = *reinterpret_cast<const uint4*>(h2);     // 16-byte chunk g of the row
-                    }
-                }
-            }
-            l += rs;
-            fence_proxy_async();
-            tc_fence_before();
-            mbar_arrive(p_full);
-        }
-        mbar_wait(pv_full, 0);
-        tc_fence_after();
-        {
-            uint32_t va[32], vb[32];
-            tmem_ld32_issue(t_row + 128u, va); tmem_ld32_issue(t_row + 160u, vb); tmem_ld_wait();
-            if (q0 + r < p.T) {
-                const float inv = 1.f / l;
-                __half* dst = p.o + ((size_t)batch * p.T + q0 + r) * p.ldo + head * 64;
+            const int st = j & 1;
+            const uint32_t par = ((uint32_t)j >> 1) & 1u;
+            float s[64];
+            mbar_wait(&k_full[st], par);
+            wg::fence();
+            {
+                const uint64_t dq = wg::desc_sw128(sq_u), dk = wg::desc_sw128(sk_u + (uint32_t)(st * kTile));
                 #pragma unroll
-                for (int g = 0; g < 4; g++) {
-                    __align__(16) __half2 h2[4];
-                    #pragma unroll
-                    for (int i = 0; i < 4; i++) h2[i] = __floats2half2_rn(__uint_as_float(va[g * 8 + 2 * i]) * inv, __uint_as_float(va[g * 8 + 2 * i + 1]) * inv);
-                    *reinterpret_cast<uint4*>(dst + g * 8) = *reinterpret_cast<const uint4*>(h2);
-                    #pragma unroll
-                    for (int i = 0; i < 4; i++) h2[i] = __floats2half2_rn(__uint_as_float(vb[g * 8 + 2 * i]) * inv, __uint_as_float(vb[g * 8 + 2 * i + 1]) * inv);
-                    *reinterpret_cast<uint4*>(dst + 32 + g * 8) = *reinterpret_cast<const uint4*>(h2);
+                for (int k = 0; k < 4; k++) wg::wgmma_f16_n128<0, 0>(s, dq + (uint64_t)(2 * k), dk + (uint64_t)(2 * k), k > 0 ? 1u : 0u);
+            }
+            wg::commit();
+            wg::wait<0>();
+            wg::reg_fence(s);
+            if (lane == 0) mbar_arrive(&k_empty[st]);
+            const int kbase = j * 128;
+            if (kbase + 128 > p.kv_valid) {
+                #pragma unroll
+                for (int jj = 0; jj < 16; jj++) {
+                    const int col = kbase + 8 * jj + 2 * (lane & 3);
+                    if (col >= p.kv_valid) { s[4 * jj] = -INFINITY; s[4 * jj + 2] = -INFINITY; }
+                    if (col + 1 >= p.kv_valid) { s[4 * jj + 1] = -INFINITY; s[4 * jj + 3] = -INFINITY; }
                 }
             }
+            float mx0 = -INFINITY, mx1 = -INFINITY;
+            #pragma unroll
+            for (int jj = 0; jj < 16; jj++) {
+                mx0 = fmaxf(mx0, fmaxf(s[4 * jj], s[4 * jj + 1]));
+                mx1 = fmaxf(mx1, fmaxf(s[4 * jj + 2], s[4 * jj + 3]));
+            }
+            #pragma unroll
+            for (int off = 1; off <= 2; off <<= 1) {           // the four lanes of a row
+                mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, off));
+                mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, off));
+            }
+            // every key block holds at least one valid key, so the new maxima are finite
+            const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);
+            const float al0 = ex2((m0 - mn0) * c), al1 = ex2((m1 - mn1) * c);      // 0 on the first block (m = -inf)
+            m0 = mn0; m1 = mn1;
+            l0 *= al0; l1 *= al1;
+            #pragma unroll
+            for (int jj = 0; jj < 8; jj++) { o[4 * jj] *= al0; o[4 * jj + 1] *= al0; o[4 * jj + 2] *= al1; o[4 * jj + 3] *= al1; }
+            const float mc0 = m0 * c, mc1 = m1 * c;
+            // P = ex2(s c - m c) -> fp16 A fragments: k16 block kk of P is n8 blocks 2 kk, 2 kk + 1 of S
+            uint32_t a[8][4];
+            #pragma unroll
+            for (int kk = 0; kk < 8; kk++) {
+                float pr[8];
+                #pragma unroll
+                for (int i = 0; i < 8; i++) pr[i] = ex2(fmaf(s[8 * kk + i], c, (i & 2) ? -mc1 : -mc0));
+                l0 += (pr[0] + pr[1]) + (pr[4] + pr[5]);
+                l1 += (pr[2] + pr[3]) + (pr[6] + pr[7]);
+                a[kk][0] = pack_h2(pr[0], pr[1]); a[kk][1] = pack_h2(pr[2], pr[3]);
+                a[kk][2] = pack_h2(pr[4], pr[5]); a[kk][3] = pack_h2(pr[6], pr[7]);
+            }
+            mbar_wait(&v_full[st], par);
+            wg::fence();
+            {
+                const uint64_t dv = wg::desc_sw128(sv_u + (uint32_t)(st * kTile), 8192u);
+                #pragma unroll
+                for (int kk = 0; kk < 8; kk++) wg::wgmma_f16_rs_n64<1>(o, a[kk], dv + (uint64_t)(128 * kk), 1u);    // 16 keys = 2048 B
+            }
+            wg::commit();
+            wg::wait<0>();
+            wg::reg_fence(o);
+            if (lane == 0) mbar_arrive(&v_empty[st]);
+        }
+        #pragma unroll
+        for (int off = 1; off <= 2; off <<= 1) { l0 += __shfl_xor_sync(0xffffffffu, l0, off); l1 += __shfl_xor_sync(0xffffffffu, l1, off); }
+        const float inv0 = 1.f / l0, inv1 = 1.f / l1;
+        const int r = q0 + g * 64 + wl * 16 + (lane >> 2);
+        #pragma unroll
+        for (int hh = 0; hh < 2; hh++) {
+            if (r + 8 * hh >= p.T) continue;
+            const float inv = hh ? inv1 : inv0;
+            __half* dst = p.o + ((size_t)batch * p.T + r + 8 * hh) * p.ldo + head * 64 + 2 * (lane & 3);
+            #pragma unroll
+            for (int jj = 0; jj < 8; jj++)
+                *reinterpret_cast<__half2*>(dst + 8 * jj) = __floats2half2_rn(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 5) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 struct Maps { CUtensorMap q, k, v; };

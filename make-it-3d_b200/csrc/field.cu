@@ -1,4 +1,4 @@
-// field.cu -- fused NeRF field evaluation for sm_100a (C ABI: include/mi3d.h)
+// field.cu -- fused NeRF field evaluation for sm_90a (C ABI: include/mi3d.h)
 //
 // One kernel evaluates, per marched sample, everything nerf/network_tcnn.py:102-170 + nerf/renderer.py:513-524
 // do with 13 separate encoder/MLP passes in the reference:
@@ -16,7 +16,7 @@
 // purpose: the finite-difference normals difference two densities 0.02 apart, so the MLP needs full fp32
 // (fp16/bf16/tf32 tensor-core inputs would put ~1e-2 relative error on the normals; see DESIGN.md).
 //
-// Grid: persistent, gridDim = 148 SMs x resident CTAs; the number of valid rows is read from device memory
+// Grid: persistent, gridDim = SM count (132 on H100 SXM) x resident CTAs; the number of valid rows is read from device memory
 // (counter[0] written by mi3d_march_rays_train), so there is no host synchronisation between march and field.
 #include "mi3d_common.cuh"
 #include "tf32_tile.cuh"
@@ -117,7 +117,7 @@ __device__ __forceinline__ void scatter_levels(float* __restrict__ gtable, const
 
 // Warp-aggregated variant for the tensor-core backward: lanes are consecutive samples of (mostly) one ray, so at the coarse
 // levels whole runs of lanes fall into the same cell.  A segmented inclusive scan keyed by the table index (5 shuffle steps)
-// folds each run; only the last lane of a run issues the RED.  LSU atomics, not issue slots, bound the backward (ncu: issue 14 %).
+// folds each run; only the last lane of a run issues the RED, so the L2 sees fewer same-address atomics.
 // Must be called by all 32 lanes (inactive lanes pass active = false).
 __device__ __forceinline__ void scatter_level_agg(float* __restrict__ gtable, const LevelSm& L, float u0, float u1, float u2,
                                                   float g0, float g1, bool active, bool aggregate, int lane) {
@@ -141,7 +141,7 @@ __device__ __forceinline__ void scatter_level_agg(float* __restrict__ gtable, co
     const bool issue = active && (!aggregate || tail);
     // the two x-neighbours of a (cy, cz) corner pair are adjacent table entries whenever idx(x+1) == idx(x) ^ 1 (dense levels with an
     // even index; hashed power-of-two levels with an even cell x, where the +1 only flips bit 0 of the xor-hash): one 16-byte RED
-    // then carries both.  RED rate, not issue slots, bounds this kernel (measured), so fewer, wider REDs are the lever.
+    // then carries both.  Fewer, wider REDs cut the RED count, which is what bounds the scatter.
     #pragma unroll
     for (int yz = 0; yz < 4; yz++) {
         const uint32_t cy = cw.c[1] + (yz & 1), cz = cw.c[2] + (yz >> 1);
@@ -198,7 +198,7 @@ __device__ __forceinline__ void gather16s(const float* __restrict__ table, const
 
 // gather + trilinear blend of levels [l0, l0 + lcount) (lcount <= 8) of point u into f[2i], f[2i+1].
 // Levels are processed in PAIRS: 16 independent 8-byte loads are in flight per thread before any is consumed (the kernels
-// are bound by gather latency, not by issue slots or L1 wavefronts -- ncu: long_scoreboard dominates).
+// wait on gather latency, so loads in flight are what counts).
 __device__ __forceinline__ void gather16(const float* __restrict__ table, const LevelSm* __restrict__ lv, int l0, int lcount,
                                          float u0, float u1, float u2, float (&f)[16]) {
     #pragma unroll
@@ -624,46 +624,69 @@ __global__ void __launch_bounds__(NT, 2) k_field_fwd(const FwdArgs a) {
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// forward, tensor-core variant: the three layer GEMMs run on tcgen05.mma (kind::tf32) with a 3-term split
+// forward, tensor-core variant: the three layer GEMMs run on wgmma (tf32) with a 3-term split
 //   x = hi + lo (hi = tf32-rounded x):  A.B ~= A_hi.B_hi + A_lo.B_hi + A_hi.B_lo     (error ~2^-21, fp32-class)
 // so the finite-difference normals keep their accuracy while the MLP leaves the FFMA pipe.
-// CTA = 416 threads, one 128-sample tile at a time (persistent):
-//   warps 0-3   owners  : thread r owns sample r == TMEM lane r; epilogues (bias, ReLU, hi/lo split -> next A operand in
-//                         shared memory, UMMA K-major 128B-swizzle layout) and all per-sample math / outputs
+// CTA = 512 threads, one 128-sample tile at a time (persistent):
+//   warps 0-3   owners  : thread r owns sample r; epilogues (bias, ReLU, hi/lo split -> next A operand in shared memory,
+//                         K-major 128B-swizzle layout) and all per-sample math / outputs
 //   warps 4-11  encoders: hash-grid gathers for the NEXT evaluation while the MMA / epilogue chain of the current one runs
-//   warp 12     MMA     : one thread issues tcgen05.mma; accumulators D1 | D2 | D3 live in TMEM columns [0,64) [64,128) [128,144)
-// Hand-offs are mbarriers (count = arriving threads, or tcgen05.commit from the MMA thread).
+//   warps 12-15 MMA     : one warpgroup issues the wgmma chain; it writes each accumulator (registers, fragment layout) into a
+//                         row-major staging tile in shared memory, from which owner r reads row r
+// Hand-offs are mbarriers (count = arriving threads).
 // ---------------------------------------------------------------------------------------------------------
+// Accumulator hand-off between the MMA warpgroup and the row owners.  d[h] is an m64 accumulator (rows 64 h ..) in the wgmma fragment
+// layout; stage_frag writes its columns [c0, c0 + nc) to dst[row * ld + col - c0] (rows 0..127), stg_row32 reads one row's 32 columns.
+template <int R>
+__device__ __forceinline__ void stage_frag(const float (&d)[2][R], float* dst, int ld, int c0, int nc, int wl, int lane) {
+    #pragma unroll
+    for (int h = 0; h < 2; h++)
+        #pragma unroll
+        for (int j = 0; j < R / 4; j++)
+            #pragma unroll
+            for (int hh = 0; hh < 2; hh++) {
+                const int row = 64 * h + 16 * wl + (lane >> 2) + 8 * hh, col = 8 * j + 2 * (lane & 3) - c0;
+                if (col >= 0 && col < nc) {
+                    if (col + 1 < nc) *reinterpret_cast<float2*>(dst + row * ld + col) = make_float2(d[h][4 * j + 2 * hh], d[h][4 * j + 2 * hh + 1]);
+                    else dst[row * ld + col] = d[h][4 * j + 2 * hh];
+                }
+            }
+}
+__device__ __forceinline__ void stg_row32(const float* src, uint32_t (&v)[32]) {
+    #pragma unroll
+    for (int q = 0; q < 8; q++) {
+        const float4 t = reinterpret_cast<const float4*>(src)[q];
+        v[4 * q] = __float_as_uint(t.x); v[4 * q + 1] = __float_as_uint(t.y); v[4 * q + 2] = __float_as_uint(t.z); v[4 * q + 3] = __float_as_uint(t.w);
+    }
+}
+
 namespace fwdtc {
 using namespace ::ftc;
-constexpr int kThreads = 416;
+constexpr int kThreads = 512;
 constexpr int kA1 = 128 * 32 * 4;             // one [128 x 32] fp32 tile = 16 KB
-constexpr uint32_t kTmemCols = 256;
 // smem carve (bytes): A1_hi, A1_lo, A2_hi[2], A2_lo[2], W1_hi, W1_lo, W2_hi[2], W2_lo[2], W3_hi[2], W3_lo[2], then misc
 constexpr int oA1H = 0, oA1L = oA1H + kA1, oA2H = oA1L + kA1, oA2L = oA2H + 2 * kA1;
 constexpr int oW1H = oA2L + 2 * kA1, oW1L = oW1H + 8192, oW2H = oW1L + 8192, oW2L = oW2H + 16384;
-constexpr int oW3H = oW2L + 16384, oW3L = oW3H + 4096, oMisc = oW3L + 4096;
+constexpr int oW3H = oW2L + 16384, oW3L = oW3H + 4096, oStg = oW3L + 4096;
+constexpr int kStgLd = 68;                    // staging row stride (floats): float4 row reads by consecutive rows hit distinct banks
+constexpr int oStg3 = oStg + 128 * kStgLd * 4;    // layer-3 outputs [128][4]: kept apart so that layer 1 of the next evaluation may stage
+constexpr int oMisc = oStg3 + 128 * 4 * 4;
 constexpr size_t kSmem = 1024 + oMisc + 2048;
 
-// D (+)= A[128 x 32*KB] . B[N x 32*KB]^T over hi/lo split tiles; a_hi/a_lo/b_hi/b_lo are smem addresses of the first K-block
-__device__ __forceinline__ void issue_layer(uint32_t tmem_d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, int kblocks,
-                                            uint32_t a_kb_stride, uint32_t b_kb_stride, uint32_t idesc) {
-    uint32_t acc = 0;
+// D (+)= A[128 x 32*KB] . B[N x 32*KB]^T over hi/lo split tiles as two m64 halves; a_hi/a_lo/b_hi/b_lo are smem addresses of the first
+// K-block.  Issues, commits and waits.
+template <int N>
+__device__ __forceinline__ void mma_layer(float (&d)[2][N / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, int kblocks,
+                                          uint32_t a_kb_stride, uint32_t b_kb_stride) {
+    wg::fence();
     #pragma unroll
-    for (int kb = 0; kb < kblocks; kb++) {
-        const uint64_t dah = tc::make_sw128_desc(a_hi + kb * a_kb_stride), dal = tc::make_sw128_desc(a_lo + kb * a_kb_stride);
-        const uint64_t dbh = tc::make_sw128_desc(b_hi + kb * b_kb_stride), dbl = tc::make_sw128_desc(b_lo + kb * b_kb_stride);
-        #pragma unroll
-        for (int k = 0; k < 4; k++) {           // 4 x (K = 8 tf32 = 32 B) per 128 B swizzle row
-            umma_tf32(tmem_d, dah + 2 * k, dbh + 2 * k, idesc, acc); acc = 1;
-            umma_tf32(tmem_d, dal + 2 * k, dbh + 2 * k, idesc, 1);
-            umma_tf32(tmem_d, dah + 2 * k, dbl + 2 * k, idesc, 1);
-        }
-    }
+    for (int h = 0; h < 2; h++) issue_3tf32<N>(d[h], a_hi + 8192u * h, a_lo + 8192u * h, a_kb_stride, b_hi, b_lo, b_kb_stride, 32 * kblocks, 0u);
+    wg::commit();
+    wg::wait<0>();
+    wg::reg_fence(d[0]); wg::reg_fence(d[1]);
 }
 }  // namespace fwdtc
 
-// 13 warps are allocated as 16 for the register file -> 128 registers per thread is the hard ceiling for this CTA shape
 __global__ void __launch_bounds__(fwdtc::kThreads, 1) k_field_fwd_tc(const FwdArgs a) {
     using namespace fwdtc;
     extern __shared__ uint8_t smem_dyn[];
@@ -673,8 +696,7 @@ __global__ void __launch_bounds__(fwdtc::kThreads, 1) k_field_fwd_tc(const FwdAr
     float* b3s = b2s + 64;                                      // 4 (+pad)
     LevelSm* lv = reinterpret_cast<LevelSm*>(b3s + 8);          // 16 * 20 B
     uint64_t* bars = reinterpret_cast<uint64_t*>(sm + oMisc + 896);   // a1_full, a1_empty, d1_full, a2_full, d2_full, a3_full, d3_full
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
-    float* red = reinterpret_cast<float*>(tmem_slot + 2);       // [2][4] loss partials
+    float* red = reinterpret_cast<float*>(bars + 8);            // [2][4] loss partials
     float* s_loss = red + 8;                                    // [MI3D_MAX_VIEWS][2] per-view loss sums (multi-view batches)
     __shared__ mi3d_view_segs segs_sm;
     uint64_t *a1_full = bars, *a1_empty = bars + 1, *d1_full = bars + 2, *a2_full = bars + 3, *d2_full = bars + 4, *a3_full = bars + 5, *d3_full = bars + 6;
@@ -708,17 +730,15 @@ __global__ void __launch_bounds__(fwdtc::kThreads, 1) k_field_fwd_tc(const FwdAr
     if (a.segs && tid < (int)(sizeof(mi3d_view_segs) / 4)) reinterpret_cast<uint32_t*>(&segs_sm)[tid] = reinterpret_cast<const uint32_t*>(a.segs)[tid];
     if (tid < 2 * MI3D_MAX_VIEWS) s_loss[tid] = 0.f;
     if (tid == 0) {
-        tc::mbar_init(a1_full, 256); tc::mbar_init(a1_empty, 1); tc::mbar_init(d1_full, 1); tc::mbar_init(a2_full, 128);
-        tc::mbar_init(d2_full, 1); tc::mbar_init(a3_full, 128); tc::mbar_init(d3_full, 1);
+        tc::mbar_init(a1_full, 256); tc::mbar_init(a1_empty, 128); tc::mbar_init(d1_full, 128); tc::mbar_init(a2_full, 128);
+        tc::mbar_init(d2_full, 128); tc::mbar_init(a3_full, 128); tc::mbar_init(d3_full, 128);
         tc::fence_barrier_init();
     }
-    if (warp == 12) tc::tmem_alloc(tmem_slot, kTmemCols);
-    tc::fence_proxy_async();                 // weight tiles were written through the generic proxy, UMMA reads through the async proxy
-    tc::tc_fence_before();
+    tc::fence_proxy_async();                 // weight tiles were written through the generic proxy, wgmma reads through the async proxy
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
     const uint32_t sbase = tc::smem_u32(sm);
+    const float* stg = reinterpret_cast<const float*>(sm + oStg);
+    const float* stg3 = reinterpret_cast<const float*>(sm + oStg3);
 
     const Rows R = rows_make(a.counter, a.m_fixed, a.align, a.cap, a.segs ? &segs_sm : nullptr);
     const uint32_t m_pad = R.m_pad;
@@ -730,7 +750,6 @@ __global__ void __launch_bounds__(fwdtc::kThreads, 1) k_field_fwd_tc(const FwdAr
     if (warp < 4) {
         // ================================ owners ================================
         const int r = tid;
-        const uint32_t lane_addr = tmem + ((uint32_t)(warp * 32) << 16);
         for (uint32_t tile = blockIdx.x; (uint64_t)tile * T < m_pad; tile += gridDim.x) {
             const uint32_t row = tile * T + r;
             const RowInfo ri = row_info(R, row);
@@ -756,11 +775,10 @@ __global__ void __launch_bounds__(fwdtc::kThreads, 1) k_field_fwd_tc(const FwdAr
                 const uint32_t par = it & 1;
                 // ---- epilogue 1: H1 = relu(D1 + b1) -> A2 (hi/lo) ----
                 tc::mbar_wait(d1_full, par);
-                tc::tc_fence_after();
                 #pragma unroll 1
                 for (int c0 = 0; c0 < D_H; c0 += 32) {
                     uint32_t v[32];
-                    tc::tmem_ld32(lane_addr + (uint32_t)c0, v);
+                    stg_row32(stg + r * kStgLd + c0, v);
                     #pragma unroll
                     for (int q = 0; q < 8; q++) {
                         float h[4], l[4];
@@ -772,15 +790,13 @@ __global__ void __launch_bounds__(fwdtc::kThreads, 1) k_field_fwd_tc(const FwdAr
                     }
                 }
                 tc::fence_proxy_async();
-                tc::tc_fence_before();
                 mbar_arrive(a2_full);
                 // ---- epilogue 2: H2 = relu(D2 + b2) -> A3 (reuses the A2 tiles: layer-2 MMAs have retired) ----
                 tc::mbar_wait(d2_full, par);
-                tc::tc_fence_after();
                 #pragma unroll 1
                 for (int c0 = 0; c0 < D_H; c0 += 32) {
                     uint32_t v[32];
-                    tc::tmem_ld32(lane_addr + 64u + (uint32_t)c0, v);
+                    stg_row32(stg + r * kStgLd + c0, v);
                     #pragma unroll
                     for (int q = 0; q < 8; q++) {
                         float h[4], l[4];
@@ -792,14 +808,14 @@ __global__ void __launch_bounds__(fwdtc::kThreads, 1) k_field_fwd_tc(const FwdAr
                     }
                 }
                 tc::fence_proxy_async();
-                tc::tc_fence_before();
                 mbar_arrive(a3_full);
                 // ---- epilogue 3: outputs ----
                 tc::mbar_wait(d3_full, par);
-                tc::tc_fence_after();
                 uint32_t o4[4];
-                tmem_ld4(lane_addr + 128u, o4);
-                tc::tc_fence_before();
+                {
+                    const float4 t4 = *reinterpret_cast<const float4*>(stg3 + 4 * r);
+                    o4[0] = __float_as_uint(t4.x); o4[1] = __float_as_uint(t4.y); o4[2] = __float_as_uint(t4.z); o4[3] = __float_as_uint(t4.w);
+                }
                 float p[3];
                 eval_pos(e, x, xp, a.bound, p);
                 const float sg = expf(__uint_as_float(o4[0]) + b3s[0] + blob(p, a.blob_density, a.two_r2));
@@ -894,39 +910,28 @@ __global__ void __launch_bounds__(fwdtc::kThreads, 1) k_field_fwd_tc(const FwdAr
             }
         }
     } else {
-        // ================================ MMA issuer ================================
-        // whole warp on the (uniform) loop and the barrier waits, one elected lane issues: see tc::elect_one()
-        {
-            constexpr uint32_t id64 = idesc_tf32(128, 64), id16 = idesc_tf32(128, 16);
-            const uint32_t tm = __shfl_sync(0xffffffffu, tmem, 0), sb0 = __shfl_sync(0xffffffffu, sbase, 0);
-            for (uint32_t tile = blockIdx.x; (uint64_t)tile * T < m_pad; tile += gridDim.x) {
-                for (int e = 0; e < n_evals; e++, it++) {
-                    uint32_t sb = sb0;
-                    asm volatile("" : "+r"(sb));            // keeps the (loop-invariant) descriptors from being hoisted and spilled
-                    const uint32_t par = it & 1;
-                    tc::mbar_wait(a1_full, par);
-                    tc::tc_fence_after();
-                    if (tc::elect_one()) {
-                        issue_layer(tm, sb + oA1H, sb + oA1L, sb + oW1H, sb + oW1L, 1, kA1, 8192, id64);
-                        tc::umma_commit(a1_empty);
-                        tc::umma_commit(d1_full);
-                    }
-                    __syncwarp();
-                    tc::mbar_wait(a2_full, par);
-                    tc::tc_fence_after();
-                    if (tc::elect_one()) {
-                        issue_layer(tm + 64u, sb + oA2H, sb + oA2L, sb + oW2H, sb + oW2L, 2, kA1, 8192, id64);
-                        tc::umma_commit(d2_full);
-                    }
-                    __syncwarp();
-                    tc::mbar_wait(a3_full, par);
-                    tc::tc_fence_after();
-                    if (tc::elect_one()) {
-                        issue_layer(tm + 128u, sb + oA2H, sb + oA2L, sb + oW3H, sb + oW3L, 2, kA1, 2048, id16);
-                        tc::umma_commit(d3_full);
-                    }
-                    __syncwarp();
-                }
+        // ================================ MMA warpgroup ================================
+        float* stg_w = reinterpret_cast<float*>(sm + oStg);
+        float* stg3_w = reinterpret_cast<float*>(sm + oStg3);
+        const int wl = warp & 3;
+        for (uint32_t tile = blockIdx.x; (uint64_t)tile * T < m_pad; tile += gridDim.x) {
+            for (int e = 0; e < n_evals; e++, it++) {
+                const uint32_t par = it & 1;
+                float d[2][32];
+                tc::mbar_wait(a1_full, par);
+                mma_layer<64>(d, sbase + oA1H, sbase + oA1L, sbase + oW1H, sbase + oW1L, 1, kA1, 8192);
+                mbar_arrive(a1_empty);
+                stage_frag<32>(d, stg_w, kStgLd, 0, 64, wl, lane);
+                mbar_arrive(d1_full);
+                tc::mbar_wait(a2_full, par);
+                mma_layer<64>(d, sbase + oA2H, sbase + oA2L, sbase + oW2H, sbase + oW2L, 2, kA1, 8192);
+                stage_frag<32>(d, stg_w, kStgLd, 0, 64, wl, lane);
+                mbar_arrive(d2_full);
+                tc::mbar_wait(a3_full, par);
+                float d3[2][8];
+                mma_layer<16>(d3, sbase + oA2H, sbase + oA2L, sbase + oW3H, sbase + oW3L, 2, kA1, 2048);
+                stage_frag<8>(d3, stg3_w, 4, 0, 4, wl, lane);
+                mbar_arrive(d3_full);
             }
         }
     }
@@ -937,14 +942,12 @@ __global__ void __launch_bounds__(fwdtc::kThreads, 1) k_field_fwd_tc(const FwdAr
         for (int o = 16; o > 0; o >>= 1) { v0 += __shfl_xor_sync(0xffffffffu, v0, o); v1 += __shfl_xor_sync(0xffffffffu, v1, o); }
         if (warp < 4 && lane == 0) { red[warp] = v0; red[4 + warp] = v1; }
     }
-    tc::tc_fence_before();
     __syncthreads();
     if (tid == 0 && a.loss_partials && !a.segs) {
         a.loss_partials[2 * blockIdx.x] = (red[0] + red[1]) + (red[2] + red[3]);
         a.loss_partials[2 * blockIdx.x + 1] = (red[4] + red[5]) + (red[6] + red[7]);
     }
     if (a.loss_partials && a.segs && tid < 2 * (int)segs_sm.n_views) a.loss_partials[(size_t)blockIdx.x * 2 * segs_sm.n_views + tid] = s_loss[tid];
-    if (warp == 12) { tc::tc_fence_after(); tc::tmem_dealloc(tmem, kTmemCols); }
 }
 
 // loss_orient = sum / m_pad ; loss_smooth = sum / (3 m_pad)   (renderer.py:517-518, 523-524: .mean() over the padded rows).
@@ -1177,11 +1180,11 @@ __device__ __forceinline__ void load16(const float* __restrict__ src, float (&f)
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Split backward pipeline.  ncu showed the single-kernel tensor-core backward bound by the ~8 gather/scatter warps it can
-// afford next to 200 KB of operand tiles (issue 14 %, tensor pipe 3 %, long_scoreboard dominant).  The hash-grid gather and
+// Split backward pipeline.  The single-kernel tensor-core backward can afford only 8 gather / scatter warps next to ~200 KB of operand
+// tiles.  The hash-grid gather and
 // the RED scatter are embarrassingly parallel over (sample, level), so they run as their own full-occupancy kernels around the
 // chain kernel and exchange encodings / encoding-gradients through a per-chunk HBM buffer (128 B per evaluation each way:
-// ~1.4 GB per backward at 128x128, i.e. ~0.2 ms of HBM time for ~2x less wall time).
+// ~1.4 GB per backward at 128x128).
 //   k_bwd_encode : block = (tile, evaluation), thread = (row, group of 4 levels)  -> enc_buf[tile][e][row][32]
 //   k_field_bwd_tc (ext mode): loads enc, runs the MMA chain, stores d(enc) -> denc_buf
 //   k_bwd_scatter: same mapping as encode, warp-aggregated REDs (lanes = consecutive samples of a ray)
@@ -1262,30 +1265,31 @@ __global__ void __launch_bounds__(512, 2) k_bwd_enc_scatter(const BwdArgs a) {
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// backward, tensor-core variant.  Same roles as k_field_fwd_tc; per evaluation the MMA thread runs
+// backward, tensor-core variant.  Same roles as k_field_fwd_tc; per evaluation the MMA warpgroup runs
 //   F1: D1 = Enc W1^T          F2: D2 = H1 W2^T                               (recompute, K-major operands)
 //   G2: dH1 = dZ2 W2           WG2: dW2 += dZ2^T H1   (A3/A2/W2 tiles re-read MN-major: no transposed copies)
 //   G1: dEnc = dZ1 W1          WG1: dW1 += dZ1^T Enc
-// all as bf16 3-way splits x = h + m + l with six product terms (kind::f16, fp32-class; 16-bit operands can be consumed
-// MN-major, kind::tf32 cannot).  dW2 / dW1 accumulate in TMEM across the whole persistent CTA (M = 128 with the upper 64 rows
-// unused) and are flushed once at the end.  dZ3 -> dH2 (K = 4) and dW3 / db3 stay on the owner threads; db2 / db1 are column
-// sums of the dZ tiles taken by the encoder warps, which also read dEnc straight from TMEM and scatter it (RED.v2.f32).
-// TMEM columns: D1 [0,64) D2 [64,128) dH1 [128,192) dEnc [192,224) dW2 [256,320) dW1 [320,352).
+// all as bf16 3-way splits x = h + m + l with six product terms (wgmma bf16, fp32-class; 16-bit operands can be consumed
+// MN-major, tf32 ones cannot).  dW2 / dW1 accumulate in the MMA warpgroup's registers across the whole persistent CTA and are
+// flushed once at the end.  D1 / D2 / dH1 reach the owners through a [128 x 32] staging tile, half an accumulator at a time
+// (stg_full / stg_empty); dEnc is written as fp32 [128][32] over the dZ tiles once G1 / WG1 have retired, the encoder warps read it
+// there (d4_full -> denc_free) and scatter it (RED.v2.f32).  dZ3 -> dH2 (K = 4) and dW3 / db3 stay on the owner threads; db2 / db1
+// are column sums the owners take from registers.
 // ---------------------------------------------------------------------------------------------------------
 namespace bwdtc {
 using namespace ::fbf;
-constexpr int kThreads = 416;
+constexpr int kThreads = 512;
 constexpr int kTile = 128 * 128;               // one [128 x 64 bf16] tile = 16 KB
-constexpr uint32_t kTmemCols = 512;
 // every operand = three part tiles (h, m, l) back to back; tiles are [rows x 64 bf16]
 constexpr int oE = 0;                                              // Enc  3 x [128 x 64] (cols 32..63 stay zero)
 constexpr int oH = oE + 3 * kTile;                                 // H1   3 x [128 x 64]
 constexpr int oZ = oH + 3 * kTile;                                 // dZ2 then dZ1, 3 x [128 x 64]
 constexpr int oW1 = oZ + 3 * kTile;                                // W1   3 x [64 x 64] (cols 32..63 zero)
 constexpr int oW2 = oW1 + 3 * 8192;                                // W2   3 x [64 x 64]
-constexpr int oMisc = oW2 + 3 * 8192;
+constexpr int oStg = oW2 + 3 * 8192;                               // staging [128][kStgLd] fp32: 32 accumulator columns at a time
+constexpr int kStgLd = 36;
+constexpr int oMisc = oStg + 128 * kStgLd * 4;
 constexpr size_t kSmem = 1024 + oMisc + 3072;
-constexpr uint32_t cD1 = 0, cD2 = 64, cG2 = 128, cG1 = 192, cW2 = 256, cW1 = 320;
 
 // column-wise sum over the 32 lanes of a warp of v[0..31]; lane j returns the total of column j (recursive halving, 31 shuffles)
 __device__ __forceinline__ float warp_colsum32(float (&v)[32], int lane) {
@@ -1316,9 +1320,8 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
     float* w3s = b2s + 64;                                      // [4][64]
     LevelSm* lv = reinterpret_cast<LevelSm*>(w3s + 256);        // 16 * 20 B = 320 B  (ends at 1856)
     uint64_t* bars = reinterpret_cast<uint64_t*>(sm + oMisc + 2048);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 12);
-    uint64_t *a1_full = bars, *d1_full = bars + 1, *a2_full = bars + 2, *d2_full = bars + 3, *a3_full = bars + 4,
-             *d3_full = bars + 6, *a4_full = bars + 7, *d4_full = bars + 9;
+    uint64_t *a1_full = bars, *d1_full = bars + 1, *a2_full = bars + 2, *a3_full = bars + 3, *a4_full = bars + 4, *d4_full = bars + 5,
+             *stg_full = bars + 6, *stg_empty = bars + 7, *denc_free = bars + 8;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     for (int i = tid; i < (oMisc - oE) / 16; i += kThreads) reinterpret_cast<uint4*>(sm + oE)[i] = make_uint4(0, 0, 0, 0);   // zero pads, finite tiles
@@ -1345,16 +1348,13 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
     }
     if (a.segs && tid < (int)(sizeof(mi3d_view_segs) / 4)) reinterpret_cast<uint32_t*>(&segs_sm)[tid] = reinterpret_cast<const uint32_t*>(a.segs)[tid];
     if (tid == 0) {
-        tc::mbar_init(a1_full, 256); tc::mbar_init(d1_full, 1); tc::mbar_init(a2_full, 128); tc::mbar_init(d2_full, 1);
-        tc::mbar_init(a3_full, 128); tc::mbar_init(d3_full, 1); tc::mbar_init(a4_full, 128); tc::mbar_init(d4_full, 1);
+        tc::mbar_init(a1_full, 256); tc::mbar_init(d1_full, 128); tc::mbar_init(a2_full, 128); tc::mbar_init(a3_full, 128);
+        tc::mbar_init(a4_full, 128); tc::mbar_init(d4_full, 128); tc::mbar_init(stg_full, 128); tc::mbar_init(stg_empty, 128);
+        tc::mbar_init(denc_free, 256);
         tc::fence_barrier_init();
     }
-    if (warp == 12) tc::tmem_alloc(tmem_slot, kTmemCols);
     tc::fence_proxy_async();
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
     const uint32_t sbase = tc::smem_u32(sm);
 
     const Rows R = rows_make(a.counter, a.m_fixed, a.align, a.cap, a.segs ? &segs_sm : nullptr);
@@ -1368,7 +1368,14 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
     if (warp < 4) {
         // ================================ owners ================================
         const int r = tid;
-        const uint32_t lane_addr = tmem + ((uint32_t)(warp * 32) << 16);
+        const float* stg = reinterpret_cast<const float*>(sm + oStg);
+        uint32_t su = 0;                     // staging hand-offs taken so far (mbarrier phase)
+        auto stg_take = [&](uint32_t (&v)[32]) {
+            tc::mbar_wait(stg_full, su & 1u);
+            stg_row32(stg + r * kStgLd, v);
+            mbar_arrive(stg_empty);
+            su++;
+        };
         // persistent partial sums over this warp's rows: lane j owns columns j and j+32 of dW3[o][.] ; db3 on lane o
         float aw3[4][2] = {{0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}}, ab3 = 0.f;
         // db2 / db1 = column sums of dZ2 / dZ1 over this warp's rows, same lane <-> column mapping.  (Round 1 had the encoder warps
@@ -1394,7 +1401,6 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                 sample_out_grads(a, row, real, d, lit, light, Go, Gs, need_ptaps, dh, dtap);
             }
             for (int e = 0; e < e_end; e++, it++) {
-                const uint32_t par = it & 1;
                 float dO[4] = {0.f, 0.f, 0.f, 0.f};
                 if (e == 0) { dO[0] = dh[0]; dO[1] = dh[1]; dO[2] = dh[2]; dO[3] = dh[3]; }
                 else {
@@ -1403,12 +1409,10 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                 }
                 uint32_t m1[2] = {0u, 0u};
                 // ---- epilogue 1: H1 = relu(D1 + b1) -> A2 ; remember the ReLU mask ----
-                tc::mbar_wait(d1_full, par);
-                tc::tc_fence_after();
                 #pragma unroll 1
                 for (int c0 = 0; c0 < D_H; c0 += 32) {
                     uint32_t v[32];
-                    tc::tmem_ld32(lane_addr + cD1 + (uint32_t)c0, v);
+                    stg_take(v);
                     uint32_t mk = 0u;
                     float tv[32];
                     #pragma unroll
@@ -1423,16 +1427,14 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                     m1[c0 >> 5] = mk;
                 }
                 tc::fence_proxy_async();
-                tc::tc_fence_before();
                 mbar_arrive(a2_full);
                 // ---- epilogue 2: H2 = relu(D2 + b2) ; dZ2 = relu'(H2) * (dO W3) -> A3 ; dW3 / db3 partial sums ----
-                tc::mbar_wait(d2_full, par);
-                tc::tc_fence_after();
-                if (it > 0) tc::mbar_wait(d4_full, (it - 1) & 1);   // A3 (the dZ tiles) free: the previous evaluation's G1 / WG1 have retired
+                // A3 (the dZ tiles) free: the previous evaluation's G1 / WG1 have retired and its dEnc (written over them) was read
+                if (it > 0) tc::mbar_wait(denc_free, (it - 1) & 1);
                 #pragma unroll 1
                 for (int c0 = 0; c0 < D_H; c0 += 32) {
                     uint32_t v[32];
-                    tc::tmem_ld32(lane_addr + cD2 + (uint32_t)c0, v);
+                    stg_take(v);
                     float h2[32];
                     #pragma unroll
                     for (int j = 0; j < 32; j++) h2[j] = fmaxf(__uint_as_float(v[j]) + b2s[c0 + j], 0.f);
@@ -1469,7 +1471,6 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                     }
                 }
                 tc::fence_proxy_async();
-                tc::tc_fence_before();
                 mbar_arrive(a3_full);
                 {   // db3[o] = sum of dO[o] over rows: lane o keeps the total
                     float s0 = dO[0], s1 = dO[1], s2 = dO[2], s3 = dO[3];
@@ -1481,12 +1482,10 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                     ab3 += lane == 0 ? s0 : (lane == 1 ? s1 : (lane == 2 ? s2 : (lane == 3 ? s3 : 0.f)));
                 }
                 // ---- epilogue 3: dZ1 = relu'(H1) * dH1 -> A3 (after G2 / WG2 retired and the db2 readers are done) ----
-                tc::mbar_wait(d3_full, par);
-                tc::tc_fence_after();
                 #pragma unroll 1
                 for (int c0 = 0; c0 < D_H; c0 += 32) {
                     uint32_t v[32];
-                    tc::tmem_ld32(lane_addr + cG2 + (uint32_t)c0, v);
+                    stg_take(v);
                     const uint32_t mk = m1[c0 >> 5];
                     float tv[32];
                     #pragma unroll
@@ -1501,7 +1500,6 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                     ab1[c0 >> 5] += warp_colsum32(tv, lane);          // db1
                 }
                 tc::fence_proxy_async();
-                tc::tc_fence_before();
                 mbar_arrive(a4_full);
             }
         }
@@ -1513,8 +1511,9 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
         atomicAdd(a.g_mlp.b1 + lane, ab1[0]); atomicAdd(a.g_mlp.b1 + 32 + lane, ab1[1]);
     } else if (warp < 12) {
         // ================================ encoders / scatterers ================================
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 96;");
         const int et = tid - 128, r = et & (T - 1), half = et >> 7;
-        const uint32_t lane_addr = tmem + ((uint32_t)((warp & 3) * 32) << 16);
+        const float* denc = reinterpret_cast<const float*>(sm + oZ);
         const bool ext = a.enc_buf != nullptr, ext_out = a.denc_buf != nullptr, pp = a.e_pingpong != 0;
         for (uint32_t tile = a.tile0 + blockIdx.x; tile < a.tile1 && (uint64_t)tile * T < m_pad; tile += gridDim.x) {
             const uint32_t row = tile * T + r;
@@ -1530,7 +1529,7 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
             }
             // Software pipeline over the evaluations of this tile.
             //   single-buffered E (pp == false): write E(e+1) as soon as chain(e) has retired (d4) and BEFORE scattering dEnc(e), so that the
-            //     MMA / epilogue chain of e+1 overlaps the scatter of e and the gather of e+2.  The hand-off (d4 -> TMEM load -> split -> store ->
+            //     MMA / epilogue chain of e+1 overlaps the scatter of e and the gather of e+2.  The hand-off (d4 -> dEnc load -> split -> store ->
             //     a1) sits on the chain's critical path.
             //   ping-pong E (pp == true): the encoding uses 32 of the tile's 64 columns, so evaluation `it` lives in columns 32 (it & 1) .. + 31
             //     (operand start address + 64 B).  E(it+2) is written at the END of iteration `it` (its half was last read by chain(it), retired
@@ -1573,12 +1572,15 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                 const int en = pp ? e + 2 : e + 1;              // the evaluation whose encodings this iteration hands over
                 // single-buffered: prefetch the next evaluation's gather while the MMA / epilogue chain of this one runs
                 if (!pp && en < e_end) fetch(en, f);
-                // dEnc (this thread's 16 columns of its row) straight from TMEM into registers
+                // dEnc (this thread's 16 columns of its row: 8j + 4 half .. + 3, j = 0..3) into registers
                 tc::mbar_wait(d4_full, par);
-                tc::tc_fence_after();
                 uint32_t g[16];
-                tmem_ld4x4(lane_addr + cG1 + (uint32_t)(4 * half), g);      // columns 8j + 4 half .. + 3, j = 0..3
-                tc::tc_fence_before();
+                #pragma unroll
+                for (int j = 0; j < 4; j++) {
+                    const float4 t = *reinterpret_cast<const float4*>(denc + r * 32 + 8 * j + 4 * half);
+                    g[4 * j] = __float_as_uint(t.x); g[4 * j + 1] = __float_as_uint(t.y); g[4 * j + 2] = __float_as_uint(t.z); g[4 * j + 3] = __float_as_uint(t.w);
+                }
+                mbar_arrive(denc_free);
                 // chain(e) has retired: E is free -> hand the next evaluation to the MMA warp before scattering this one
                 if (!pp && en < e_end) write_E(f, it + 1);
                 if (pp && en < e_end) fetch(en, f);            // ping-pong: loads in flight under the scatter
@@ -1600,87 +1602,97 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
             }
         }
     } else {
-        // ================================ MMA issuer ================================
-        // The whole warp walks the loop and the barrier waits; one elected lane issues.  tmem / smem bases go through a lane-0 broadcast so
-        // that the compiler keeps every tcgen05 operand in uniform registers (see tc::elect_one).
-        {
-            const uint32_t tm = __shfl_sync(0xffffffffu, tmem, 0), sb0 = __shfl_sync(0xffffffffu, sbase, 0);
-            const bool pp = a.e_pingpong != 0;
-            uint32_t accW = 0;
-            for (uint32_t tile = a.tile0 + blockIdx.x; tile < a.tile1 && (uint64_t)tile * T < m_pad; tile += gridDim.x) {
-                for (int e = 0; e < e_end; e++, it++) {
-                    // the ~100 descriptors are loop-invariant; left alone the compiler hoists them all out of the loops and spills them.
-                    // Re-deriving them from an opaque copy of the base keeps them as a few uniform adds next to each use.
-                    uint32_t sb = sb0;
-                    asm volatile("" : "+r"(sb));
-                    // MN-major with M = 128 reads a second 64-column block at +lbo: it lands on the next part tile (finite; rows 64.. of D unused)
-                    const uint32_t eoff = pp ? 64u * (it & 1u) : 0u;            // ping-pong E: columns 32 (it & 1) .. + 31 of the tile
-                    const Operand Ek{sb + oE + eoff, (uint32_t)kTile, 16u, 0}, Em{sb + oE + eoff, (uint32_t)kTile, (uint32_t)kTile, 1};
-                    const Operand Hk{sb + oH, (uint32_t)kTile, 16u, 0}, Hm{sb + oH, (uint32_t)kTile, (uint32_t)kTile, 1};
-                    const Operand Zk{sb + oZ, (uint32_t)kTile, 16u, 0}, Zm{sb + oZ, (uint32_t)kTile, (uint32_t)kTile, 1};
-                    const Operand W1k{sb + oW1, 8192u, 16u, 0}, W1m{sb + oW1, 8192u, 8192u, 1};
-                    const Operand W2k{sb + oW2, 8192u, 16u, 0}, W2m{sb + oW2, 8192u, 8192u, 1};
-                    const uint32_t par = it & 1;
-                    if (!(pp && e > 0)) { tc::mbar_wait(a1_full, par); tc::tc_fence_after(); }     // ping-pong: consumed before d4 of the previous evaluation
-                    if (tc::elect_one()) {
-                        issue_bf16x3(tm + cD1, Ek, W1k, 32, idesc_bf16(128, 64, 0, 0), 0);           // F1 (K = 32: the zero columns 32..63 of the tiles are skipped)
-                        tc::umma_commit(d1_full);
-                    }
-                    __syncwarp();
-                    tc::mbar_wait(a2_full, par); tc::tc_fence_after();
-                    if (tc::elect_one()) {
-                        issue_bf16x3(tm + cD2, Hk, W2k, 64, idesc_bf16(128, 64, 0, 0), 0);           // F2
-                        tc::umma_commit(d2_full);
-                    }
-                    __syncwarp();
-                    tc::mbar_wait(a3_full, par); tc::tc_fence_after();
-                    if (tc::elect_one()) {
-                        issue_bf16x3(tm + cG2, Zk, W2m, 64, idesc_bf16(128, 64, 0, 1), 0);           // G2 : dH1 = dZ2 W2
-                        issue_bf16x3(tm + cW2, Zm, Hm, 128, idesc_bf16(128, 64, 1, 1), accW);       // WG2: dW2 += dZ2^T H1
-                        tc::umma_commit(d3_full);
-                    }
-                    __syncwarp();
-                    tc::mbar_wait(a4_full, par); tc::tc_fence_after();
-                    if (tc::elect_one()) {
-                        issue_bf16x3(tm + cG1, Zk, W1m, 64, idesc_bf16(128, 32, 0, 1), 0);           // G1 : dEnc = dZ1 W1
-                        issue_bf16x3(tm + cW1, Zm, Em, 128, idesc_bf16(128, 32, 1, 1), accW);       // WG1: dW1 += dZ1^T Enc
-                    }
-                    __syncwarp();
-                    // ping-pong: E(it+1) is already there (other half).  Consuming its a1 phase BEFORE releasing d4(it) keeps the encoders,
-                    // who arrive for it+2 only after d4(it), from lapping this waiter.
-                    if (pp && e + 1 < e_end) { tc::mbar_wait(a1_full, par ^ 1u); tc::tc_fence_after(); }
-                    if (tc::elect_one()) tc::umma_commit(d4_full);
-                    __syncwarp();
-                    accW = 1;
+        // ================================ MMA warpgroup ================================
+        // two accumulators plus the resident dW2 / dW1 do not fit the 128-register share of a 512-thread CTA: take the encoders' spare ones
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 192;");
+        float* stg_w = reinterpret_cast<float*>(sm + oStg);
+        float* denc_w = reinterpret_cast<float*>(sm + oZ);
+        const int wl = warp & 3;
+        const bool pp = a.e_pingpong != 0;
+        // dW2 [64 x 64], dW1 [64 x 32] over every sample of this CTA: each evaluation's product starts a fresh accumulator and is added
+        // here in fp32 (round to nearest) -- a chain of thousands of accumulating MMAs drifts further from the fp32 sum
+        float dw2[32], dw1[16];
+        #pragma unroll
+        for (int i = 0; i < 32; i++) dw2[i] = 0.f;
+        #pragma unroll
+        for (int i = 0; i < 16; i++) dw1[i] = 0.f;
+        uint32_t su = 0;
+        auto stage = [&](const float (&d)[2][32]) {         // 64 accumulator columns, 32 at a time, to the owners
+            #pragma unroll
+            for (int c0 = 0; c0 < 64; c0 += 32) {
+                if (su > 0) tc::mbar_wait(stg_empty, (su - 1) & 1u);
+                stage_frag<32>(d, stg_w, kStgLd, c0, 32, wl, lane);
+                mbar_arrive(stg_full);
+                su++;
+            }
+        };
+        auto rows64 = [](const Operand& o, int h) { return Operand{o.base + 8192u * (uint32_t)h, o.part_stride, o.lbo}; };   // K-major A: rows 64 h ..
+        for (uint32_t tile = a.tile0 + blockIdx.x; tile < a.tile1 && (uint64_t)tile * T < m_pad; tile += gridDim.x) {
+            for (int e = 0; e < e_end; e++, it++) {
+                const uint32_t par = it & 1;
+                const uint32_t eoff = pp ? 64u * (it & 1u) : 0u;            // ping-pong E: columns 32 (it & 1) .. + 31 of the tile
+                const Operand E{sbase + oE + eoff, (uint32_t)kTile, (uint32_t)kTile}, H{sbase + oH, (uint32_t)kTile, (uint32_t)kTile};
+                const Operand Z{sbase + oZ, (uint32_t)kTile, (uint32_t)kTile};
+                const Operand W1{sbase + oW1, 8192u, 8192u}, W2{sbase + oW2, 8192u, 8192u};
+                float d[2][32];
+                if (!(pp && e > 0)) tc::mbar_wait(a1_full, par);     // ping-pong: consumed before d4 of the previous evaluation
+                mbar_arrive(d1_full);
+                wg::fence();
+                #pragma unroll
+                for (int h = 0; h < 2; h++) issue_bf16x3<64, 0, 0>(d[h], rows64(E, h), W1, 32, 0u);   // F1 (K = 32: the zero columns 32..63 are skipped)
+                wg::commit(); wg::wait<0>(); wg::reg_fence(d[0]); wg::reg_fence(d[1]);
+                stage(d);
+                tc::mbar_wait(a2_full, par);
+                wg::fence();
+                #pragma unroll
+                for (int h = 0; h < 2; h++) issue_bf16x3<64, 0, 0>(d[h], rows64(H, h), W2, 64, 0u);   // F2
+                wg::commit(); wg::wait<0>(); wg::reg_fence(d[0]); wg::reg_fence(d[1]);
+                stage(d);
+                tc::mbar_wait(a3_full, par);
+                wg::fence();
+                #pragma unroll
+                for (int h = 0; h < 2; h++) issue_bf16x3<64, 0, 1>(d[h], rows64(Z, h), W2, 64, 0u);   // G2 : dH1 = dZ2 W2
+                float t2[32];
+                issue_bf16x3<64, 1, 1>(t2, Z, H, 128, 0u);                                              // WG2: dW2 += dZ2^T H1
+                wg::commit(); wg::wait<0>(); wg::reg_fence(d[0]); wg::reg_fence(d[1]); wg::reg_fence(t2);
+                #pragma unroll
+                for (int i = 0; i < 32; i++) dw2[i] += t2[i];
+                stage(d);
+                tc::mbar_wait(a4_full, par);
+                float g1[2][16];
+                wg::fence();
+                #pragma unroll
+                for (int h = 0; h < 2; h++) issue_bf16x3<32, 0, 1>(g1[h], rows64(Z, h), W1, 64, 0u);  // G1 : dEnc = dZ1 W1
+                float t1[16];
+                issue_bf16x3<32, 1, 1>(t1, Z, E, 128, 0u);                                              // WG1: dW1 += dZ1^T Enc
+                wg::commit(); wg::wait<0>(); wg::reg_fence(g1[0]); wg::reg_fence(g1[1]); wg::reg_fence(t1);
+                #pragma unroll
+                for (int i = 0; i < 16; i++) dw1[i] += t1[i];
+                stage_frag<16>(g1, denc_w, 32, 0, 32, wl, lane);                                       // over the dZ tiles, now free
+                // ping-pong: E(it+1) is already there (other half).  Consuming its a1 phase BEFORE releasing d4(it) keeps the encoders,
+                // who arrive for it+2 only after d4(it), from lapping this waiter.
+                if (pp && e + 1 < e_end) tc::mbar_wait(a1_full, par ^ 1u);
+                mbar_arrive(d4_full);
+            }
+        }
+        // ---- flush the register-resident weight gradients: dW2 [64 x 64] and dW1 [64 x 32] (row = output feature) ----
+        if (it > 0) {
+            #pragma unroll
+            for (int hh = 0; hh < 2; hh++) {
+                const int j = 16 * wl + (lane >> 2) + 8 * hh;
+                #pragma unroll
+                for (int n8 = 0; n8 < 8; n8++) {
+                    const int c = 8 * n8 + 2 * (lane & 3);
+                    atomicAdd(a.g_mlp.w2 + j * D_H + c, dw2[4 * n8 + 2 * hh]); atomicAdd(a.g_mlp.w2 + j * D_H + c + 1, dw2[4 * n8 + 2 * hh + 1]);
+                }
+                #pragma unroll
+                for (int n8 = 0; n8 < 4; n8++) {
+                    const int c = 8 * n8 + 2 * (lane & 3);
+                    atomicAdd(a.g_mlp.w1 + j * D_IN + c, dw1[4 * n8 + 2 * hh]); atomicAdd(a.g_mlp.w1 + j * D_IN + c + 1, dw1[4 * n8 + 2 * hh + 1]);
                 }
             }
         }
     }
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::tc_fence_after();
-    // ---- flush the TMEM-resident weight gradients: rows 0..63 of dW2 [64 x 64] and dW1 [64 x 32] ----
-    if (warp < 2 && it > 0) {
-        const int j = tid;                                      // TMEM lane == output-feature index
-        const uint32_t lane_addr = tmem + ((uint32_t)(warp * 32) << 16);
-        #pragma unroll 1
-        for (int c0 = 0; c0 < D_H; c0 += 16) {
-            uint32_t v[16];
-            tmem_ld16(lane_addr + cW2 + (uint32_t)c0, v);
-            #pragma unroll
-            for (int i = 0; i < 16; i++) atomicAdd(a.g_mlp.w2 + j * D_H + c0 + i, __uint_as_float(v[i]));
-        }
-        #pragma unroll 1
-        for (int c0 = 0; c0 < D_IN; c0 += 16) {
-            uint32_t v[16];
-            tmem_ld16(lane_addr + cW1 + (uint32_t)c0, v);
-            #pragma unroll
-            for (int i = 0; i < 16; i++) atomicAdd(a.g_mlp.w1 + j * D_IN + c0 + i, __uint_as_float(v[i]));
-        }
-        tc::tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 12) { tc::tc_fence_after(); tc::tmem_dealloc(tmem, kTmemCols); }
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1785,7 +1797,7 @@ int num_sms() {
     if (g_num_sms == 0) {
         int dev = 0; cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-        if (g_num_sms <= 0) g_num_sms = 148;
+        if (g_num_sms <= 0) g_num_sms = 132;
     }
     return g_num_sms;
 }
@@ -1911,18 +1923,16 @@ int mi3d_field_backward(const mi3d_field_io* io, const float* table, const mi3d_
                 if (cached && (t0 + kBwdChunkTiles < total_tiles ? t0 + kBwdChunkTiles : total_tiles) <= io->enc_cache_tiles)
                     a.enc_buf = io->enc_cache + (size_t)t0 * 13 * T * 32;   // saved by the forward
                 else { a.enc_buf = enc_tmp; k_bwd_enc_scatter<false><<<num_sms() * 4, 512, 0, (cudaStream_t)stream>>>(a); }
-                // Where the table-gradient REDs are issued.  Measured at 128x128, M = 424 k (tools/prof_render.py, profiles/r2_scatter_ab.txt):
-                // full 13-evaluation backward 8.2 ms split vs 5.8 ms fused; 7-evaluation backward 3.7 vs 3.4; centre-only (SDS) 0.91 vs 0.89.
-                // The RED stream is LSU-issue-bound (1.29 cycles per lane), the chain is latency-bound: they overlap in one kernel.
+                // Where the table-gradient REDs are issued: the RED stream is bound by the load / store unit, the MMA / epilogue chain by
+                // its serial hand-offs, so by default they overlap in one kernel (impl = TCGEN05_SPLIT_SCATTER runs the scatter as a kernel
+                // of its own; tools/prof_render.py --impl times both arms).
                 const bool fuse = cfg->impl != MI3D_FIELD_IMPL_TCGEN05_SPLIT_SCATTER;
                 // Which levels' REDs are warp-aggregated inside the chain kernel.  The scans cost issue slots next to the owner warps, the REDs
                 // they remove are the ones that serialise in L2 (the benchmark scene concentrates every sample in a sphere of radius 0.2:
-                // ~2 k occupied cells at level 5).  Measured, M = 424 k, full backward (tools/prof_render.py --agg): no aggregation 11.7 ms;
-                // round-2a kernel: 25 -> 6.74, 50 -> 5.36, 60 -> 5.29, 120 -> 5.56, 200 -> 5.79; with the elected-lane MMA issue, packed
-                // splits and both scatter halves sharing the coarse levels: 25 -> 6.44, 50 -> 5.02, 100 -> 4.81, 200 -> 4.93.
+                // ~2 k occupied cells at level 5).  The threshold is cfg->scatter_agg_scale (default 100); tools/prof_render.py --agg times it.
                 a.agg_scale_max = cfg->scatter_agg_scale > 0.f ? cfg->scatter_agg_scale : 100.f;
                 if (fuse) {
-                    // the chain kernel's encoder warps scatter d(enc) themselves, straight from TMEM: the RED stream (LSU-bound) runs
+                    // the chain kernel's encoder warps scatter d(enc) themselves, from shared memory: the RED stream (LSU-bound) runs
                     // under the MMA / epilogue chain (latency-bound) of the next evaluation instead of in a kernel of its own
                     float* const denc = a.denc_buf;
                     a.denc_buf = nullptr;

@@ -1,4 +1,4 @@
-// mi3d_common.cuh -- shared helpers for the sm_100a kernels behind include/mi3d.h
+// mi3d_common.cuh -- shared helpers for the sm_90a kernels behind include/mi3d.h
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

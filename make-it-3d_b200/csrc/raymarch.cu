@@ -1,10 +1,10 @@
-// raymarch.cu -- occupancy-grid ray marching + alpha compositing for sm_100a (C ABI: include/mi3d.h)
+// raymarch.cu -- occupancy-grid ray marching + alpha compositing for sm_90a (C ABI: include/mi3d.h)
 //
 // Replaces raymarching/src/raymarching.cu of the reference (file:line cited per entry point in
 // include/mi3d.h).  Compiled with -fmad=false so that every fp32 op is a single IEEE rounding and the
 // marched sample positions are bit-identical to the CPU oracle (oracle/raymarch_oracle.c).
 //
-// B200 notes: these kernels are launch-latency sized (N = 16k..65k rays); the design goal is *zero host
+// Notes: these kernels are launch-latency sized (N = 16k..65k rays); the design goal is *zero host
 // synchronisation and zero fill traffic*:
 //   * march_train is ONE kernel: count pass -> block scan -> decoupled look-back across CTAs (ticketed
 //     block ids, so a CTA only ever waits on CTAs that already started) -> emit pass.  Compaction order is

@@ -2,7 +2,7 @@
 //
 //   mi3d_render_forward : [ray generation ->] near/far -> occupancy march -> fused field (hash grid + MLP + normals + shading +
 //                         regulariser sums) -> composite + background / depth epilogue           (SURVEY.md 8b "mi3d_render_fwd")
-//   mi3d_render_backward: composite backward -> fused field backward (gather | tcgen05 chain | RED scatter), accumulating into
+//   mi3d_render_backward: composite backward -> fused field backward (gather | wgmma chain | RED scatter), accumulating into
 //                         grad_table / grad_mlp                                                    (SURVEY.md 8b "mi3d_render_bwd")
 // A non-Python host gets the whole fused path from these two entry points; nerf/field_ops.py uses them too.  Everything they
 // launch is the same kernels the unfused B1 / B2 entry points expose (raymarch.cu, field.cu): this file only sequences them,

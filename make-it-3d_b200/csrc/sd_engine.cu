@@ -2,7 +2,7 @@
 //
 // Replaces what nerf/sd.py:117-174,212-220 runs inside diffusers (UNet2DConditionModel, AutoencoderKL.encode,
 // DDIMScheduler.add_noise) with a statically planned list of launches over ONE tensor-core tile kernel
-// (tc_gemm.cuh: tcgen05.mma / TMEM / TMA) plus the memory-bound kernels of sd_kernels.cuh:
+// (tc_gemm.cuh: wgmma / TMA) plus the memory-bound kernels of sd_kernels.cuh:
 //   * every Linear, 1x1 conv, attention product and im2col'ed strided conv   -> tc plain GEMM
 //   * every 3x3 stride-1 conv (U-Net ResBlocks, VAE encoder, their dgrads)   -> tc implicit GEMM (TMA-shifted taps)
 //   * GroupNorm(+SiLU), LayerNorm, softmax, GEGLU (GEMM epilogue), time-embedding, CFG + SDS gradient -> sdk kernels
@@ -46,7 +46,7 @@ struct Param {
 struct Engine {
     mi3d_unet_cfg ucfg; mi3d_vae_cfg vcfg;
     uint8_t* base = nullptr; size_t cap = 0, off = 0; bool dry = true; int err = 0;
-    int num_sms = 148;
+    int num_sms = 132;
     std::vector<Param> params; std::map<std::string, int> pindex;
     std::vector<Op> unet_ops, enc_ops, enc_bwd_ops;
     std::vector<Op>* cur = nullptr;
@@ -197,7 +197,7 @@ struct Engine {
         const int HW = x.h * x.w, C = x.c, G = g.G, N = x.n;
         const int VPP = C / 8, PL = std::max(1, 256 / VPP), threads = PL * VPP;
         if (G > 64 || threads > 1024 || C % 8) { err = MI3D_ERR_ARG; return g; }
-        // enough CTAs to fill the machine twice, at least PL*8 pixels each (8 CTAs per SM measured slower: more partial-sum atomics)
+        // enough CTAs to fill the machine twice, at least PL*8 pixels each (more CTAs would only add partial sums to fold)
         int chunks = std::max(1, std::min((HW + PL * 8 - 1) / (PL * 8), (2 * num_sms + N - 1) / N));
         const int ppc = (HW + chunks - 1) / chunks; chunks = (HW + ppc - 1) / ppc;
         const __half* xp = x.p; __half* yp = y.p; const GN gg = g;
@@ -248,7 +248,7 @@ struct Engine {
             return (int)cudaGetLastError();
         });
     }
-    static int blocks_for(size_t n) { return (int)std::min<size_t>((n + 255) / 256, 148 * 16); }
+    static int blocks_for(size_t n) { return (int)std::min<size_t>((n + 255) / 256, 132 * 16); }
     // persistent grids of the small direct convolutions: as many CTAs per SM as their weight staging area allows
     int small_cin_grid(size_t outputs, size_t smem) const { const int per_sm = (int)std::max<size_t>(1, std::min<size_t>(8, (200 * 1024) / std::max<size_t>(smem, 1))); return (int)std::min<size_t>((outputs / 8 + 255) / 256, (size_t)num_sms * per_sm); }
     int small_cout_grid(size_t pixels, int cin) const { const int ppw = cin <= 128 ? 2 : 1; return (int)std::min<size_t>((pixels / ppw + 7) / 8 + 1, (size_t)num_sms * 8); }
@@ -853,8 +853,7 @@ struct Engine {
         return MI3D_OK;
     }
     // The launch lists are static (fixed pointers, shapes and order; the timestep and every input live in device buffers), so a list
-    // replays as ONE CUDA graph from its third call on (~200-330 launches lose their CPU launch cost and inter-kernel gaps; measured
-    // U-Net pass 7.68 -> 6.67 ms, VAE encode 2.89 -> 2.73 ms, VAE backward 3.55 -> 3.37 ms).  Enabled per engine with
+    // replays as ONE CUDA graph from its third call on (~200-330 launches lose their CPU launch cost and inter-kernel gaps).  Enabled per engine with
     // mi3d_sd_set_graph_replay(); needs a capturable stream (torch's legacy default stream is not: nerf/sd.py runs the engine on its
     // own stream, event-ordered against the caller's).  A list whose capture fails falls back to plain launches for good.
     struct ListGraph { cudaGraphExec_t exec = nullptr; int calls = 0; bool failed = false; };

@@ -74,8 +74,8 @@ __device__ __forceinline__ void gn_group_consts(const double* __restrict__ stats
 }
 
 // Fold the per-thread partial sums sm[PL][C][2] of one CTA into its (group) totals and add them to out[G][2], in a FIXED order (run-to-run
-// deterministic): thread (g, q) first sums the group's channels of pixel lane q, then thread g sums the PL lanes.  (One thread per group
-// walking all cpg x PL slots serially was ~45 % of these kernels' duration on the U-Net shapes: ncu source view, F2F.F64 / DADD chain.)
+// deterministic): thread (g, q) first sums the group's channels of pixel lane q, then thread g sums the PL lanes (one thread per group
+// walking all cpg x PL slots serially would be a long dependent chain of double-precision adds).
 // Dynamic shared memory: 2 * PL * C floats + 2 * G * PL doubles (gn_smem_bytes).
 __device__ __forceinline__ void gn_fold(const float* sm, int C, int G, int cpg, int PL, double* __restrict__ out) {
     double* part = reinterpret_cast<double*>(const_cast<float*>(sm) + (((size_t)2 * PL * C + 1) & ~(size_t)1));
@@ -104,8 +104,8 @@ __global__ void k_gn_stats(const __half* __restrict__ x, int HW, int C, int G, i
     for (int k = 0; k < 8; k++) { s[k] = 0.f; ss[k] = 0.f; }
     if (pl < PL) {
         const __half* base = x + ((size_t)n * HW) * C + (size_t)cv * 8;
-        // 4 independent 16-byte loads in flight per thread: with 2 CTAs x 8 warps per SM a single load per iteration left the
-        // kernel latency-bound at ~1.5 TB/s (Little's law); the pixel order of the sums is unchanged (still deterministic)
+        // 4 independent 16-byte loads in flight per thread: with 2 CTAs x 8 warps per SM a single load per iteration leaves the
+        // kernel latency-bound (Little's law); the pixel order of the sums is unchanged (still deterministic)
         int p = p0 + pl;
         for (; p + 3 * PL < p1; p += 4 * PL) {
             uint4 raw[4];

@@ -1,10 +1,10 @@
 // tc_gemm.cuh -- the one tensor-core tile kernel behind every dense contraction of the SD guidance path
 // (nerf/sd.py:117-174: U-Net convs / linears / attention products, VAE encoder forward and input-gradient).
 //
-// sm_100a only: operands are staged by TMA (cp.async.bulk.tensor, 128B swizzle) into a multi-stage shared-memory
-// ring, multiplied by tcgen05.mma (cta_group::1, kind::f16, M=128 x N=BLOCK_N x K=16 per instruction, one elected
-// thread issues) into an fp32 accumulator that lives in TMEM, and read back with tcgen05.ld by four epilogue warps
-// that fuse bias / time-embedding / residual / GEGLU / transposed-store before writing fp16 (or fp32) to HBM.
+// sm_90a: operands are staged by TMA (cp.async.bulk.tensor, 128B swizzle) into a multi-stage shared-memory ring and multiplied by
+// wgmma.mma_async (fp16 in, fp32 accumulate in registers) by two consumer warpgroups, each owning 64 rows of the 128-row tile; the
+// same warpgroups run the epilogue straight from their accumulator registers (bias / time-embedding / residual / GEGLU /
+// transposed store) and write fp16 (or fp32) to HBM.
 //
 //   D[m, n] = sum_k A[m, k] * B[n, k]         A, B both K-major (K contiguous), fp16 in, fp32 accumulate
 //
@@ -14,20 +14,20 @@
 //           map, the K loop runs over 9 taps x C/64 channel blocks, each stage is ONE 4-D TMA box shifted by the tap
 //           offset; out-of-bounds rows/columns are zero-filled by the TMA unit (that is the padding).
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer, warps 2..5 = epilogue
-// (warp w owns TMEM lanes 32*(w%4) .. +31, i.e. accumulator rows).
+// Warp roles (384 threads): warp 0 = TMA producer (warps 1..3 idle), warpgroups 1 and 2 = MMA + epilogue for tile rows 0..63 / 64..127.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "wgmma.cuh"
 
 namespace tc {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;          // 64 fp16 = 128 B = one swizzle-128B atom row
-constexpr int UMMA_K = 16;
-constexpr int kThreads = 192;
+constexpr int MMA_K = 16;
+constexpr int kThreads = 384;
 
 enum EpiMode : int { EPI_PLAIN = 0, EPI_GEGLU = 1, EPI_TRANSPOSED = 2 };
 
@@ -98,94 +98,36 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
 // One lane of a converged warp (the lowest): callers keep the whole warp on the (warp-uniform) control path and predicate only the
-// tcgen05 issue on it -- with `if (lane == 0)` the compiler cannot prove that a single lane is active and wraps EVERY tcgen05.mma in a
-// uniform-register "waterfall" loop (ELECT / R2UR.BROADCAST / BRA.U.ANY, ~12 SASS instructions and ~60 cycles per MMA).
+// TMA issue on it.
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
     return pred != 0;
 }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// issue only (no wait): lets the next chunk's TMEM read overlap the arithmetic / stores of the current one
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major, 128B-swizzled operand tile descriptor (cute::UMMA::SmemDescriptor layout, version 1):
-//   start_address[0,14) = addr >> 4 ; LBO[16,30) = 1 ; SBO[32,46) = 1024 >> 4 (8 rows x 128 B) ; version[46,48) = 1 ;
-//   layout_type[61,64) = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-// cute::UMMA::InstrDescriptor: c_format F32 (1) @4, a/b format F16 (0) @7/@10, K-major A and B, N>>3 @17, M>>4 @24
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N, int b_mn = 0) {
-    return (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)b_mn << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// MN-major 128B-swizzle descriptor: LBO = byte distance between 64-element MN blocks, SBO = 1024 B (8 K-rows)
-__device__ __forceinline__ uint64_t make_sw128_desc_mn(uint32_t smem_addr, uint32_t lbo_bytes) {
-    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-
 template <int BLOCK_N> struct Cfg {
-    static constexpr int kStages = BLOCK_N == 256 ? 4 : (BLOCK_N == 128 ? 6 : 4);   // BN=64: 96 KB -> 2 CTAs/SM ; BN=160: 4 x 36 KB
+    static constexpr int kStages = BLOCK_N == 256 ? 4 : (BLOCK_N == 128 ? 6 : (BLOCK_N == 160 ? 5 : 4));   // BN=64: 96 KB -> 2 CTAs/SM
     static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;
     static constexpr int kBBytes = BLOCK_N * BLOCK_K * 2;
     static constexpr int kStageBytes = kABytes + kBBytes;
-    // two accumulator stages (epilogue(i) overlaps mainloop(i+1)); allocations are powers of two
-    static constexpr int kTmemCols = 2 * BLOCK_N <= 128 ? 128 : (2 * BLOCK_N <= 256 ? 256 : 512);
-    static constexpr size_t kSmemBytes = 1024 /*align slack*/ + (size_t)kStages * kStageBytes + 512;
+    static constexpr size_t kSmemBytes = 1024 /*align slack*/ + (size_t)kStages * kStageBytes + 256;
+    static constexpr int kMinBlocks = BLOCK_N == 64 ? 2 : 1;
 };
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
 
+// acc (+)= A[64 x 16] . B[BLOCK_N x 16]^T ; TB = 1: B is MN-major
+template <int BLOCK_N, int TB>
+__device__ __forceinline__ void mma_tile(float (&acc)[BLOCK_N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
+    if constexpr (BLOCK_N == 64) wg::wgmma_f16_n64<0, TB>(acc, da, db, accumulate);
+    else if constexpr (BLOCK_N == 128) wg::wgmma_f16_n128<0, TB>(acc, da, db, accumulate);
+    else if constexpr (BLOCK_N == 160) wg::wgmma_f16_n160<0, TB>(acc, da, db, accumulate);
+    else wg::wgmma_f16_n256<0, TB>(acc, da, db, accumulate);
+}
+
 template <int BLOCK_N>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kThreads, Cfg<BLOCK_N>::kMinBlocks)
 k_tc_gemm(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmParams p) {
     using C = Cfg<BLOCK_N>;
     extern __shared__ uint8_t smem_raw[];
@@ -193,216 +135,133 @@ k_tc_gemm(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
     uint8_t* tiles = smem;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)C::kStages * C::kStageBytes);
     uint64_t* empty_bar = full_bar + C::kStages;
-    uint64_t* tmem_full_bar = empty_bar + C::kStages;            // [2]
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;                // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (warp == 0 && lane == 0) {
         prefetch_tmap(&map_a); prefetch_tmap(&map_b);
-        for (int s = 0; s < C::kStages; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        for (int s = 0; s < 2; s++) { mbar_init(&tmem_full_bar[s], 1); mbar_init(&tmem_empty_bar[s], 4); }
+        for (int s = 0; s < C::kStages; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }   // empty: one arrive per consumer warp
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, C::kTmemCols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     if (warp == 0) {
         // ===================== TMA producer =====================
         // whole warp on the (uniform) loop and the barrier waits, one elected lane issues: see elect_one()
-        {
-            int stage = 0; uint32_t phase = 0;
-            for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x) {
-                const int sp = t % p.splits, tt = t / p.splits;
-                const int n_blk = tt % p.n_tiles, rest = tt / p.n_tiles, m_blk = rest % p.m_tiles, z = rest / p.m_tiles;
-                const int kb0 = sp * p.kb_per_split, kb1 = min(p.num_k_blocks, kb0 + p.kb_per_split);
-                const int m0 = m_blk * BLOCK_M, n0 = n_blk * BLOCK_N;
-                int cw = 0, ch = 0, cn = 0;
-                if (p.conv) {
-                    const int hw = p.conv_H * p.conv_W;
-                    cn = m0 / hw; const int rem = m0 - cn * hw;
-                    ch = rem / p.conv_W; cw = rem - ch * p.conv_W;
-                }
-                const int az0 = p.a_z1 > 0 ? z % p.a_z1 : 0, az1 = p.a_z1 > 0 ? z / p.a_z1 : 0;
-                const int bz0 = p.b_batched ? (p.b_z1 > 0 ? z % p.b_z1 : 0) : 0, bz1 = p.b_batched ? (p.b_z1 > 0 ? z / p.b_z1 : 0) : 0;
-                for (int kb = kb0; kb < kb1; kb++) {
-                    mbar_wait(&empty_bar[stage], phase ^ 1);
-                    uint8_t* sa = tiles + (size_t)stage * C::kStageBytes;
-                    uint8_t* sb = sa + C::kABytes;
-                    int c0 = kb * BLOCK_K, c1 = m0, c2 = az0, c3 = az1;
-                    if (p.conv) {
-                        const int tap = kb / p.cin_blocks, cc = kb - tap * p.cin_blocks;
-                        const int ky = tap / 3, kx = tap - ky * 3;
-                        c0 = cc * BLOCK_K; c1 = cw + kx - 1; c2 = ch + ky - 1; c3 = cn;
-                    }
-                    if (elect_one()) {
-                        mbar_arrive_expect_tx(&full_bar[stage], C::kStageBytes);
-                        tma_load_4d(&map_a, &full_bar[stage], sa, c0, c1, c2, c3);
-                        if (p.b_mn) {
-                            #pragma unroll
-                            for (int nb = 0; nb < BLOCK_N / 64; nb++) tma_load_4d(&map_b, &full_bar[stage], sb + nb * 8192, n0 + nb * 64, kb * BLOCK_K, 0, 0);
-                        } else
-                        tma_load_4d(&map_b, &full_bar[stage], sb, kb * BLOCK_K, n0, bz0, bz1);
-                    }
-                    __syncwarp();
-                    if (++stage == C::kStages) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        // whole warp on the (uniform) loop and the barrier waits, one elected lane issues: see elect_one()
-        {
-            const uint32_t idesc = make_idesc_f16(BLOCK_M, BLOCK_N, p.b_mn);
-            const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0), tiles_u = __shfl_sync(0xffffffffu, smem_u32(tiles), 0);
-            int stage = 0; uint32_t phase = 0;
-            int it = 0;
-            for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x, it++) {
-                const int as = it & 1;
-                mbar_wait(&tmem_empty_bar[as], ((uint32_t)(it >> 1) & 1u) ^ 1u);     // epilogue drained this accumulator stage
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_u + (uint32_t)(as * BLOCK_N);
-                const int sp = t % p.splits;
-                const int kb0 = sp * p.kb_per_split, kb1 = min(p.num_k_blocks, kb0 + p.kb_per_split);
-                for (int kb = kb0; kb < kb1; kb++) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    if (elect_one()) {
-                        const uint32_t sa = tiles_u + (uint32_t)stage * (uint32_t)C::kStageBytes;
-                        const uint64_t da = make_sw128_desc(sa), db = p.b_mn ? make_sw128_desc_mn(sa + C::kABytes, 8192u) : make_sw128_desc(sa + C::kABytes);
-                        #pragma unroll
-                        for (int k = 0; k < BLOCK_K / UMMA_K; k++) {
-                            // advancing K inside the 128B swizzle atom = +32 B on the start address (>>4 => +2);
-                            // MN-major B: K runs over rows, 16 rows = 2048 B (>>4 => +128)
-                            umma_f16(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(p.b_mn ? 128 * k : 2 * k), idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-                        }
-                        umma_commit(&empty_bar[stage]);            // frees the smem stage when these MMAs retire
-                        if (kb + 1 == kb1) umma_commit(&tmem_full_bar[as]);               // accumulator complete
-                    }
-                    __syncwarp();
-                    if (++stage == C::kStages) { stage = 0; phase ^= 1; }
-                }
-                if (kb1 <= kb0) {                                   // empty K-range (the split-K planner never produces one): still release the epilogue
-                    if (elect_one()) umma_commit(&tmem_full_bar[as]);
-                    __syncwarp();
-                }
-            }
-        }
-    } else {
-        // ===================== epilogue: TMEM -> registers -> HBM =====================
-        const int quarter = warp & 3;                      // TMEM lane quarter this warp may access
-        const int row = quarter * 32 + lane;               // accumulator row == tile row
-        int it = 0;
-        for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x, it++) {
-            const int tt = t / p.splits;
+        int stage = 0; uint32_t phase = 0;
+        for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x) {
+            const int sp = t % p.splits, tt = t / p.splits;
             const int n_blk = tt % p.n_tiles, rest = tt / p.n_tiles, m_blk = rest % p.m_tiles, z = rest / p.m_tiles;
-            const int as = it & 1;
-            mbar_wait(&tmem_full_bar[as], (uint32_t)(it >> 1) & 1u);
-            tc_fence_after();
-            const int m = m_blk * BLOCK_M + row;
-            const bool row_ok = m < p.m_valid;
-            const size_t zoff = (size_t)(z % p.out_z1) * p.out_s_lo + (size_t)(z / p.out_z1) * p.out_s_hi;
-            const float* rb = (p.row_bias && row_ok) ? p.row_bias + (size_t)(((long long)z * p.M + m) / p.rows_per_group) * p.N : nullptr;
-            const uint32_t t_acc = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(as * BLOCK_N);
-            // one 32-column chunk: registers -> (alpha, bias, row bias, residual / GEGLU) -> global.  v is consumed before the call returns.
-            auto chunk = [&](const uint32_t (&v)[32], const int c0) {
-                const int n0 = n_blk * BLOCK_N + c0;
-                if (p.splits > 1) {
-                    // split-K partial: fp32 RED (16 bytes each) into the workspace; bias / residual / conversion happen in k_splitk_finish
-                    if (row_ok) {
-                        float4* wsp = reinterpret_cast<float4*>(p.splitk_ws + (size_t)m * p.N + n0);
-                        #pragma unroll
-                        for (int q = 0; q < 8; q++)
-                            atomicAdd(wsp + q, make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]), __uint_as_float(v[4 * q + 3])));
-                    }
-                    return;
-                }
-                float f[32];
-                #pragma unroll
-                for (int i = 0; i < 32; i++) f[i] = __uint_as_float(v[i]) * p.alpha;
-                if (p.bias) {          // 16-byte loads (launch() checks the alignment): 8 instead of 32 load + address instructions per chunk
-                    #pragma unroll
-                    for (int q = 0; q < 8; q++) {
-                        const float4 bv = __ldg(reinterpret_cast<const float4*>(p.bias + n0) + q);
-                        f[4 * q] += bv.x; f[4 * q + 1] += bv.y; f[4 * q + 2] += bv.z; f[4 * q + 3] += bv.w;
-                    }
-                }
-                if (rb) {
-                    #pragma unroll
-                    for (int q = 0; q < 8; q++) {
-                        const float4 bv = __ldg(reinterpret_cast<const float4*>(rb + n0) + q);
-                        f[4 * q] += bv.x; f[4 * q + 1] += bv.y; f[4 * q + 2] += bv.z; f[4 * q + 3] += bv.w;
-                    }
-                }
-                if (!row_ok) return;
-                if (p.epi_mode == EPI_GEGLU) {
-                    // weight rows were interleaved (value, gate) at plan time: out[:, n/2] = value * gelu(gate)
-                    __half* o = p.out + zoff + (size_t)m * p.ldc + (n0 >> 1);
-                    __align__(16) __half h[16];
-                    #pragma unroll
-                    for (int i = 0; i < 16; i++) h[i] = __float2half_rn(f[2 * i] * gelu_erf(f[2 * i + 1]));
-                    *reinterpret_cast<uint4*>(o) = *reinterpret_cast<const uint4*>(h);
-                    *reinterpret_cast<uint4*>(o + 8) = *reinterpret_cast<const uint4*>(h + 8);
-                } else if (p.epi_mode == EPI_TRANSPOSED) {
-                    // out[z][n][m]: lanes hold consecutive m -> each store instruction writes 64 contiguous bytes per n
-                    __half* o = p.out + zoff + (size_t)n0 * p.ldc + m;
-                    #pragma unroll
-                    for (int i = 0; i < 32; i++) o[(size_t)i * p.ldc] = __float2half_rn(f[i]);
-                } else {
-                    if (p.residual) {
-                        const __half* r = p.residual + zoff + (size_t)m * p.ld_res + n0;
-                        #pragma unroll
-                        for (int q = 0; q < 4; q++) {
-                            const uint4 rv = __ldg(reinterpret_cast<const uint4*>(r) + q);
-                            const __half* rh = reinterpret_cast<const __half*>(&rv);
-                            #pragma unroll
-                            for (int i = 0; i < 8; i++) f[8 * q + i] += __half2float(rh[i]);
-                        }
-                    }
-                    if (p.out_f32) {
-                        float* o = p.out_f32 + zoff + (size_t)m * p.ldc + n0;
-                        #pragma unroll
-                        for (int q = 0; q < 8; q++) reinterpret_cast<float4*>(o)[q] = make_float4(f[4 * q], f[4 * q + 1], f[4 * q + 2], f[4 * q + 3]);
-                    } else {
-                        __half* o = p.out + zoff + (size_t)m * p.ldc + n0;
-                        __align__(16) __half h[32];
-                        #pragma unroll
-                        for (int i = 0; i < 32; i++) h[i] = __float2half_rn(f[i]);
-                        #pragma unroll
-                        for (int q = 0; q < 4; q++) reinterpret_cast<uint4*>(o)[q] = reinterpret_cast<const uint4*>(h)[q];
-                    }
-                }
-            };
-            // software pipeline over the chunks: the TMEM read of chunk c+1 is in flight while chunk c is converted and stored
-            constexpr int NC = BLOCK_N / 32;
-            uint32_t va[32], vb[32];
-            tmem_ld32_issue(t_acc, va);
-            #pragma unroll 1
-            for (int c = 0; c < NC; c += 2) {
-                tmem_ld_wait();
-                if (c + 1 < NC) tmem_ld32_issue(t_acc + (uint32_t)((c + 1) * 32), vb);
-                chunk(va, c * 32);
-                if (c + 1 < NC) {
-                    tmem_ld_wait();
-                    if (c + 2 < NC) tmem_ld32_issue(t_acc + (uint32_t)((c + 2) * 32), va);
-                    chunk(vb, (c + 1) * 32);
-                }
+            const int kb0 = sp * p.kb_per_split, kb1 = min(p.num_k_blocks, kb0 + p.kb_per_split);
+            const int m0 = m_blk * BLOCK_M, n0 = n_blk * BLOCK_N;
+            int cw = 0, ch = 0, cn = 0;
+            if (p.conv) {
+                const int hw = p.conv_H * p.conv_W;
+                cn = m0 / hw; const int rem = m0 - cn * hw;
+                ch = rem / p.conv_W; cw = rem - ch * p.conv_W;
             }
-            // release this accumulator stage to the MMA warp (one arrive per epilogue warp)
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&tmem_empty_bar[as])) : "memory");
+            const int az0 = p.a_z1 > 0 ? z % p.a_z1 : 0, az1 = p.a_z1 > 0 ? z / p.a_z1 : 0;
+            const int bz0 = p.b_batched ? (p.b_z1 > 0 ? z % p.b_z1 : 0) : 0, bz1 = p.b_batched ? (p.b_z1 > 0 ? z / p.b_z1 : 0) : 0;
+            for (int kb = kb0; kb < kb1; kb++) {
+                mbar_wait(&empty_bar[stage], phase ^ 1);
+                uint8_t* sa = tiles + (size_t)stage * C::kStageBytes;
+                uint8_t* sb = sa + C::kABytes;
+                int c0 = kb * BLOCK_K, c1 = m0, c2 = az0, c3 = az1;
+                if (p.conv) {
+                    const int tap = kb / p.cin_blocks, cc = kb - tap * p.cin_blocks;
+                    const int ky = tap / 3, kx = tap - ky * 3;
+                    c0 = cc * BLOCK_K; c1 = cw + kx - 1; c2 = ch + ky - 1; c3 = cn;
+                }
+                if (elect_one()) {
+                    mbar_arrive_expect_tx(&full_bar[stage], C::kStageBytes);
+                    tma_load_4d(&map_a, &full_bar[stage], sa, c0, c1, c2, c3);
+                    if (p.b_mn) {
+                        #pragma unroll
+                        for (int nb = 0; nb < BLOCK_N / 64; nb++) tma_load_4d(&map_b, &full_bar[stage], sb + nb * 8192, n0 + nb * 64, kb * BLOCK_K, 0, 0);
+                    } else
+                    tma_load_4d(&map_b, &full_bar[stage], sb, kb * BLOCK_K, n0, bz0, bz1);
+                }
+                __syncwarp();
+                if (++stage == C::kStages) { stage = 0; phase ^= 1; }
+            }
+        }
+    } else if (warp >= 4) {
+        // ===================== MMA + epilogue: warpgroup g owns tile rows 64 g .. 64 g + 63 =====================
+        const int g = (warp >> 2) - 1, wl = warp & 3;
+        const uint32_t tiles_u = smem_u32(tiles);
+        int stage = 0; uint32_t phase = 0;
+        float acc[BLOCK_N / 2];
+        for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x) {
+            const int sp = t % p.splits, tt = t / p.splits;
+            const int n_blk = tt % p.n_tiles, rest = tt / p.n_tiles, m_blk = rest % p.m_tiles, z = rest / p.m_tiles;
+            const int kb0 = sp * p.kb_per_split, kb1 = min(p.num_k_blocks, kb0 + p.kb_per_split);
+            #pragma unroll
+            for (int i = 0; i < BLOCK_N / 2; i++) acc[i] = 0.f;          // an empty K-range (never planned) still stores zeros
+            int prev = -1;
+            for (int kb = kb0; kb < kb1; kb++) {
+                mbar_wait(&full_bar[stage], phase);
+                const uint32_t sa = tiles_u + (uint32_t)stage * (uint32_t)C::kStageBytes;
+                const uint64_t da = wg::desc_sw128(sa + (uint32_t)g * 8192u);            // 64 rows x 128 B further down the A tile
+                wg::fence();
+                if (p.b_mn) {
+                    const uint64_t db = wg::desc_sw128(sa + C::kABytes, 8192u);
+                    #pragma unroll
+                    for (int k = 0; k < BLOCK_K / MMA_K; k++)                              // MN-major B: 16 K-rows = 2048 B (>>4 => +128)
+                        mma_tile<BLOCK_N, 1>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(128 * k), (kb > kb0 || k > 0) ? 1u : 0u);
+                } else {
+                    const uint64_t db = wg::desc_sw128(sa + C::kABytes);
+                    #pragma unroll
+                    for (int k = 0; k < BLOCK_K / MMA_K; k++)                              // +32 B inside the swizzle row (>>4 => +2)
+                        mma_tile<BLOCK_N, 0>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb > kb0 || k > 0) ? 1u : 0u);
+                }
+                wg::commit();
+                wg::wait<1>();                                   // the previous stage's MMAs have retired: hand its buffers back
+                if (prev >= 0 && lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&empty_bar[prev])) : "memory");
+                prev = stage;
+                if (++stage == C::kStages) { stage = 0; phase ^= 1; }
+            }
+            wg::wait<0>();
+            wg::reg_fence(acc);
+            if (prev >= 0 && lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&empty_bar[prev])) : "memory");
+
+            // epilogue: this thread holds rows r0 and r0 + 8, columns 8 j + 2 (lane % 4) + {0, 1}
+            const size_t zoff = (size_t)(z % p.out_z1) * p.out_s_lo + (size_t)(z / p.out_z1) * p.out_s_hi;
+            #pragma unroll
+            for (int hh = 0; hh < 2; hh++) {
+                const int m = m_blk * BLOCK_M + g * 64 + wl * 16 + (lane >> 2) + 8 * hh;
+                const bool row_ok = m < p.m_valid;
+                if (!row_ok) continue;
+                const float* rb = p.row_bias ? p.row_bias + (size_t)(((long long)z * p.M + m) / p.rows_per_group) * p.N : nullptr;
+                #pragma unroll
+                for (int j = 0; j < BLOCK_N / 8; j++) {
+                    const int n = n_blk * BLOCK_N + 8 * j + 2 * (lane & 3);
+                    float f0 = acc[4 * j + 2 * hh], f1 = acc[4 * j + 2 * hh + 1];
+                    if (p.splits > 1) {
+                        // split-K partial: fp32 RED into the workspace; bias / residual / conversion happen in k_splitk_finish
+                        atomicAdd(reinterpret_cast<float2*>(p.splitk_ws + (size_t)m * p.N + n), make_float2(f0, f1));
+                        continue;
+                    }
+                    f0 *= p.alpha; f1 *= p.alpha;
+                    if (p.bias) { const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + n)); f0 += bv.x; f1 += bv.y; }
+                    if (rb) { const float2 bv = __ldg(reinterpret_cast<const float2*>(rb + n)); f0 += bv.x; f1 += bv.y; }
+                    if (p.epi_mode == EPI_GEGLU) {
+                        // weight rows were interleaved (value, gate) at plan time: out[:, n/2] = value * gelu(gate)
+                        p.out[zoff + (size_t)m * p.ldc + (n >> 1)] = __float2half_rn(f0 * gelu_erf(f1));
+                    } else if (p.epi_mode == EPI_TRANSPOSED) {
+                        __half* o = p.out + zoff + (size_t)n * p.ldc + m;
+                        o[0] = __float2half_rn(f0); o[p.ldc] = __float2half_rn(f1);
+                    } else {
+                        if (p.residual) {
+                            const __half2 rv = *reinterpret_cast<const __half2*>(p.residual + zoff + (size_t)m * p.ld_res + n);
+                            f0 += __low2float(rv); f1 += __high2float(rv);
+                        }
+                        if (p.out_f32) *reinterpret_cast<float2*>(p.out_f32 + zoff + (size_t)m * p.ldc + n) = make_float2(f0, f1);
+                        else *reinterpret_cast<__half2*>(p.out + zoff + (size_t)m * p.ldc + n) = __floats2half2_rn(f0, f1);
+                    }
+                }
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, C::kTmemCols); }
 }
 
 // split-K epilogue: out = alpha * ws + bias + row_bias (+ residual) -> fp16 ; 8 elements per thread

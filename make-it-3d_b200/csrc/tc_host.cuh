@@ -74,7 +74,7 @@ inline int launch_bn(const CUtensorMap& ma, const CUtensorMap& mb, const GemmPar
     if (q.splits <= 1) { q.splits = 1; q.kb_per_split = q.num_k_blocks; }
     q.num_tiles = q.m_tiles * q.n_tiles * batch * q.splits;
     static int sms = 0;
-    if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 148; }
+    if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
     const int resident = (Cfg<BN>::kSmemBytes <= 110 * 1024) ? 2 : 1;       // persistent grid: one (or two) CTAs per SM loop over the tiles
     const int grid = q.num_tiles < sms * resident ? q.num_tiles : sms * resident;
     k_tc_gemm<BN><<<grid, kThreads, Cfg<BN>::kSmemBytes, st>>>(ma, mb, q);
@@ -83,6 +83,7 @@ inline int launch_bn(const CUtensorMap& ma, const CUtensorMap& mb, const GemmPar
 
 inline int launch(const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams& p, int block_n, int batch, cudaStream_t st) {
     if (p.K % BLOCK_K || p.N % block_n || p.out_z1 < 1) return MI3D_ERR_ARG;
+    if (p.b_mn && block_n % 64) return MI3D_ERR_ARG;                                   // MN-major B is loaded in 64-column boxes
     if (((uintptr_t)p.bias | (uintptr_t)p.row_bias | (uintptr_t)p.splitk_ws) & 15) return MI3D_ERR_ARG;     // read / RED-added 16 bytes at a time
     switch (block_n) {
         case 64: return launch_bn<64>(ma, mb, p, batch, st);
@@ -96,7 +97,7 @@ inline int launch(const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams
 // Split-K for the deep U-Net / VAE levels (M = 128 .. 512 rows): a handful of output tiles with K = 3 000 .. 23 000 would otherwise
 // run on a handful of SMs.  ws: fp32 [M][N] scratch (zeroed here).  Only plain fp16-output GEMMs / convs with batch == 1.
 inline int plan_splits(long long tiles, int num_k_blocks, int num_sms) {
-    if (tiles * 2 > num_sms || num_k_blocks < 48) return 1;      // the zero-fill + finish passes cost ~10 us: only deep K pays
+    if (tiles * 2 > num_sms || num_k_blocks < 48) return 1;      // the zero-fill + finish passes are two more launches: only deep K pays
     int s = (int)(num_sms / tiles);
     if (s > 8) s = 8;
     while (s > 1 && num_k_blocks / s < 8) s--;

@@ -10,7 +10,7 @@ extern "C" {
 static int gemm_f16_impl(const void* a, const void* b, void* out, int out_is_f32, int M, int N, int K, int block_n, float alpha,
                   const float* bias, const void* residual, int epi_mode, int b_mn, mi3d_stream_t stream, int splits = 1, float* ws = nullptr) {
     if (M % 128 || K % 64) return MI3D_ERR_ARG;
-    if (block_n == 0) block_n = tc::pick_block_n(N, M / 128, 148);
+    if (block_n == 0) block_n = tc::pick_block_n(N, M / 128, 132);
     if (block_n == 0 || N % block_n) return MI3D_ERR_ARG;
     CUtensorMap ma, mb;
     int r = tc::make_map_matrix(&ma, (const __half*)a, K, M, K, 128);
@@ -65,7 +65,7 @@ int mi3d_conv3x3_f16(const void* x, const void* w, void* y, int Nimg, int H, int
     if (Mtot % 128 || Cin % 64) return MI3D_ERR_ARG;
     int bw = W < 128 ? W : 128, bh = 128 / bw; if (bh > H) bh = H; int bn = 128 / (bw * bh);
     if (bw * bh * bn != 128 || W % bw || H % bh || Nimg % bn) return MI3D_ERR_ARG;
-    if (block_n == 0) block_n = tc::pick_block_n(Cout, Mtot / 128, 148);
+    if (block_n == 0) block_n = tc::pick_block_n(Cout, Mtot / 128, 132);
     if (block_n == 0 || Cout % block_n) return MI3D_ERR_ARG;
     CUtensorMap ma, mb;
     int r = tc::make_map_nhwc(&ma, (const __half*)x, Cin, W, H, Nimg, bw, bh, bn);

@@ -1,5 +1,5 @@
-// tf32_test.cu -- C-ABI unit-test entry for the hand-written tcgen05 kind::tf32 tiles used by the fused field kernels:
-// validates the thread-written 128B-swizzle layout, the 3-term split accuracy, and K-major / MN-major operand descriptors.
+// tf32_test.cu -- C-ABI unit-test entry for the hand-written wgmma tf32 tiles used by the fused field forward kernel:
+// validates the thread-written 128B-swizzle layout, the 3-term split accuracy and the K-major operand descriptors.
 #include "tf32_tile.cuh"
 #include "mi3d_common.cuh"
 #include "../../include/mi3d.h"
@@ -16,54 +16,55 @@ __device__ void stage(const float* __restrict__ X, int R, int C, uint8_t* hi, ui
     }
 }
 
-// mode 0: D = A[128xK] . B[NxK]^T (both K-major) ; mode 1: D = A'[Kx128]^T . B'[KxN] (both MN-major) ; mode 2: A K-major, B' MN-major
-__global__ void __launch_bounds__(160, 1) k_tf32_tile_test(const float* __restrict__ A, const float* __restrict__ B, float* __restrict__ D, int N, int K, int mode) {
+// D = A[128 x K] . B[N x K]^T, both K-major; one warpgroup, two m64 halves
+template <int N>
+__global__ void __launch_bounds__(128, 1) k_tf32_tile_test(const float* __restrict__ A, const float* __restrict__ B, float* __restrict__ D, int K) {
     extern __shared__ uint8_t smem_dyn[];
     uint8_t* sm = smem_dyn + ((1024u - (tc::smem_u32(smem_dyn) & 1023u)) & 1023u);   // offset arithmetic keeps the shared address space (STS / LDS, not generic ST / LD)
-    const int swapv = mode >= 3; if (swapv) mode -= 2;
-    const int a_mn = mode == 1, b_mn = mode >= 1;
-    const int Ra = a_mn ? K : 128, Ca = a_mn ? 128 : K, Rb = b_mn ? K : N, Cb = b_mn ? N : K;
-    const uint32_t a_bytes = (uint32_t)Ra * Ca * 4, b_bytes = (uint32_t)Rb * Cb * 4;
+    const uint32_t a_bytes = 128u * (uint32_t)K * 4u, b_bytes = (uint32_t)N * (uint32_t)K * 4u;
     uint8_t *a_hi = sm, *a_lo = sm + a_bytes, *b_hi = sm + 2 * a_bytes, *b_lo = sm + 2 * a_bytes + b_bytes;
-    uint64_t* bar = reinterpret_cast<uint64_t*>(sm + 2 * a_bytes + 2 * b_bytes);
-    uint32_t* slot = reinterpret_cast<uint32_t*>(bar + 1);
-    const int tid = threadIdx.x, warp = tid >> 5;
-    stage(A, Ra, Ca, a_hi, a_lo, tid, blockDim.x);
-    stage(B, Rb, Cb, b_hi, b_lo, tid, blockDim.x);
-    if (tid == 0) { tc::mbar_init(bar, 1); tc::fence_barrier_init(); }
-    if (warp == 4) tc::tmem_alloc(slot, 64);
-    tc::fence_proxy_async();
-    tc::tc_fence_before();
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    stage(A, 128, K, a_hi, a_lo, tid, blockDim.x);
+    stage(B, N, K, b_hi, b_lo, tid, blockDim.x);
+    tc::fence_proxy_async();                 // tiles were written through the generic proxy, wgmma reads through the async proxy
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem = *slot;
-    if (warp == 4 && (tid & 31) == 0) {
-        ftc::Operand oa{tc::smem_u32(a_hi), tc::smem_u32(a_lo), (uint32_t)Ra * 128u, a_mn};
-        ftc::Operand ob{tc::smem_u32(b_hi), tc::smem_u32(b_lo), (uint32_t)Rb * 128u, b_mn};
-        ftc::g_swap_lbo_sbo = swapv;
-        ftc::issue_3tf32(tmem, oa, ob, K, ftc::idesc_tf32(128, N, a_mn, b_mn), 0);
-        tc::umma_commit(bar);
+    float d[2][N / 2];
+    wg::fence();
+    #pragma unroll
+    for (int h = 0; h < 2; h++)
+        ftc::issue_3tf32<N>(d[h], tc::smem_u32(a_hi) + 8192u * h, tc::smem_u32(a_lo) + 8192u * h, 128u * 128u,
+                            tc::smem_u32(b_hi), tc::smem_u32(b_lo), (uint32_t)N * 128u, K, 0u);
+    wg::commit();
+    wg::wait<0>();
+    #pragma unroll
+    for (int h = 0; h < 2; h++) {
+        wg::reg_fence(d[h]);
+        #pragma unroll
+        for (int j = 0; j < N / 8; j++)
+            #pragma unroll
+            for (int hh = 0; hh < 2; hh++) {
+                const int row = 64 * h + 16 * warp + (lane >> 2) + 8 * hh, col = 8 * j + 2 * (lane & 3);
+                D[(size_t)row * N + col] = d[h][4 * j + 2 * hh];
+                D[(size_t)row * N + col + 1] = d[h][4 * j + 2 * hh + 1];
+            }
     }
-    if (warp < 4) {
-        tc::mbar_wait(bar, 0);
-        tc::tc_fence_after();
-        for (int c0 = 0; c0 < N; c0 += 16) {
-            uint32_t v[16];
-            ftc::tmem_ld16(tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
-            for (int j = 0; j < 16; j++) D[(size_t)tid * N + c0 + j] = __uint_as_float(v[j]);
-        }
-        tc::tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 4) { tc::tc_fence_after(); tc::tmem_dealloc(tmem, 64); }
 }
 
 }  // namespace
 
 extern "C" int mi3d_tf32_tile_test(const float* a, const float* b, float* d, int N, int K, int mode, mi3d_stream_t stream) {
-    if ((N != 16 && N != 32 && N != 64) || K % 32 || K > 128 || mode < 0 || mode > 4) return MI3D_ERR_ARG;
-    const size_t smem = 1024 + 2 * (size_t)128 * K * 4 + 2 * (size_t)N * K * 4 + 64;
-    MI3D_CHECK(cudaFuncSetAttribute(k_tf32_tile_test, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_tf32_tile_test<<<1, 160, smem, (cudaStream_t)stream>>>(a, b, d, N, K, mode);
+    if ((N != 16 && N != 32 && N != 64) || K % 32 || K > 128 || K < 32 || mode != 0) return MI3D_ERR_ARG;
+    const size_t smem = 1024 + 2 * (size_t)128 * K * 4 + 2 * (size_t)N * K * 4;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (N == 16) {
+        MI3D_CHECK(cudaFuncSetAttribute(k_tf32_tile_test<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_tf32_tile_test<16><<<1, 128, smem, st>>>(a, b, d, K);
+    } else if (N == 32) {
+        MI3D_CHECK(cudaFuncSetAttribute(k_tf32_tile_test<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_tf32_tile_test<32><<<1, 128, smem, st>>>(a, b, d, K);
+    } else {
+        MI3D_CHECK(cudaFuncSetAttribute(k_tf32_tile_test<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_tf32_tile_test<64><<<1, 128, smem, st>>>(a, b, d, K);
+    }
     MI3D_RETURN_LAUNCH();
 }

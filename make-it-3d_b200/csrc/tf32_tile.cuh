@@ -1,10 +1,8 @@
-// tf32_tile.cuh -- helpers for hand-written tcgen05 kind::tf32 tiles with a 3-term hi/lo split (fp32-class accuracy):
+// tf32_tile.cuh -- helpers for hand-written wgmma tf32 tiles with a 3-term hi/lo split (fp32-class accuracy):
 //   x = hi + lo (hi = tf32-rounded x):  A.B ~= A_hi.B_hi + A_lo.B_hi + A_hi.B_lo
 // Storage convention for every operand tile: column blocks of [rows][32 fp32] (128-byte rows, 8-row / 1024-byte swizzle
-// atoms, block stride = rows * 128 B), written by ordinary threads through sw_off().  The SAME storage serves two uses:
-//   K-major  operand: rows = M or N index, columns = K   (descriptor: SBO = 1024 B, K advances by +32 B inside the row)
-//   MN-major operand: rows = K index,      columns = M/N (descriptor: LBO = block stride, SBO = 1024 B, K advances by +1024 B)
-// (cute::UMMA canonical layouts  K-major ((8,n),2):((8,SBO),1)  and  MN-major ((8,n),(8,k)):((1,LBO),(8,SBO)), in 16-byte units.)
+// atoms, block stride = rows * 128 B), written by ordinary threads through sw_off().  tf32 wgmma reads both operands K-major:
+// rows = M or N index, columns = K (descriptor: SBO = 1024 B, K advances by +32 B inside the row).
 #pragma once
 #include "tc_gemm.cuh"
 
@@ -17,80 +15,39 @@ __device__ __forceinline__ uint32_t sw_off(int row, int k) {
 __device__ __forceinline__ float tf32_hi(float x) {
     uint32_t r; asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x)); return __uint_as_float(r);
 }
-// cute::UMMA::InstrDescriptor, kind::tf32: c_format F32 (1) @4, a/b format TF32 (2) @7/@10, a_major @15, b_major @16 (1 = MN-major)
-__host__ __device__ constexpr uint32_t idesc_tf32(int M, int N, int a_mn = 0, int b_mn = 0) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// SW128 descriptor with an explicit leading-dimension byte offset (MN-major: distance between 32-element column blocks)
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
-    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t acc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-                 :: "r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(acc) : "memory");
-}
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(tc::smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, uint32_t (&v)[4]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-                   "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]) : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// four 4-column chunks, 8 columns apart: v[4j .. 4j+3] = columns taddr + 8j .. + 3 of this thread's TMEM lane; one wait for all four
-__device__ __forceinline__ void tmem_ld4x4(uint32_t taddr, uint32_t (&v)[16]) {
+// D[64 x N] (+)= A[64 x K] . B[N x K]^T with the 3-term split (both operands K-major hi / lo column blocks, K % 32 == 0).
+// a_hi .. b_lo: shared addresses of the first column block; *_blk: byte distance between column blocks.  Issue only: the caller
+// commits and waits.  `acc` = 0: the first MMA overwrites D.
+template <int N>
+__device__ __forceinline__ void issue_3tf32(float (&d)[N / 2], uint32_t a_hi, uint32_t a_lo, uint32_t a_blk, uint32_t b_hi, uint32_t b_lo,
+                                            uint32_t b_blk, int K, uint32_t acc) {
     #pragma unroll
-    for (int j = 0; j < 4; j++)
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-                     : "=r"(v[4 * j]), "=r"(v[4 * j + 1]), "=r"(v[4 * j + 2]), "=r"(v[4 * j + 3]) : "r"(taddr + 8u * (uint32_t)j));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-__device__ int g_swap_lbo_sbo = 0;   // experiment switch used by the unit-test kernel only
-// One operand = (hi base, lo base) of its first block + how to walk it.
-struct Operand { uint32_t hi, lo; uint32_t blk_stride; int mn_major; };
-
-// D[128 x N] (+)= A . B over K elements with the 3-term split.  K-major operands walk K as (block, +32 B); MN-major operands as (+1024 B).
-// `acc` in: 0 -> the first MMA overwrites D.  Returns 1.
-__device__ __forceinline__ uint32_t issue_3tf32(uint32_t tmem_d, const Operand& A, const Operand& B, int K, uint32_t idesc, uint32_t acc) {
     for (int k8 = 0; k8 < K / 8; k8++) {
-        const uint32_t oa = A.mn_major ? (uint32_t)k8 * 1024u : (uint32_t)(k8 >> 2) * A.blk_stride + (uint32_t)(k8 & 3) * 32u;
-        const uint32_t ob = B.mn_major ? (uint32_t)k8 * 1024u : (uint32_t)(k8 >> 2) * B.blk_stride + (uint32_t)(k8 & 3) * 32u;
-        const uint32_t la = A.mn_major ? A.blk_stride : 16u, lb = B.mn_major ? B.blk_stride : 16u;
-        uint64_t dah = desc_sw128(A.hi + oa, la), dal = desc_sw128(A.lo + oa, la);
-        uint64_t dbh = desc_sw128(B.hi + ob, lb), dbl = desc_sw128(B.lo + ob, lb);
-        if (g_swap_lbo_sbo) {
-            auto sw = [](uint64_t d) { const uint64_t l = (d >> 16) & 0x3FFF, s = (d >> 32) & 0x3FFF; return (d & ~((0x3FFFull << 16) | (0x3FFFull << 32))) | (s << 16) | (l << 32); };
-            if (A.mn_major) { dah = sw(dah); dal = sw(dal); }
-            if (B.mn_major) { dbh = sw(dbh); dbl = sw(dbl); }
-        }
-        umma_tf32(tmem_d, dah, dbh, idesc, acc); acc = 1;
-        umma_tf32(tmem_d, dal, dbh, idesc, 1);
-        umma_tf32(tmem_d, dah, dbl, idesc, 1);
+        const uint32_t oa = (uint32_t)(k8 >> 2) * a_blk + (uint32_t)(k8 & 3) * 32u, ob = (uint32_t)(k8 >> 2) * b_blk + (uint32_t)(k8 & 3) * 32u;
+        const uint64_t dah = wg::desc_sw128(a_hi + oa), dal = wg::desc_sw128(a_lo + oa);
+        const uint64_t dbh = wg::desc_sw128(b_hi + ob), dbl = wg::desc_sw128(b_lo + ob);
+        if constexpr (N == 16) { wg::wgmma_tf32_n16(d, dah, dbh, acc); wg::wgmma_tf32_n16(d, dal, dbh, 1u); wg::wgmma_tf32_n16(d, dah, dbl, 1u); }
+        else if constexpr (N == 32) { wg::wgmma_tf32_n32(d, dah, dbh, acc); wg::wgmma_tf32_n32(d, dal, dbh, 1u); wg::wgmma_tf32_n32(d, dah, dbl, 1u); }
+        else { wg::wgmma_tf32_n64(d, dah, dbh, acc); wg::wgmma_tf32_n64(d, dal, dbh, 1u); wg::wgmma_tf32_n64(d, dah, dbl, 1u); }
+        acc = 1u;
     }
-    return acc;
 }
 
 }  // namespace ftc
 
 // ---------------------------------------------------------------------------------------------------------------------
-// bf16 3-way split tiles (kind::f16, bf16 operands): x = h + m + l (each bf16, together ~24 bits) -> fp32-class products,
-// used by the fused field BACKWARD because 16-bit operands may be consumed MN-major
-// (kind::tf32 has no working MN-major form; the 16-bit one is verified by tools/explore_mn.py / mi3d_gemm_f16_bt).
+// bf16 3-way split tiles (wgmma bf16): x = h + m + l (each bf16, together ~24 bits) -> fp32-class products,
+// used by the fused field BACKWARD because 16-bit operands may be consumed MN-major (tf32 wgmma is K-major only;
+// the 16-bit MN-major descriptor form is also exercised by mi3d_gemm_f16_bt).
 // Storage: [rows][64 bf16] = 128-byte rows, 8-row swizzle atoms; the same tile is read K-major (rows = M/N, +32 B per
 // K = 16 step) or MN-major (rows = K, +2048 B per K = 16 step, LBO = distance to the next 64-column block).
 // ---------------------------------------------------------------------------------------------------------------------
 #include <cuda_bf16.h>
 namespace fbf {
 using ftc::mbar_arrive;
-using ftc::tmem_ld16;
-using ftc::tmem_ld4x4;
 
 // byte offset of element (row, c) inside a [rows x 64 bf16] tile
 __device__ __forceinline__ uint32_t sw_off16(int row, int c) {
@@ -123,38 +80,32 @@ __device__ __forceinline__ void split8(const float (&x)[8], uint4& ph, uint4& pm
     for (int i = 0; i < 4; i++) split3x2(x[2 * i], x[2 * i + 1], h[i], m[i], l[i]);
     ph = make_uint4(h[0], h[1], h[2], h[3]); pm = make_uint4(m[0], m[1], m[2], m[3]); pl = make_uint4(l[0], l[1], l[2], l[3]);
 }
-// kind::f16 instruction descriptor with BF16 operands (format 1), fp32 accumulate
-__host__ __device__ constexpr uint32_t idesc_bf16(int M, int N, int a_mn = 0, int b_mn = 0) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// one operand: three part tiles laid out back to back (h, m, l at +0, +part_stride, +2 part_stride)
-struct Operand { uint32_t base; uint32_t part_stride; uint32_t lbo; int mn_major; };
+// one operand: three part tiles laid out back to back (h, m, l at +0, +part_stride, +2 part_stride); lbo: MN-major distance between
+// 64-column blocks
+struct Operand { uint32_t base; uint32_t part_stride; uint32_t lbo; };
 
-// D[128 x N] (+)= A . B over K elements (K % 16 == 0; K-major operands: K <= 64).  Six MMAs per K = 16 step keep every
-// product term down to 2^-16 of the leading one: hh, hm, mh, hl, lh, mm  -> fp32-class accuracy.
-// The descriptors of one operand differ only in the 14-bit start-address field: one base descriptor per operand, then a 32-bit add of
-// (byte offset >> 4) per use (all tiles live below 256 KB, the field cannot carry into the LBO field).
-__device__ __forceinline__ uint32_t issue_bf16x3(uint32_t tmem_d, const Operand& A, const Operand& B, int K, uint32_t idesc, uint32_t acc) {
-    const uint64_t a0 = ftc::desc_sw128(A.base, A.mn_major ? A.lbo : 16u), b0 = ftc::desc_sw128(B.base, B.mn_major ? B.lbo : 16u);
-    const uint32_t a_lo = (uint32_t)a0, b_lo = (uint32_t)b0;
-    const uint64_t a_hi = a0 & 0xFFFFFFFF00000000ull, b_hi = b0 & 0xFFFFFFFF00000000ull;
+// D[64 x N] (+)= A . B over K elements (K % 16 == 0; K-major operands: K <= 64).  TA / TB = 1: operand is MN-major.  Six MMAs per
+// K = 16 step keep every product term down to 2^-16 of the leading one: hh, hm, mh, hl, lh, mm  -> fp32-class accuracy.
+// Issue only: the caller commits and waits.
+template <int N, int TA, int TB>
+__device__ __forceinline__ void issue_bf16x3(float (&d)[N / 2], const Operand& A, const Operand& B, int K, uint32_t acc) {
+    const uint64_t a0 = wg::desc_sw128(A.base, TA ? A.lbo : 16u), b0 = wg::desc_sw128(B.base, TB ? B.lbo : 16u);
     #pragma unroll
     for (int k16 = 0; k16 < K / 16; k16++) {
-        const uint32_t oa = (A.mn_major ? (uint32_t)k16 * 2048u : (uint32_t)k16 * 32u) >> 4;
-        const uint32_t ob = (B.mn_major ? (uint32_t)k16 * 2048u : (uint32_t)k16 * 32u) >> 4;
+        const uint32_t oa = (TA ? (uint32_t)k16 * 2048u : (uint32_t)k16 * 32u) >> 4;
+        const uint32_t ob = (TB ? (uint32_t)k16 * 2048u : (uint32_t)k16 * 32u) >> 4;
         uint64_t da[3], db[3];
         #pragma unroll
-        for (int q = 0; q < 3; q++) {
-            da[q] = a_hi | (uint64_t)(a_lo + oa + q * (A.part_stride >> 4));
-            db[q] = b_hi | (uint64_t)(b_lo + ob + q * (B.part_stride >> 4));
-        }
-        tc::umma_f16(tmem_d, da[0], db[0], idesc, acc); acc = 1;
-        tc::umma_f16(tmem_d, da[0], db[1], idesc, 1);
-        tc::umma_f16(tmem_d, da[1], db[0], idesc, 1);
-        tc::umma_f16(tmem_d, da[0], db[2], idesc, 1);
-        tc::umma_f16(tmem_d, da[2], db[0], idesc, 1);
-        tc::umma_f16(tmem_d, da[1], db[1], idesc, 1);
+        for (int q = 0; q < 3; q++) { da[q] = a0 + oa + q * (A.part_stride >> 4); db[q] = b0 + ob + q * (B.part_stride >> 4); }
+        auto mma = [&](uint64_t x, uint64_t y, uint32_t s) {
+            if constexpr (N == 32) wg::wgmma_bf16_n32<TA, TB>(d, x, y, s); else wg::wgmma_bf16_n64<TA, TB>(d, x, y, s);
+        };
+        mma(da[0], db[0], acc); acc = 1u;
+        mma(da[0], db[1], 1u);
+        mma(da[1], db[0], 1u);
+        mma(da[0], db[2], 1u);
+        mma(da[2], db[0], 1u);
+        mma(da[1], db[1], 1u);
     }
-    return acc;
 }
 }  // namespace fbf

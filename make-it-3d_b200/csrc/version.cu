@@ -1,2 +1,2 @@
 #include "../../include/mi3d.h"
-extern "C" const char* mi3d_version(void) { return "mi3d-b200 0.1 (sm_100a)"; }
+extern "C" const char* mi3d_version(void) { return "mi3d-b200 0.1 (sm_90a)"; }

@@ -3,7 +3,7 @@
 `train_step(text_embeddings, pred_rgb, ref_rgb=None, noise=None, islarge=False, ref_text=None, clip_model=None,
 guidance_scale=10) -> (loss, imgs)` performs the SDS backward itself into pred_rgb's graph exactly like the reference
 (nerf/sd.py:163-172) and returns (0, None) on that branch.  Everything between pred_rgb and the gradient runs in the
-engine of csrc/sd_engine.cu (tcgen05 tile kernel + fused memory-bound kernels); there is no diffusers / cuDNN / cuBLAS
+engine of csrc/sd_engine.cu (wgmma tile kernel + fused memory-bound kernels); there is no diffusers / cuDNN / cuBLAS
 call and no CPU fallback.
 
 Weights: parameters are enumerated by diffusers' state_dict names; real SD-2.0-base checkpoints load through

@@ -60,7 +60,7 @@ def shared_seed(base_seed, iteration):
 class GradientAllReduce:
     """Flat-bucket all-reduce of the two optimizer groups of NeRFNetwork.get_params (nerf/network_tcnn.py:195-206):
     encoder.params (12 196 240 fp32, reduced in place, no copy) and the 6 MLP tensors (6 532 fp32, packed into one bucket).
-    Payload 48.8 MB per step -> ~0.1 ms at NVLink-5 line rate (SURVEY.md section 5)."""
+    Payload 48.8 MB per step -> ~0.19 ms at NVLink-4 line rate, 450 GB/s per direction (SURVEY.md section 5)."""
 
     def __init__(self, encoder_params, mlp_params, op="sum"):
         self.encoder_params = encoder_params

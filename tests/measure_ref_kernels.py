@@ -1,8 +1,10 @@
-"""The reference's OWN ray-march / composite kernels (raymarching/src/raymarching.cu compiled for sm_100a into oracle/_ref/, driven
+"""The reference's OWN ray-march / composite kernels (raymarching/src/raymarching.cu compiled for sm_90a into oracle/_ref/, driven
 exactly like raymarching/raymarching.py:173-303 drives them: 268 MB zero-fill, .item() host sync, zeros_like for the gradients)
 timed beside the mi3d kernels on the bench's rays (128x128, sphere r = 0.2, front view: M ~ 635 k samples).  CUDA events, median
 of 20, legacy default stream for the reference (its launches use <<<g,b>>> with no stream).  TEST/MEASUREMENT TOOL, not product.
-    python tests/measure_ref_kernels.py > profiles/r2_ref_kernels.txt       (GPU box)"""
+It needs oracle/_ref/, which build() only makes when MI3D_REFERENCE_DIR names a checkout of Make-It-3D:
+    MI3D_REFERENCE_DIR=<checkout> python -c "import __graft_entry__ as g; g.build()"
+    python tests/measure_ref_kernels.py       (GPU machine)"""
 import ctypes as C
 import importlib
 import os

@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds for sm_100a, loads without a GPU, and exports exactly what include/mi3d.h declares."""
+"""CPU: the C-ABI library builds for sm_90a, loads without a GPU, and exports exactly what include/mi3d.h declares."""
 import ctypes
 import os
 import re
@@ -19,7 +19,7 @@ def test_library_exports_every_declared_symbol(mi3d):
     for s in syms:
         assert hasattr(lib, s), f"libmi3d.so does not export {s}"
     assert sorted(mi3d._lib.SYMBOLS) == syms
-    assert b"sm_100a" in lib.mi3d_version()
+    assert b"sm_90a" in lib.mi3d_version()
 
 
 def test_workspace_queries_are_pure_host(mi3d):
@@ -70,10 +70,11 @@ def test_state_dict_keys_match_reference(mi3d):
 
 
 def test_committed_bench_line_has_every_contract_key():
-    """profiles/r1_final_bench.json is the last line bench.py printed on a B200: the keys the driver parses must all be there"""
+    """profiles/bench_h100_n1.json is the line bench.py printed on an H100 (80 GB HBM3, 400 W power limit): every key a consumer of
+    the bench line parses must be there"""
     import json
     import os
-    path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "profiles", "r1_final_bench.json")
+    path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "profiles", "bench_h100_n1.json")
     line = json.loads(open(path).read())
     for key in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline", "dtype",
                 "data", "config", "e2e", "gpu_launches", "clocks", "roofline", "cpu_baseline"):
@@ -102,22 +103,12 @@ def test_engine_stream_context_is_a_no_op_without_graph_replay():
 
 def test_backend_mi3d_covers_reference_call_sites():
     """Every `get_backend().<name>(...)` call in the REFERENCE's raymarching/raymarching.py must resolve on backend_mi3d._backend
-    with the same positional arity (build container only: /root/reference is absent on the GPU box)."""
-    import ast
+    with the same positional arity (the calls and their arities are stored in tests/golden/reference_call_sites.json)."""
     import importlib
     import inspect
-    import os
-
-    import pytest
-    path = "/root/reference/raymarching/raymarching.py"
-    if not os.path.exists(path):
-        pytest.skip("reference tree not present")
+    import json
     be = importlib.import_module("make-it-3d_b200.backend_mi3d")._backend
-    calls = {}
-    for node in ast.walk(ast.parse(open(path).read())):
-        if isinstance(node, ast.Call) and isinstance(node.func, ast.Attribute) and isinstance(node.func.value, ast.Call) \
-                and getattr(node.func.value.func, "id", "") == "get_backend":
-            calls.setdefault(node.func.attr, set()).add(len(node.args))
+    calls = json.load(open(os.path.join(ROOT, "tests", "golden", "reference_call_sites.json")))["calls"]
     assert {"near_far_from_aabb", "march_rays_train", "composite_rays_train_forward", "composite_rays_train_backward", "packbits",
             "morton3D", "morton3D_invert", "march_rays", "composite_rays"} <= set(calls)
     for name, arities in calls.items():
@@ -126,4 +117,4 @@ def test_backend_mi3d_covers_reference_call_sites():
         params = list(inspect.signature(fn).parameters.values())
         if any(p.kind == p.VAR_POSITIONAL for p in params):
             continue                                   # the loudly-failing stubs of unreachable entry points
-        assert arities == {len(params)}, (name, arities, len(params))
+        assert set(arities) == {len(params)}, (name, arities, len(params))

@@ -106,7 +106,7 @@ def _worker(rank, world, port, result):
 
 def test_sharded_adan_equals_single_process_update():
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     mgr = mp.Manager()
     result = mgr.dict()
     mp.spawn(_worker, args=(2, _free_port(), result), nprocs=2, join=True)

@@ -113,7 +113,7 @@ def test_density_matches_oracle_and_k1_backward():
 def test_fused_render_step_matches_reference_golden(case, impl):
     """The drop-in call Trainer.train_step makes (model.render(...), nerf/utils.py:496) on the fused CUDA path vs the
     golden vectors recorded from the reference's Python: image / depth / weights_sum / losses and parameter gradients.
-    Both kernel families (mi3d_field_cfg.impl: tcgen05 split-precision tiles, fp32 FFMA tiles) are held to the same bounds."""
+    Both kernel families (mi3d_field_cfg.impl: tensor-core split-precision tiles, fp32 FFMA tiles) are held to the same bounds."""
     g = load_golden(f"render_{case}.npz")
     net = _net_from_golden(g, field_impl=impl)
     net.train()
@@ -124,7 +124,7 @@ def test_fused_render_step_matches_reference_golden(case, impl):
                      smooth_noise=_cu(g["smooth_noise"]))
     ws = list(net._workspaces.values())[0]
     assert int(ws.counter[0]) == int(g["total"])
-    tol = 1e-3   # BASELINE.json north_star: "outputs within 1e-3 rel of reference"; measured margins are ~100x tighter
+    tol = 1e-3   # BASELINE.json north_star: "outputs within 1e-3 rel of reference"
     assert max_abs(out["image"][0].detach().cpu(), g["image"]) < 2e-5
     assert max_abs(out["weights_sum"][0].detach().cpu(), g["weights_sum"]) < 2e-5
     assert rel_err(out["depth"][0, :, 0].detach().cpu(), g["depth"], floor=1e-2) < 1e-4

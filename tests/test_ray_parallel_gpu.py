@@ -1,4 +1,4 @@
-"""2 GPUs (gpurun --gpus 2; skipped on a 1-GPU box): the ray-parallel render step over NCCL ==
+"""2 GPUs (skipped on a 1-GPU machine): the ray-parallel render step over NCCL ==
 single-process sequential accumulation of the same G = 2 views (SURVEY.md 8e: "define G-GPU step == single-GPU accumulation of
 the same G poses' gradients ... and test exactly that equivalence").
 
@@ -6,7 +6,7 @@ Each rank marches every 2nd pixel of BOTH views (balanced sample counts whatever
 all-to-all, per-view loss means use the all-gathered total sample counts, gradients are summed by GradientAllReduce.  Expected:
   * the owner's image / depth / weights_sum are BIT-identical to the unsharded render of that view (same samples, same kernels),
   * per-view regulariser means and the summed parameter gradients agree to summation-order accuracy,
-  * the two ranks march (nearly) the same number of samples although one view is heavier than the other (measured 317 666 vs 268 728)."""
+  * the two ranks march (nearly) the same number of samples although one view is heavier than the other."""
 import argparse
 import importlib
 import math
@@ -104,7 +104,7 @@ def _worker(rank, world, port, result):
 
 def test_two_rank_ray_parallel_step_equals_sequential_accumulation():
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     mgr = mp.Manager()
     result = mgr.dict()
     mp.spawn(_worker, args=(2, _free_port(), result), nprocs=2, join=True)
@@ -118,7 +118,7 @@ def test_two_rank_ray_parallel_step_equals_sequential_accumulation():
     gs = r0["seq_g_table"]
     assert float((r0["g_table"] - gs).abs().max()) <= 5e-5 * float(gs.abs().max())
     assert int((r0["g_table"] != 0).sum()) == int((gs != 0).sum())
-    for a, b in zip(r0["g_mlp"], r0["seq_g_mlp"]):        # TMEM-resident sums over ~1.5 M evaluations in a different tile order (measured 5.8e-5)
+    for a, b in zip(r0["g_mlp"], r0["seq_g_mlp"]):        # per-CTA weight-gradient sums over ~1.5 M evaluations in a different tile order
         assert float((a - b).abs().max()) <= 2e-4 * float(b.abs().max())
     # balance: the views differ in samples (close view ~1.18x the far one), the ranks do not
     assert seq[0]["marched"] > 1.1 * seq[1]["marched"]

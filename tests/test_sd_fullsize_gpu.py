@@ -12,9 +12,9 @@ execution there is) and its deviation from the fp32 oracle is printed next to th
 per tensor, i.e. the engine may not be meaningfully worse than the best possible fp16 execution of the reference arithmetic.
 Random-init weights make this a harsh test: without trained weights nothing damps rounding noise through 25 residual blocks, and
 classifier-free guidance multiplies the (text - uncond) difference by 10.
-Measured on B200 (profiles/r2_pytest_gpu.txt): U-Net taps 2.9e-4 .. 1.9e-3 (fp16-storage oracle: 2.1e-4 .. 1.4e-3), CFG noise_pred
-1.07e-2 (8.9e-3), SDS grad 4.7e-3 (3.9e-3), latents 3.8e-4 (3.3e-4), d pred_rgb 3.3e-3 (2.7e-3): the engine sits within 1.5x of
-the fp16-storage floor everywhere; the 1e-3 figure of north_star is not reachable by ANY fp16-activation execution of this network."""
+Measured on an H100 80GB HBM3 (sm_90a, 400 W power limit), engine (fp16-storage oracle) relative L2 error vs fp32: U-Net taps
+2.9e-4 .. 1.9e-3 (2.1e-4 .. 1.3e-3), CFG noise_pred 1.08e-2 (9.0e-3), SDS grad 4.7e-3 (3.9e-3), latents 3.8e-4 (3.3e-4), d pred_rgb
+3.3e-3 (2.7e-3): the engine sits within 1.5x of the fp16-storage floor everywhere; the 1e-3 figure of north_star is not reachable by ANY fp16-activation execution of this network."""
 import importlib
 import time
 

@@ -1,4 +1,4 @@
-"""GPU parity of the SD guidance engine (tcgen05 tiles + fused memory-bound kernels) against the fp32 PyTorch restatement of
+"""GPU parity of the SD guidance engine (wgmma tiles + fused memory-bound kernels) against the fp32 PyTorch restatement of
 diffusers' U-Net / VAE (oracle/sd_ref.py), on reduced configurations with seeded random weights (no SD weights offline).
 Tolerance: the engine stores activations in fp16 and accumulates in fp32 -> "fp16 tolerance" of BASELINE.json's north_star;
 asserted as relative L2 error < 1e-2 per tensor and cosine similarity > 0.9999 (observed values printed)."""

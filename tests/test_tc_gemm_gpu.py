@@ -1,4 +1,4 @@
-"""GPU: the tcgen05/TMEM/TMA tile kernel vs a plain PyTorch fp32 reference of the same op (floating-point kernel:
+"""GPU: the wgmma/TMA tile kernel vs a plain PyTorch fp32 reference of the same op (floating-point kernel:
 torch fp32 is the stated checker).  Inputs are fp16; products are exact in fp32, accumulation order differs -> the
 bound is K * eps_fp32 * |a||b| plus one fp16 rounding of the output (2^-11 relative)."""
 import ctypes as C
@@ -105,8 +105,8 @@ def test_implicit_conv3x3_matches_fp32_reference(L, Nimg, H, W, Cin, Cout):
 
 @pytest.mark.parametrize("N,K", [(64, 32), (64, 64), (32, 64), (16, 64), (64, 128), (32, 128)])
 def test_tf32_split_tiles(L, N, K):
-    """Hand-written kind::tf32 tiles of the field FORWARD kernel (K-major operands): the 3-term split must be fp32-class.
-    (kind::tf32 has no working MN-major form -- tools/explore_mn.py -- which is why the backward uses bf16 tiles.)"""
+    """Hand-written wgmma tf32 tiles of the field FORWARD kernel (K-major operands): the 3-term split must be fp32-class.
+    (tf32 wgmma reads K-major operands only, which is why the backward uses bf16 tiles.)"""
     g = torch.Generator(device="cuda").manual_seed(N + K)
     a = torch.randn(128, K, device="cuda", generator=g); b = torch.randn(N, K, device="cuda", generator=g); ref = a.double() @ b.double().t()
     d = torch.empty(128, N, device="cuda")
@@ -132,7 +132,7 @@ def test_gemm_mn_major_b_operand(L, M, N, K, bn):
 @pytest.mark.parametrize("B,T,Tk,valid,heads", [(2, 4096, 4096, 4096, 5), (2, 1024, 1024, 1024, 10), (2, 256, 128, 77, 20), (2, 64, 64, 64, 20),
                                                 (1, 16, 16, 16, 1), (1, 384, 300, 300, 2)])
 def test_flash_attention_matches_fp32_reference(L, B, T, Tk, valid, heads):
-    """Fused attention (S in TMEM, P through shared memory) vs torch fp32 softmax(q k^T / 8) v on the same fp16 inputs.
+    """Fused attention (S, P and O in registers) vs torch fp32 softmax(q k^T / 8) v on the same fp16 inputs.
     Bound: P is rounded to fp16 before the second product (2^-11 relative per term) + one fp16 rounding of the output."""
     g = torch.Generator(device="cuda").manual_seed(B * T + heads)
     C_ = heads * 64
@@ -153,7 +153,7 @@ def test_flash_attention_matches_fp32_reference(L, B, T, Tk, valid, heads):
 
 
 def test_flash_attention_lazy_rescale(L):
-    """Logits that keep growing along the key axis force the lazy-rescale path (O row in TMEM multiplied by alpha) in every block;
+    """Logits that keep growing along the key axis force the online rescale (O rows in registers multiplied by alpha) in every block;
     logits that shrink never trigger it.  Both must match the fp32 reference."""
     B, T, heads, C_ = 1, 256, 2, 128
     g = torch.Generator(device="cuda").manual_seed(3)

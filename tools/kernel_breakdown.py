@@ -1,6 +1,6 @@
 """Per-kernel GPU time of the bench step IN PIPELINE CONTEXT (CUPTI activity records through torch.profiler: real timeline, kernels
 of graph replays included, no serialisation / cache flush like ncu) -- the nsys substitute of this image.
-    python tools/kernel_breakdown.py [--steps 4] [--defer-backward] > profiles/r2_kernel_breakdown.txt        (GPU box, 1 GPU)
+    python tools/kernel_breakdown.py [--steps 4] [--defer-backward]        (1 GPU)
 Prints per kernel name: launches / step, total us / step, mean us, share of the summed kernel time; then the GPU busy time per step
 (union of kernel intervals) and the wall time per step, i.e. how much of the step the GPU sits idle between launches."""
 import argparse

@@ -1,6 +1,6 @@
-"""SASS instruction histogram of libmi3d.so per kernel: the Blackwell-native mnemonics (UTCHMMA = tcgen05.mma, LDTM/STTM = tcgen05.ld/st,
-UTMALDG/UTMASTG = TMA, UTCBAR = tcgen05.commit, SYNCS = mbarrier) that prove which kernels run on the 5th-gen tensor cores.
-    python tools/sass_histogram.py > profiles/r2_sass_histogram.txt        (no GPU needed: cuobjdump reads the cubin in the .so)"""
+"""SASS instruction histogram of libmi3d.so per kernel: the Hopper mnemonics (HGMMA = wgmma.mma_async, WARPGROUP = its fences,
+UTMALDG/UTMASTG = TMA, SYNCS = mbarrier) that show which kernels run on the tensor cores, next to RED / ATOM / FFMA / loads / stores.
+    python tools/sass_histogram.py        (no GPU needed: cuobjdump reads the cubin in the .so)"""
 import collections
 import os
 import re
@@ -9,7 +9,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SO = os.path.join(ROOT, "make-it-3d_b200", "libmi3d.so")
-WATCH = ["UTCHMMA", "UTCQMMA", "UTCBAR", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UTMAPF", "SYNCS", "RED", "ATOM", "HMMA", "FFMA", "LDG", "STG", "MUFU"]
+WATCH = ["HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UTMAPF", "SYNCS", "RED", "ATOM", "HMMA", "FFMA", "LDG", "STG", "LDL", "STL", "MUFU"]
 
 
 def main():
@@ -31,7 +31,7 @@ def main():
                 if op.startswith(w):
                     hist[kern][w] += 1
                     break
-    print(f"# cuobjdump -sass {os.path.relpath(SO, ROOT)} : instruction counts per kernel (static SASS, sm_100a)")
+    print(f"# cuobjdump -sass {os.path.relpath(SO, ROOT)} : instruction counts per kernel (static SASS, sm_90a)")
     print(f"{'kernel':70s} {'total':>7s} " + " ".join(f"{w:>7s}" for w in WATCH))
     tot = collections.Counter()
     for k, c in hist.items():
