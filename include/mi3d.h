@@ -466,6 +466,46 @@ int mi3d_sd_graph_replays(mi3d_sd_t h);
 /* debug tap: device pointer + size of a named intermediate ("unet.mid", "vae.grad_in", ...) */
 int mi3d_sd_debug_tensor(mi3d_sd_t h, const char* name, void** ptr, size_t* bytes);
 
+/* ------------------------------------------------------------------------------------------------------
+ * B4: CLIP losses  (replaces openai CLIP's encode_image / encode_text behind the per-step CLIP losses, nerf/utils.py:436-453, 561-563,
+ * and the denoise branch's, nerf/sd.py:97-114, 157-158)
+ * ------------------------------------------------------------------------------------------------------ */
+typedef struct {
+    int image_res, patch;      /* 224, 16 */
+    int width, layers, heads;  /* image tower: 768, 12, 12 (head_dim 64); layers = 0: no image tower in this engine */
+    int embed_dim;             /* 512: output features of both towers */
+    int context_len, vocab;    /* 77, 49408 */
+    int text_width, text_layers, text_heads;   /* 512, 12, 8; text_layers = 0: no text tower in this engine */
+    int max_batch;             /* images / prompts per call (1..8); 2 encodes [rendered, reference] in one pass */
+} mi3d_clip_cfg;
+
+typedef struct mi3d_clip* mi3d_clip_t;
+
+/* HOST: bytes of device workspace the engine needs (0: invalid configuration); create plans inside it, NULL on failure */
+size_t mi3d_clip_workspace_bytes(const mi3d_clip_cfg* cfg);
+mi3d_clip_t mi3d_clip_create(const mi3d_clip_cfg* cfg, void* workspace, size_t workspace_bytes);
+void mi3d_clip_destroy(mi3d_clip_t h);
+/* Parameters are enumerated by openai CLIP's state_dict names ("visual.conv1.weight", "transformer.resblocks.0.attn.in_proj_weight",
+ * "visual.proj", ...; a '#...' suffix marks a derived copy of the base tensor).  load: src = fp32 DEVICE tensor in openai's layout. */
+int mi3d_clip_num_params(mi3d_clip_t h);
+const char* mi3d_clip_param_name(mi3d_clip_t h, int i);
+int mi3d_clip_param_shape(mi3d_clip_t h, int i, int* shape4); /* returns rank */
+int mi3d_clip_load_param(mi3d_clip_t h, int i, const float* src, mi3d_stream_t stream);
+/* CUDA-graph replay of the static launch lists, from a list's third call on (`stream` must then be capturable); off by default.
+ * mi3d_clip_graph_replays: lists currently instantiated. */
+int mi3d_clip_set_graph_replay(mi3d_clip_t h, int enable);
+int mi3d_clip_graph_replays(mi3d_clip_t h);
+/* img fp32 [B,3,H,W] -> feats fp32 [B,embed_dim] (encode_image).  aug != 0: the reference's aug first (Resize((res,res)): bilinear,
+ * align_corners=False, no antialiasing; then Normalize with CLIP's mean / std); aug = 0: img is already augmented and res x res.
+ * need_grad != 0 keeps a tape for mi3d_clip_encode_image_backward; any image forward replaces the previous tape.  B <= max_batch. */
+int mi3d_clip_encode_image(mi3d_clip_t h, const float* img, int B, int H, int W, int aug, int need_grad, float* feats, mi3d_stream_t stream);
+/* input gradient of the first n_grad images of the last (taped) image forward: dfeats fp32 [n_grad,embed_dim] -> dimg fp32
+ * [n_grad,3,H,W] (overwritten).  Weights frozen.  MI3D_ERR_ARG without a tape or with n_grad outside 1..B of that forward. */
+int mi3d_clip_encode_image_backward(mi3d_clip_t h, const float* dfeats, int n_grad, float* dimg, mi3d_stream_t stream);
+/* tokens int64 [B,context_len] (clip.tokenize ids; the features are taken at each row's argmax, the EOT token) -> feats fp32
+ * [B,embed_dim] (encode_text, causal attention).  Ids outside [0, vocab) are clamped into it. */
+int mi3d_clip_encode_text(mi3d_clip_t h, const long long* tokens, int B, float* feats, mi3d_stream_t stream);
+
 /* unit-test entry for the hand-written wgmma tf32 tiles of the field forward (3-term split, K-major operands):
  * mode 0 (the only one): d[128,N] = a[128,K] . b[N,K]^T, N in {16, 32, 64}, K in {32, 64, 96, 128}.  fp32 in/out. */
 int mi3d_tf32_tile_test(const float* a, const float* b, float* d, int N, int K, int mode, mi3d_stream_t stream);

@@ -1,0 +1,251 @@
+// clip_kernels.cuh -- the memory-bound kernels of the CLIP engine (clip_engine.cu) that the SD kernels do not already provide:
+// image preprocessing (resize / normalise / patchify) and its input gradient, token / class / positional embeddings, the EOT-row
+// select, LayerNorm backward and the causal softmax of the text tower.  Activations are token rows of fp16 ("tokens x C"),
+// reductions are fp32, and every output element is written by exactly one thread (no atomics: run-to-run deterministic).
+#pragma once
+#include <cuda_fp16.h>
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "sd_kernels.cuh"
+
+namespace clipk {
+
+// openai CLIP's Normalize constants
+__device__ __forceinline__ float norm_mean(int c) { return c == 0 ? 0.48145466f : (c == 1 ? 0.4578275f : 0.40821073f); }
+__device__ __forceinline__ float norm_inv_std(int c) { return c == 0 ? 1.f / 0.26862954f : (c == 1 ? 1.f / 0.26130258f : 1.f / 0.27577711f); }
+
+// Source coordinate of a bilinear resize, F.interpolate(mode='bilinear', align_corners=False, antialias=False)
+struct Tap { int i0, i1; float l; };
+__device__ __forceinline__ Tap bilinear_tap(int o, float scale, int in) {
+    const float f = fmaxf((o + 0.5f) * scale - 0.5f, 0.f);
+    Tap t; t.i0 = min((int)f, in - 1); t.i1 = min(t.i0 + 1, in - 1); t.l = f - t.i0;
+    return t;
+}
+
+// img fp32 [B,3,H,W] -> patch rows fp16 [B * G*G][3*P*P], column (c, ky, kx), row (b, py, px), G = R / P.
+// aug != 0: bilinear resize H x W -> R x R, then (x - mean) / std.  aug == 0: the image is already R x R and augmented.
+// One thread per 8 consecutive kx of one (row, c, ky).
+__global__ void k_preprocess(const float* __restrict__ img, int B, int H, int W, int R, int P, int aug, __half* __restrict__ out) {
+    const int G = R / P, KP = 3 * P * P, vec = P / 8;
+    const size_t total = (size_t)B * G * G * 3 * P * vec;
+    const float sy = (float)H / R, sx = (float)W / R;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int v = (int)(i % vec); size_t r = i / vec;
+        const int ky = (int)(r % P); r /= P;
+        const int c = (int)(r % 3); const size_t row = r / 3;
+        const int px = (int)(row % G), py = (int)((row / G) % G), b = (int)(row / ((size_t)G * G));
+        const int oy = py * P + ky;
+        const float* ch = img + ((size_t)b * 3 + c) * H * W;
+        __align__(16) __half o[8];
+        if (aug) {
+            const Tap ty = bilinear_tap(oy, sy, H);
+            #pragma unroll
+            for (int k = 0; k < 8; k++) {
+                const Tap tx = bilinear_tap(px * P + v * 8 + k, sx, W);
+                const float val = (1.f - ty.l) * ((1.f - tx.l) * ch[(size_t)ty.i0 * W + tx.i0] + tx.l * ch[(size_t)ty.i0 * W + tx.i1]) +
+                                  ty.l * ((1.f - tx.l) * ch[(size_t)ty.i1 * W + tx.i0] + tx.l * ch[(size_t)ty.i1 * W + tx.i1]);
+                o[k] = __float2half_rn((val - norm_mean(c)) * norm_inv_std(c));
+            }
+        } else {
+            #pragma unroll
+            for (int k = 0; k < 8; k++) o[k] = __float2half_rn(ch[(size_t)oy * W + px * P + v * 8 + k]);
+        }
+        *reinterpret_cast<uint4*>(out + row * KP + ((size_t)c * P + ky) * P + v * 8) = *reinterpret_cast<const uint4*>(o);
+    }
+}
+
+// Input gradient of k_preprocess, as a gather: grad[b,c,y,x] = sum over the output pixels whose bilinear taps touch (y, x) of
+// tap weight * dpatch / std, divided by the gradient scale s of k_grad_in.  dpatch fp16 [n * G*G][3*P*P]; grad fp32 [n,3,H,W] (overwritten).
+__global__ void k_preprocess_bwd(const __half* __restrict__ dpatch, int n, int H, int W, int R, int P, int aug, const float* __restrict__ scale,
+                                 float* __restrict__ grad) {
+    const int G = R / P, KP = 3 * P * P;
+    const float inv_s = 1.f / *scale;
+    const size_t total = (size_t)n * 3 * H * W;
+    const float sy = (float)H / R, sx = (float)W / R;
+    auto at = [&](int b, int c, int oy, int ox) {
+        const size_t row = ((size_t)b * G + oy / P) * G + ox / P;
+        return __half2float(dpatch[row * KP + ((size_t)c * P + oy % P) * P + ox % P]);
+    };
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int x = (int)(i % W), y = (int)((i / W) % H), c = (int)((i / ((size_t)W * H)) % 3), b = (int)(i / ((size_t)3 * W * H));
+        if (!aug) { grad[i] = at(b, c, y, x) * inv_s; continue; }
+        // output pixels whose source footprint can touch (x, y): source coordinate within (x - 1, x + 1)
+        const int ox_lo = max(0, (int)floorf((x - 1 + 0.5f) / sx - 0.5f)), ox_hi = min(R - 1, (int)ceilf((x + 1 + 0.5f) / sx - 0.5f));
+        const int oy_lo = max(0, (int)floorf((y - 1 + 0.5f) / sy - 0.5f)), oy_hi = min(R - 1, (int)ceilf((y + 1 + 0.5f) / sy - 0.5f));
+        float acc = 0.f;
+        for (int oy = oy_lo; oy <= oy_hi; oy++) {
+            const Tap ty = bilinear_tap(oy, sy, H);
+            float wy = 0.f; if (ty.i0 == y) wy += 1.f - ty.l; if (ty.i1 == y) wy += ty.l;
+            if (wy == 0.f) continue;
+            for (int ox = ox_lo; ox <= ox_hi; ox++) {
+                const Tap tx = bilinear_tap(ox, sx, W);
+                float wx = 0.f; if (tx.i0 == x) wx += 1.f - tx.l; if (tx.i1 == x) wx += tx.l;
+                if (wx == 0.f) continue;
+                acc += wy * wx * at(b, c, oy, ox);
+            }
+        }
+        grad[i] = acc * norm_inv_std(c) * inv_s;
+    }
+}
+
+// Feature gradient fp32 [n] -> fp16, scaled by the power of two s that brings max |g| into [128, 256); s is stored for k_preprocess_bwd.
+// The input-gradient pass runs in fp16 and is linear in g: without the scale, the per-token gradients (about 1e-3 of the feature
+// gradient after the attention spreads it over the tokens) fall into fp16's subnormal range.  One block.
+__global__ void k_grad_in(const float* __restrict__ g, int n, __half* __restrict__ out, float* __restrict__ scale) {
+    __shared__ float s_max[32];
+    float m = 0.f;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, fabsf(g[i]));
+    m = sdk::warp_max(m);
+    if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = m;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        m = threadIdx.x < (blockDim.x >> 5) ? s_max[threadIdx.x] : 0.f;
+        m = sdk::warp_max(m);
+        if (threadIdx.x == 0) {
+            int e = 0;
+            if (m > 0.f && isfinite(m)) frexpf(m, &e);
+            s_max[0] = m > 0.f && isfinite(m) ? ldexpf(1.f, min(max(8 - e, -100), 100)) : 1.f;
+        }
+    }
+    __syncthreads();
+    const float s = s_max[0];
+    for (int i = threadIdx.x; i < n; i += blockDim.x) out[i] = __float2half_rn(g[i] * s);
+    if (threadIdx.x == 0) *scale = s;
+}
+
+// x[b*Tpad + t] = (t == 0 ? cls : patch[b*np + t - 1]) + pos[t] for t <= np; rows np+1 .. Tpad-1 are zero.  8 channels per thread.
+__global__ void k_image_embed(const __half* __restrict__ patch, const float* __restrict__ cls, const float* __restrict__ pos, __half* __restrict__ x,
+                              int B, int np, int Tpad, int C) {
+    const int vc = C / 8;
+    const size_t total = (size_t)B * Tpad * vc;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int v = (int)(i % vc); const size_t r = i / vc;
+        const int t = (int)(r % Tpad), b = (int)(r / Tpad);
+        __align__(16) __half o[8];
+        #pragma unroll
+        for (int k = 0; k < 8; k++) {
+            const int c = v * 8 + k;
+            float val = 0.f;
+            if (t <= np) val = (t == 0 ? cls[c] : __half2float(patch[((size_t)b * np + t - 1) * C + c])) + pos[(size_t)t * C + c];
+            o[k] = __float2half_rn(val);
+        }
+        *reinterpret_cast<uint4*>(x + i * 8) = *reinterpret_cast<const uint4*>(o);
+    }
+}
+
+// x[b*Tpad + t] = tok_emb[tokens[b, t]] + pos[t] for t < L; rows L .. Tpad-1 are zero.  Token ids outside [0, vocab) are clamped
+// into it (never read out of bounds).
+__global__ void k_text_embed(const long long* __restrict__ tokens, const float* __restrict__ tok_emb, const float* __restrict__ pos,
+                             __half* __restrict__ x, int B, int L, int Tpad, int C, int vocab) {
+    const int vc = C / 8;
+    const size_t total = (size_t)B * Tpad * vc;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int v = (int)(i % vc); const size_t r = i / vc;
+        const int t = (int)(r % Tpad), b = (int)(r / Tpad);
+        __align__(16) __half o[8];
+        if (t < L) {
+            const long long id = min(max(tokens[(size_t)b * L + t], 0ll), (long long)vocab - 1);
+            #pragma unroll
+            for (int k = 0; k < 8; k++) o[k] = __float2half_rn(tok_emb[(size_t)id * C + v * 8 + k] + pos[(size_t)t * C + v * 8 + k]);
+        } else {
+            #pragma unroll
+            for (int k = 0; k < 8; k++) o[k] = __float2half_rn(0.f);
+        }
+        *reinterpret_cast<uint4*>(x + i * 8) = *reinterpret_cast<const uint4*>(o);
+    }
+}
+
+// out[b] = x[b*Tpad + argmax_t tokens[b, t]] (the first maximum, like torch.argmax): the EOT token's row.  One block per b.
+__global__ void k_text_eot_rows(const long long* __restrict__ tokens, const __half* __restrict__ x, __half* __restrict__ out, int L, int Tpad, int C) {
+    const int b = blockIdx.x;
+    __shared__ int s_arg;
+    if (threadIdx.x == 0) {
+        long long best = tokens[(size_t)b * L]; int arg = 0;
+        for (int t = 1; t < L; t++) { const long long v = tokens[(size_t)b * L + t]; if (v > best) { best = v; arg = t; } }
+        s_arg = arg;
+    }
+    __syncthreads();
+    const __half* src = x + ((size_t)b * Tpad + s_arg) * C;
+    for (int c = threadIdx.x; c < C; c += blockDim.x) out[(size_t)b * C + c] = src[c];
+}
+
+// LayerNorm input gradient, one warp per row (statistics recomputed from x exactly as k_layernorm computes them):
+// dx = rstd * (g - mean(g) - xhat * mean(g * xhat)) (+ add),  g = dy * gamma.
+__global__ void k_layernorm_bwd(const __half* __restrict__ x, const __half* __restrict__ dy, const float* __restrict__ gamma,
+                                const __half* __restrict__ add, __half* __restrict__ dx, int rows, int C, float eps) {
+    const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (row >= rows) return;
+    const __half* xr = x + (size_t)row * C; const __half* dr = dy + (size_t)row * C;
+    float s = 0.f, ss = 0.f;
+    for (int c = lane * 8; c < C; c += 256) {
+        const uint4 raw = *reinterpret_cast<const uint4*>(xr + c);
+        const __half* h = reinterpret_cast<const __half*>(&raw);
+        #pragma unroll
+        for (int k = 0; k < 8; k++) { const float v = __half2float(h[k]); s += v; ss += v * v; }
+    }
+    s = sdk::warp_sum(s); ss = sdk::warp_sum(ss);
+    const float mean = s / C, var = fmaxf(ss / C - mean * mean, 0.f), rstd = rsqrtf(var + eps);
+    float g1 = 0.f, g2 = 0.f;
+    for (int c = lane * 8; c < C; c += 256) {
+        const uint4 rx = *reinterpret_cast<const uint4*>(xr + c), rd = *reinterpret_cast<const uint4*>(dr + c);
+        const __half* hx = reinterpret_cast<const __half*>(&rx); const __half* hd = reinterpret_cast<const __half*>(&rd);
+        #pragma unroll
+        for (int k = 0; k < 8; k++) {
+            const float g = __half2float(hd[k]) * gamma[c + k];
+            g1 += g; g2 += g * (__half2float(hx[k]) - mean) * rstd;
+        }
+    }
+    g1 = sdk::warp_sum(g1) / C; g2 = sdk::warp_sum(g2) / C;
+    for (int c = lane * 8; c < C; c += 256) {
+        const uint4 rx = *reinterpret_cast<const uint4*>(xr + c), rd = *reinterpret_cast<const uint4*>(dr + c);
+        const __half* hx = reinterpret_cast<const __half*>(&rx); const __half* hd = reinterpret_cast<const __half*>(&rd);
+        uint4 ra = make_uint4(0, 0, 0, 0);
+        if (add) ra = *reinterpret_cast<const uint4*>(add + (size_t)row * C + c);
+        const __half* ha = reinterpret_cast<const __half*>(&ra);
+        __align__(16) __half o[8];
+        #pragma unroll
+        for (int k = 0; k < 8; k++) {
+            const float xh = (__half2float(hx[k]) - mean) * rstd;
+            o[k] = __float2half_rn(rstd * (__half2float(hd[k]) * gamma[c + k] - g1 - xh * g2) + __half2float(ha[k]));
+        }
+        *reinterpret_cast<uint4*>(dx + (size_t)row * C + c) = *reinterpret_cast<const uint4*>(o);
+    }
+}
+
+// Causal row softmax in place over [Z][tq][cols] scores: row r (query q = r % tq) keeps keys j <= q (and j < valid); the other
+// columns are written as 0.  One warp per row.
+__global__ void k_softmax_causal(__half* __restrict__ s, size_t rows, int cols, int valid, int tq, float scale) {
+    const size_t row = blockIdx.x * (size_t)(blockDim.x >> 5) + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (row >= rows) return;
+    const int lim = min(valid, (int)(row % tq) + 1);
+    __half* r = s + row * cols;
+    float mx = -INFINITY;
+    for (int c = lane * 8; c < cols; c += 256) {
+        const uint4 raw = *reinterpret_cast<const uint4*>(r + c);
+        const __half* h = reinterpret_cast<const __half*>(&raw);
+        #pragma unroll
+        for (int k = 0; k < 8; k++) if (c + k < lim) mx = fmaxf(mx, __half2float(h[k]) * scale);
+    }
+    mx = sdk::warp_max(mx);
+    float sum = 0.f;
+    for (int c = lane * 8; c < cols; c += 256) {
+        const uint4 raw = *reinterpret_cast<const uint4*>(r + c);
+        const __half* h = reinterpret_cast<const __half*>(&raw);
+        #pragma unroll
+        for (int k = 0; k < 8; k++) if (c + k < lim) sum += __expf(__half2float(h[k]) * scale - mx);
+    }
+    sum = sdk::warp_sum(sum);
+    const float inv = 1.f / sum;
+    for (int c = lane * 8; c < cols; c += 256) {
+        const uint4 raw = *reinterpret_cast<const uint4*>(r + c);
+        const __half* h = reinterpret_cast<const __half*>(&raw);
+        __align__(16) __half o[8];
+        #pragma unroll
+        for (int k = 0; k < 8; k++) o[k] = __float2half_rn(c + k < lim ? __expf(__half2float(h[k]) * scale - mx) * inv : 0.f);
+        *reinterpret_cast<uint4*>(r + c) = *reinterpret_cast<const uint4*>(o);
+    }
+}
+
+}  // namespace clipk

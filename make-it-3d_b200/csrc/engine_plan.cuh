@@ -1,0 +1,212 @@
+// engine_plan.cuh -- the op-builder layer shared by the planned engines (sd_engine.cu, clip_engine.cu).
+//
+// An engine is built twice: a dry run sizes the caller's workspace, the real run carves parameters and activations out of it
+// (bump allocation, nothing is ever freed or reused) and records one closure per launch into static launch lists.  What lives
+// here: the parameter registry, the workspace carving, the op builders over the tile GEMM / fused attention / memory-bound
+// kernels, and the replay of a list as a CUDA graph.
+#pragma once
+#include <functional>
+#include <cstdio>
+#include <cstdlib>
+#include <map>
+#include <memory>
+#include <string>
+#include <vector>
+
+#include "../../include/mi3d.h"
+#include "sd_kernels.cuh"
+#include "tc_host.cuh"
+#include "attn.cuh"
+
+namespace plan {
+
+using Op = std::function<int(cudaStream_t)>;
+
+// How a parameter is stored in the workspace.  The engines' load functions turn the fp32 source tensor into this form.
+enum PKind { PK_F32 = 0, PK_LINEAR, PK_LINEAR_T, PK_LINEAR_BOTH, PK_CONV3, PK_CONV3_BOTH, PK_CONV1, PK_CONV1_BOTH, PK_GEGLU_W, PK_GEGLU_B,
+             PK_CONV_F32_OHWI, PK_CONV_SMALL_COUT, PK_CONV_SMALL_COUT_BOTH };
+
+struct Param {
+    std::string name; std::vector<int> shape; size_t numel = 0; PKind kind = PK_F32;
+    void* dst = nullptr;      // primary storage
+    void* dst2 = nullptr;     // secondary (transposed / flipped copy for the input-gradient pass)
+    std::string partner;      // GEGLU: weight <-> bias handled together
+};
+
+struct Builder {
+    uint8_t* base = nullptr; size_t cap = 0, off = 0; bool dry = true; int err = 0;
+    int num_sms = 132;
+    std::vector<Param> params; std::map<std::string, int> pindex;
+    std::vector<Op>* cur = nullptr;
+    std::map<std::string, std::pair<void*, size_t>> named;   // debug taps: name -> (ptr, bytes)
+    float* splitk_ws = nullptr; size_t splitk_elems = 0;      // fp32 scratch shared by all split-K GEMMs (they run one at a time); 0 = no split-K
+    // optional live timing of the tensor-core tile kernel (bench.py roofline leg): CUDA events around every k_tc_gemm launch
+    bool profile = false; std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_events; size_t prof_used = 0;
+    struct ProfShape { int M, N, K, bn, splits, conv, batch, epi; }; std::vector<ProfShape> prof_shapes;
+    int do_launch(const CUtensorMap& ma, const CUtensorMap& mb, const tc::GemmParams& p, int bn, int batch, cudaStream_t st) {
+        if (p.splits > 1) return tc::launch_splitk(ma, mb, p, bn, p.splits, splitk_ws, st);
+        return tc::launch(ma, mb, p, bn, batch, st);
+    }
+    int timed_launch(const CUtensorMap& ma, const CUtensorMap& mb, const tc::GemmParams& p, int bn, int batch, cudaStream_t st) {
+        if (!profile) return do_launch(ma, mb, p, bn, batch, st);
+        if (prof_used == prof_events.size()) { cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b); prof_events.push_back({a, b}); }
+        if (prof_shapes.size() < prof_events.size()) prof_shapes.resize(prof_events.size());
+        prof_shapes[prof_used] = {p.M, p.N, p.K, bn, p.splits, p.conv, batch, p.epi_mode};
+        auto& ev = prof_events[prof_used++];
+        cudaEventRecord(ev.first, st);
+        const int r = do_launch(ma, mb, p, bn, batch, st);
+        cudaEventRecord(ev.second, st);
+        return r;
+    }
+
+    void* alloc(size_t bytes) {
+        off = (off + 1023) & ~(size_t)1023;
+        void* p = dry ? (void*)(uintptr_t)(0x10000 + off) : (void*)(base + off);
+        off += bytes;
+        if (!dry && off > cap) err = MI3D_ERR_ARG;
+        return p;
+    }
+    __half* alloc16(size_t n) { return (__half*)alloc(n * 2); }
+    float* alloc32(size_t n) { return (float*)alloc(n * 4); }
+    void push(Op op) { if (!dry && cur) cur->push_back(std::move(op)); }
+    void tap(const std::string& name, void* p, size_t bytes) { if (!dry) named[name] = {p, bytes}; }
+
+    Param& param(const std::string& name, std::vector<int> shape, PKind kind) {
+        auto it = pindex.find(name);
+        if (it != pindex.end()) return params[it->second];
+        Param P; P.name = name; P.shape = shape; P.kind = kind; P.numel = 1;
+        for (int s : shape) P.numel *= (size_t)s;
+        switch (kind) {
+            case PK_F32: case PK_GEGLU_B: P.dst = alloc(P.numel * 4); break;
+            case PK_CONV_F32_OHWI: P.dst = alloc((size_t)std::max(shape[0], shape[1]) * 9 * 8 * 4); break;   // input channels padded to <= 8
+            case PK_LINEAR: case PK_CONV3: case PK_CONV1: case PK_GEGLU_W: case PK_LINEAR_T: case PK_CONV_SMALL_COUT: P.dst = alloc(P.numel * 2); break;
+            case PK_LINEAR_BOTH: case PK_CONV3_BOTH: case PK_CONV1_BOTH: case PK_CONV_SMALL_COUT_BOTH:
+                P.dst = alloc(P.numel * 2); P.dst2 = alloc(P.numel * 2); break;
+        }
+        pindex[name] = (int)params.size();
+        params.push_back(P);
+        return params.back();
+    }
+    const float* pf(const std::string& name, std::vector<int> shape) { return (const float*)param(name, shape, PK_F32).dst; }
+
+    // ------------------------------------------------------------------------------------------------------
+    // op builders
+    // ------------------------------------------------------------------------------------------------------
+    struct Mat { const __half* p; long long ld; long long rows; int K; int z1 = 1; long long sz1 = 0; int z2 = 1; long long sz2 = 0; };
+    struct Out { __half* p16 = nullptr; float* p32 = nullptr; long long ldc = 0; int z1 = 1; long long s_lo = 0, s_hi = 0; };
+    struct Epi { const float* bias = nullptr; const float* row_bias = nullptr; int rows_per_group = 1; const __half* residual = nullptr;
+                 long long ld_res = 0; int mode = tc::EPI_PLAIN; float alpha = 1.f; __half* aux = nullptr; };
+
+    void gemm(const Mat& a, const Mat& b, int N, const Out& o, const Epi& e, int batch = 1, bool b_batched = false) {
+        if (dry) return;
+        const long long mt = (a.rows + 127) / 128;
+        int bn = tc::pick_block_n(N, mt * batch, num_sms);
+        if (bn == 0 || a.K % 64) { err = MI3D_ERR_ARG; return; }
+        int splits = 1;
+        if (batch == 1 && e.mode == tc::EPI_PLAIN && o.p16 && a.rows % 128 == 0 && (size_t)a.rows * N <= splitk_elems) {
+            if (N % 128 == 0 && mt * (N / 128) * 2 <= num_sms) bn = 128;            // few, fat tiles + split-K beats many thin tiles
+            splits = tc::plan_splits(mt * (N / bn), a.K / 64, num_sms);
+        }
+        CUtensorMap ma, mb;
+        int r = tc::make_map_matrix(&ma, a.p, a.K, a.rows, a.ld, 128, a.z1, a.sz1, a.z2, a.sz2);
+        if (!r) r = tc::make_map_matrix(&mb, b.p, b.K, b.rows, b.ld, bn, b.z1, b.sz1, b.z2, b.sz2);
+        if (r) { err = r; return; }
+        tc::GemmParams p = {};
+        p.M = (int)a.rows; p.N = N; p.K = a.K; p.num_k_blocks = a.K / 64; p.conv = 0;
+        p.a_z1 = a.z1; p.b_z1 = b.z1; p.b_batched = b_batched ? 1 : 0;
+        p.out = o.p16; p.out_f32 = o.p32; p.ldc = o.ldc; p.out_z1 = o.z1; p.out_s_lo = o.s_lo; p.out_s_hi = o.s_hi;
+        p.bias = e.bias; p.row_bias = e.row_bias; p.rows_per_group = e.rows_per_group; p.residual = e.residual; p.ld_res = e.ld_res;
+        p.epi_mode = e.mode; p.alpha = e.alpha; p.m_valid = (int)a.rows; p.splits = splits; p.aux = e.aux;
+        push([this, ma, mb, p, bn, batch](cudaStream_t st) { return timed_launch(ma, mb, p, bn, batch, st); });
+    }
+
+    // y[M,N] = x[M,K] W[N,K]^T (+bias) (+residual)
+    void linear(const __half* x, long long M, int K, const __half* W, int N, __half* y, const float* bias = nullptr,
+                const __half* residual = nullptr, int mode = tc::EPI_PLAIN, long long ldc = -1) {
+        Mat a{x, K, M, K}; Mat b{W, K, N, K};
+        Out o; o.p16 = y; o.ldc = ldc >= 0 ? ldc : (mode == tc::EPI_GEGLU ? N / 2 : (mode == tc::EPI_TRANSPOSED ? M : N));
+        Epi e; e.bias = bias; e.residual = residual; e.ld_res = N; e.mode = mode;
+        gemm(a, b, N, o, e);
+    }
+
+    void layernorm(const __half* x, long long rows, int C, const std::string& pname, __half* y) {
+        const float* ga = pf(pname + ".weight", {C}); const float* be = pf(pname + ".bias", {C});
+        push([=](cudaStream_t st) {
+            sdk::k_layernorm<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(x, y, ga, be, (int)rows, C, 1e-5f);
+            return (int)cudaGetLastError();
+        });
+    }
+    void softmax(__half* s, size_t rows, int cols, int valid, float scale) {
+        push([=](cudaStream_t st) {
+            sdk::k_softmax<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(s, rows, cols, valid, scale);
+            return (int)cudaGetLastError();
+        });
+    }
+    void transpose(const __half* in, __half* out, int Z, int R, int C) {
+        push([=](cudaStream_t st) {
+            sdk::k_transpose<<<dim3((C + 31) / 32, (R + 31) / 32, Z), dim3(32, 8), 0, st>>>(in, out, R, C);
+            return (int)cudaGetLastError();
+        });
+    }
+    static int blocks_for(size_t n) { return (int)std::min<size_t>((n + 255) / 256, 132 * 16); }
+
+    // multi-head attention core on token matrices (attn.cuh).  q: [B*T, ldq] (head h at column h*64), k / v likewise
+    // [B*Tk, ld]; only the first Tk_valid keys of each batch take part.  Writes o [B*T, C].
+    void attention_core(const __half* q, long long ldq, const __half* k, long long ldk, const __half* v, long long ldv, int B, int T, int Tk,
+                        int Tk_valid, int heads, int d, __half* o, int C) {
+        if (d != 64) { err = MI3D_ERR_ARG; return; }
+        if (dry) return;
+        attn::Maps m;
+        if (int r = attn::make_maps(&m, q, ldq, k, ldk, v, ldv, B, T, Tk, heads)) { err = r; return; }
+        push([=](cudaStream_t st) {
+            if (!profile) return attn::launch(m, o, C, B, T, Tk_valid, heads, st);
+            // profiling: same event bracket as the tile kernel; recorded with conv = 2 (M = queries, N = keys, K = head_dim, batch = B * heads)
+            if (prof_used == prof_events.size()) { cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b); prof_events.push_back({a, b}); }
+            if (prof_shapes.size() < prof_events.size()) prof_shapes.resize(prof_events.size());
+            prof_shapes[prof_used] = {T, Tk_valid, 64, 0, 1, 2, B * heads, 0};
+            auto& ev = prof_events[prof_used++];
+            cudaEventRecord(ev.first, st);
+            const int r = attn::launch(m, o, C, B, T, Tk_valid, heads, st);
+            cudaEventRecord(ev.second, st);
+            return r;
+        });
+    }
+
+    int run_eager(std::vector<Op>& ops, cudaStream_t st) {
+        for (auto& op : ops) { int r = op(st); if (r) return r; }
+        return MI3D_OK;
+    }
+    // The launch lists are static (fixed pointers, shapes and order; every input lives in a device buffer), so a list replays as ONE
+    // CUDA graph from its third call on (the lists lose their CPU launch cost and inter-kernel gaps).  Enabled per engine
+    // (mi3d_sd_set_graph_replay / mi3d_clip_set_graph_replay); needs a capturable stream (torch's legacy default stream is not: the
+    // Python engines run on their own stream, event-ordered against the caller's).  A list whose capture fails falls back to plain
+    // launches for good.
+    struct ListGraph { cudaGraphExec_t exec = nullptr; int calls = 0; bool failed = false; };
+    std::map<std::vector<Op>*, ListGraph> graphs;
+    bool use_graph = false;
+    int run(std::vector<Op>& ops, cudaStream_t st) {
+        ListGraph& g = graphs[&ops];
+        if (!use_graph || profile || g.failed) return run_eager(ops, st);
+        if (g.exec) return (int)cudaGraphLaunch(g.exec, st);
+        if (g.calls++ == 0) return run_eager(ops, st);            // first call: plain launches (one-time function attributes, warm caches)
+        cudaGraph_t graph = nullptr;
+        if (cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) != cudaSuccess) { cudaGetLastError(); g.failed = true; return run_eager(ops, st); }
+        const int r = run_eager(ops, st);
+        const cudaError_t ce = cudaStreamEndCapture(st, &graph);
+        if (r || ce != cudaSuccess || !graph || cudaGraphInstantiate(&g.exec, graph, 0) != cudaSuccess) {
+            cudaGetLastError(); g.failed = true; g.exec = nullptr;
+            if (graph) cudaGraphDestroy(graph);
+            return r ? r : run_eager(ops, st);
+        }
+        cudaGraphDestroy(graph);
+        return (int)cudaGraphLaunch(g.exec, st);
+    }
+    int graph_replays() const {
+        int n = 0;
+        for (auto& kv : graphs) if (kv.second.exec) n++;
+        return n;
+    }
+    ~Builder() { for (auto& kv : graphs) if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec); }
+};
+
+}  // namespace plan

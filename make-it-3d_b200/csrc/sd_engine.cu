@@ -10,22 +10,11 @@
 // mi3d_sd_create(); a step is a fixed sequence of launches on the caller's stream -> CUDA-graph capturable.
 // Activations: NHWC fp16.  Accumulation / statistics: fp32 (fp64 group sums).  Weights: fp16 copies of the fp32
 // diffusers parameters, re-laid-out at load time (conv OIHW -> O,ky,kx,I ; GEGLU rows interleaved ; dgrad copies).
-#include <functional>
-#include <cstdio>
-#include <cstdlib>
-#include <map>
-#include <memory>
-#include <string>
-#include <vector>
-
-#include "../../include/mi3d.h"
-#include "sd_kernels.cuh"
-#include "tc_host.cuh"
-#include "attn.cuh"
+#include "engine_plan.cuh"
 
 namespace sd {
 
-using Op = std::function<int(cudaStream_t)>;
+using namespace plan;
 
 struct T4 {  // NHWC fp16 activation
     __half* p = nullptr; int n = 0, h = 0, w = 0, c = 0;
@@ -33,23 +22,9 @@ struct T4 {  // NHWC fp16 activation
     long long rows() const { return (long long)n * h * w; }
 };
 
-enum PKind { PK_F32 = 0, PK_LINEAR, PK_LINEAR_T, PK_LINEAR_BOTH, PK_CONV3, PK_CONV3_BOTH, PK_CONV1, PK_CONV1_BOTH, PK_GEGLU_W, PK_GEGLU_B,
-             PK_CONV_F32_OHWI, PK_CONV_SMALL_COUT, PK_CONV_SMALL_COUT_BOTH };
-
-struct Param {
-    std::string name; std::vector<int> shape; size_t numel = 0; PKind kind = PK_F32;
-    void* dst = nullptr;      // primary storage
-    void* dst2 = nullptr;     // secondary (transposed / flipped copy for the input-gradient pass)
-    std::string partner;      // GEGLU: weight <-> bias handled together
-};
-
-struct Engine {
+struct Engine : Builder {
     mi3d_unet_cfg ucfg; mi3d_vae_cfg vcfg;
-    uint8_t* base = nullptr; size_t cap = 0, off = 0; bool dry = true; int err = 0;
-    int num_sms = 132;
-    std::vector<Param> params; std::map<std::string, int> pindex;
     std::vector<Op> unet_ops, enc_ops, enc_bwd_ops;
-    std::vector<Op>* cur = nullptr;
     // GroupNorm statistics of one op list live in one pool, cleared by a single memset at the head of the list
     uint8_t* pool = nullptr; size_t pool_used = 0; static constexpr size_t kPoolBytes = 256 * 1024;
     void begin_list(std::vector<Op>* l) {
@@ -64,102 +39,12 @@ struct Engine {
     }
     // per-ResBlock time-embedding projections of the whole U-Net, evaluated by one grouped launch right after the embedding MLP
     std::vector<sdk::SmallLinearJob> temb_jobs; sdk::SmallLinearJob* temb_jobs_dev = nullptr; int temb_max_n = 0;
-    std::map<std::string, std::pair<void*, size_t>> named;   // debug taps: name -> (ptr, bytes)
     // fixed I/O buffers
     T4 unet_in; float* unet_out = nullptr; __half* ctx16 = nullptr; float* temb = nullptr; long long* t_dev = nullptr;
     T4 vae_in; float* vae_moments = nullptr; float* vae_gmoments = nullptr; __half* vae_gin = nullptr;
     T4 dec_in; float* dec_out = nullptr; std::vector<Op> dec_ops;          // VAE decoder (denoise side branch, nerf/sd.py:201-210)
     int ctx_pad = 128;
-    float* splitk_ws = nullptr; size_t splitk_elems = 0;      // fp32 scratch shared by all split-K GEMMs (they run one at a time)
-    // optional live timing of the tensor-core tile kernel (bench.py roofline leg): CUDA events around every k_tc_gemm launch
-    bool profile = false; std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_events; size_t prof_used = 0;
-    struct ProfShape { int M, N, K, bn, splits, conv, batch, epi; }; std::vector<ProfShape> prof_shapes;
-    int do_launch(const CUtensorMap& ma, const CUtensorMap& mb, const tc::GemmParams& p, int bn, int batch, cudaStream_t st) {
-        if (p.splits > 1) return tc::launch_splitk(ma, mb, p, bn, p.splits, splitk_ws, st);
-        return tc::launch(ma, mb, p, bn, batch, st);
-    }
-    int timed_launch(const CUtensorMap& ma, const CUtensorMap& mb, const tc::GemmParams& p, int bn, int batch, cudaStream_t st) {
-        if (!profile) return do_launch(ma, mb, p, bn, batch, st);
-        if (prof_used == prof_events.size()) { cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b); prof_events.push_back({a, b}); }
-        if (prof_shapes.size() < prof_events.size()) prof_shapes.resize(prof_events.size());
-        prof_shapes[prof_used] = {p.M, p.N, p.K, bn, p.splits, p.conv, batch, p.epi_mode};
-        auto& ev = prof_events[prof_used++];
-        cudaEventRecord(ev.first, st);
-        const int r = do_launch(ma, mb, p, bn, batch, st);
-        cudaEventRecord(ev.second, st);
-        return r;
-    }
-
-    void* alloc(size_t bytes) {
-        off = (off + 1023) & ~(size_t)1023;
-        void* p = dry ? (void*)(uintptr_t)(0x10000 + off) : (void*)(base + off);
-        off += bytes;
-        if (!dry && off > cap) err = MI3D_ERR_ARG;
-        return p;
-    }
-    __half* alloc16(size_t n) { return (__half*)alloc(n * 2); }
-    float* alloc32(size_t n) { return (float*)alloc(n * 4); }
     T4 act(int n, int h, int w, int c) { T4 t; t.n = n; t.h = h; t.w = w; t.c = c; t.p = alloc16(t.numel()); return t; }
-    void push(Op op) { if (!dry && cur) cur->push_back(std::move(op)); }
-    void tap(const std::string& name, void* p, size_t bytes) { if (!dry) named[name] = {p, bytes}; }
-
-    Param& param(const std::string& name, std::vector<int> shape, PKind kind) {
-        auto it = pindex.find(name);
-        if (it != pindex.end()) return params[it->second];
-        Param P; P.name = name; P.shape = shape; P.kind = kind; P.numel = 1;
-        for (int s : shape) P.numel *= (size_t)s;
-        switch (kind) {
-            case PK_F32: case PK_GEGLU_B: P.dst = alloc(P.numel * 4); break;
-            case PK_CONV_F32_OHWI: P.dst = alloc((size_t)std::max(shape[0], shape[1]) * 9 * 8 * 4); break;   // input channels padded to <= 8
-            case PK_LINEAR: case PK_CONV3: case PK_CONV1: case PK_GEGLU_W: case PK_LINEAR_T: case PK_CONV_SMALL_COUT: P.dst = alloc(P.numel * 2); break;
-            case PK_LINEAR_BOTH: case PK_CONV3_BOTH: case PK_CONV1_BOTH: case PK_CONV_SMALL_COUT_BOTH:
-                P.dst = alloc(P.numel * 2); P.dst2 = alloc(P.numel * 2); break;
-        }
-        pindex[name] = (int)params.size();
-        params.push_back(P);
-        return params.back();
-    }
-    const float* pf(const std::string& name, std::vector<int> shape) { return (const float*)param(name, shape, PK_F32).dst; }
-
-    // ------------------------------------------------------------------------------------------------------
-    // op builders
-    // ------------------------------------------------------------------------------------------------------
-    struct Mat { const __half* p; long long ld; long long rows; int K; int z1 = 1; long long sz1 = 0; int z2 = 1; long long sz2 = 0; };
-    struct Out { __half* p16 = nullptr; float* p32 = nullptr; long long ldc = 0; int z1 = 1; long long s_lo = 0, s_hi = 0; };
-    struct Epi { const float* bias = nullptr; const float* row_bias = nullptr; int rows_per_group = 1; const __half* residual = nullptr;
-                 long long ld_res = 0; int mode = tc::EPI_PLAIN; float alpha = 1.f; };
-
-    void gemm(const Mat& a, const Mat& b, int N, const Out& o, const Epi& e, int batch = 1, bool b_batched = false) {
-        if (dry) return;
-        const long long mt = (a.rows + 127) / 128;
-        int bn = tc::pick_block_n(N, mt * batch, num_sms);
-        if (bn == 0 || a.K % 64) { err = MI3D_ERR_ARG; return; }
-        int splits = 1;
-        if (batch == 1 && e.mode == tc::EPI_PLAIN && o.p16 && a.rows % 128 == 0 && (size_t)a.rows * N <= splitk_elems) {
-            if (N % 128 == 0 && mt * (N / 128) * 2 <= num_sms) bn = 128;            // few, fat tiles + split-K beats many thin tiles
-            splits = tc::plan_splits(mt * (N / bn), a.K / 64, num_sms);
-        }
-        CUtensorMap ma, mb;
-        int r = tc::make_map_matrix(&ma, a.p, a.K, a.rows, a.ld, 128, a.z1, a.sz1, a.z2, a.sz2);
-        if (!r) r = tc::make_map_matrix(&mb, b.p, b.K, b.rows, b.ld, bn, b.z1, b.sz1, b.z2, b.sz2);
-        if (r) { err = r; return; }
-        tc::GemmParams p = {};
-        p.M = (int)a.rows; p.N = N; p.K = a.K; p.num_k_blocks = a.K / 64; p.conv = 0;
-        p.a_z1 = a.z1; p.b_z1 = b.z1; p.b_batched = b_batched ? 1 : 0;
-        p.out = o.p16; p.out_f32 = o.p32; p.ldc = o.ldc; p.out_z1 = o.z1; p.out_s_lo = o.s_lo; p.out_s_hi = o.s_hi;
-        p.bias = e.bias; p.row_bias = e.row_bias; p.rows_per_group = e.rows_per_group; p.residual = e.residual; p.ld_res = e.ld_res;
-        p.epi_mode = e.mode; p.alpha = e.alpha; p.m_valid = (int)a.rows; p.splits = splits;
-        push([this, ma, mb, p, bn, batch](cudaStream_t st) { return timed_launch(ma, mb, p, bn, batch, st); });
-    }
-
-    // y[M,N] = x[M,K] W[N,K]^T (+bias) (+residual)
-    void linear(const __half* x, long long M, int K, const __half* W, int N, __half* y, const float* bias = nullptr,
-                const __half* residual = nullptr, int mode = tc::EPI_PLAIN, long long ldc = -1) {
-        Mat a{x, K, M, K}; Mat b{W, K, N, K};
-        Out o; o.p16 = y; o.ldc = ldc >= 0 ? ldc : (mode == tc::EPI_GEGLU ? N / 2 : (mode == tc::EPI_TRANSPOSED ? M : N));
-        Epi e; e.bias = bias; e.residual = residual; e.ld_res = N; e.mode = mode;
-        gemm(a, b, N, o, e);
-    }
 
     // 3x3 stride-1 pad-1 conv via implicit GEMM; w [Cout][3][3][Cin] fp16
     void conv3(const T4& x, const __half* w, int Cout, const T4& y, const float* bias, const float* row_bias = nullptr,
@@ -223,32 +108,12 @@ struct Engine {
             return (int)cudaGetLastError();
         });
     }
-    void layernorm(const __half* x, long long rows, int C, const std::string& pname, __half* y) {
-        const float* ga = pf(pname + ".weight", {C}); const float* be = pf(pname + ".bias", {C});
-        push([=](cudaStream_t st) {
-            sdk::k_layernorm<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(x, y, ga, be, (int)rows, C, 1e-5f);
-            return (int)cudaGetLastError();
-        });
-    }
-    void softmax(__half* s, size_t rows, int cols, int valid, float scale) {
-        push([=](cudaStream_t st) {
-            sdk::k_softmax<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(s, rows, cols, valid, scale);
-            return (int)cudaGetLastError();
-        });
-    }
-    void transpose(const __half* in, __half* out, int Z, int R, int C) {
-        push([=](cudaStream_t st) {
-            sdk::k_transpose<<<dim3((C + 31) / 32, (R + 31) / 32, Z), dim3(32, 8), 0, st>>>(in, out, R, C);
-            return (int)cudaGetLastError();
-        });
-    }
     void linear_small(const float* x, const __half* w, const float* bias, float* y, int B, int N, int K, int silu_in, int silu_out) {
         push([=](cudaStream_t st) {
             sdk::k_linear_small<<<(N + 7) / 8, 256, 0, st>>>(x, w, bias, y, B, N, K, silu_in, silu_out);
             return (int)cudaGetLastError();
         });
     }
-    static int blocks_for(size_t n) { return (int)std::min<size_t>((n + 255) / 256, 132 * 16); }
     // persistent grids of the small direct convolutions: as many CTAs per SM as their weight staging area allows
     int small_cin_grid(size_t outputs, size_t smem) const { const int per_sm = (int)std::max<size_t>(1, std::min<size_t>(8, (200 * 1024) / std::max<size_t>(smem, 1))); return (int)std::min<size_t>((outputs / 8 + 255) / 256, (size_t)num_sms * per_sm); }
     int small_cout_grid(size_t pixels, int cin) const { const int ppw = cin <= 128 ? 2 : 1; return (int)std::min<size_t>((pixels / ppw + 7) / 8 + 1, (size_t)num_sms * 8); }
@@ -289,28 +154,6 @@ struct Engine {
         if (tape) { tape->push_back(g1); tape->push_back(g2); }
         if (acts) { acts->push_back(a1); acts->push_back(a2); }
         return out;
-    }
-
-    // multi-head attention core on token matrices (attn.cuh).  q: [B*T, ldq] (head h at column h*64), k / v likewise
-    // [B*Tk, ld]; only the first Tk_valid keys of each batch take part.  Writes o [B*T, C].
-    void attention_core(const __half* q, long long ldq, const __half* k, long long ldk, const __half* v, long long ldv, int B, int T, int Tk,
-                        int Tk_valid, int heads, int d, __half* o, int C) {
-        if (d != 64) { err = MI3D_ERR_ARG; return; }
-        if (dry) return;
-        attn::Maps m;
-        if (int r = attn::make_maps(&m, q, ldq, k, ldk, v, ldv, B, T, Tk, heads)) { err = r; return; }
-        push([=](cudaStream_t st) {
-            if (!profile) return attn::launch(m, o, C, B, T, Tk_valid, heads, st);
-            // profiling: same event bracket as the tile kernel; recorded with conv = 2 (M = queries, N = keys, K = head_dim, batch = B * heads)
-            if (prof_used == prof_events.size()) { cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b); prof_events.push_back({a, b}); }
-            if (prof_shapes.size() < prof_events.size()) prof_shapes.resize(prof_events.size());
-            prof_shapes[prof_used] = {T, Tk_valid, 64, 0, 1, 2, B * heads, 0};
-            auto& ev = prof_events[prof_used++];
-            cudaEventRecord(ev.first, st);
-            const int r = attn::launch(m, o, C, B, T, Tk_valid, heads, st);
-            cudaEventRecord(ev.second, st);
-            return r;
-        });
     }
 
     T4 transformer(const std::string& pre, const T4& x, int heads) {
@@ -847,36 +690,6 @@ struct Engine {
         if (vcfg.n_levels > 0) { build_vae(); build_vae_bwd(); if (vcfg.decoder) build_vae_dec(); }
         return err;
     }
-
-    int run_eager(std::vector<Op>& ops, cudaStream_t st) {
-        for (auto& op : ops) { int r = op(st); if (r) return r; }
-        return MI3D_OK;
-    }
-    // The launch lists are static (fixed pointers, shapes and order; the timestep and every input live in device buffers), so a list
-    // replays as ONE CUDA graph from its third call on (~200-330 launches lose their CPU launch cost and inter-kernel gaps).  Enabled per engine with
-    // mi3d_sd_set_graph_replay(); needs a capturable stream (torch's legacy default stream is not: nerf/sd.py runs the engine on its
-    // own stream, event-ordered against the caller's).  A list whose capture fails falls back to plain launches for good.
-    struct ListGraph { cudaGraphExec_t exec = nullptr; int calls = 0; bool failed = false; };
-    std::map<std::vector<Op>*, ListGraph> graphs;
-    bool use_graph = false;
-    int run(std::vector<Op>& ops, cudaStream_t st) {
-        ListGraph& g = graphs[&ops];
-        if (!use_graph || profile || g.failed) return run_eager(ops, st);
-        if (g.exec) return (int)cudaGraphLaunch(g.exec, st);
-        if (g.calls++ == 0) return run_eager(ops, st);            // first call: plain launches (one-time function attributes, warm caches)
-        cudaGraph_t graph = nullptr;
-        if (cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) != cudaSuccess) { cudaGetLastError(); g.failed = true; return run_eager(ops, st); }
-        const int r = run_eager(ops, st);
-        const cudaError_t ce = cudaStreamEndCapture(st, &graph);
-        if (r || ce != cudaSuccess || !graph || cudaGraphInstantiate(&g.exec, graph, 0) != cudaSuccess) {
-            cudaGetLastError(); g.failed = true; g.exec = nullptr;
-            if (graph) cudaGraphDestroy(graph);
-            return r ? r : run_eager(ops, st);
-        }
-        cudaGraphDestroy(graph);
-        return (int)cudaGraphLaunch(g.exec, st);
-    }
-    ~Engine() { for (auto& kv : graphs) if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec); }
 };
 
 // ------------------------------------------------------------------------------------------------------------

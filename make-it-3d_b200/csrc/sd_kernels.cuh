@@ -7,6 +7,7 @@
 #include <stdint.h>
 
 namespace sdk {
+namespace {   // internal linkage: every engine's translation unit includes these kernels
 
 __device__ __forceinline__ float silu(float x) { return x / (1.f + __expf(-x)); }
 __device__ __forceinline__ float silu_grad(float x) { const float s = 1.f / (1.f + __expf(-x)); return s * (1.f + x * (1.f - s)); }
@@ -608,4 +609,5 @@ __global__ void k_time_proj(const long long* __restrict__ t, float* __restrict__
     out[(size_t)b * dim + half + j] = sinf(a);
 }
 
+}  // namespace
 }  // namespace sdk

@@ -29,7 +29,10 @@ constexpr int BLOCK_K = 64;          // 64 fp16 = 128 B = one swizzle-128B atom 
 constexpr int MMA_K = 16;
 constexpr int kThreads = 384;
 
-enum EpiMode : int { EPI_PLAIN = 0, EPI_GEGLU = 1, EPI_TRANSPOSED = 2 };
+// EPI_QUICKGELU: out = y * sigmoid(1.702 y) (CLIP's MLP activation), y = alpha * acc + bias; the pre-activation y is also stored to aux
+//                when aux is set (the input-gradient pass needs it).
+// EPI_QUICKGELU_BWD: out = y * QuickGELU'(aux), aux = the saved pre-activation (same layout as out).
+enum EpiMode : int { EPI_PLAIN = 0, EPI_GEGLU = 1, EPI_TRANSPOSED = 2, EPI_QUICKGELU = 3, EPI_QUICKGELU_BWD = 4 };
 
 struct GemmParams {
     int M, N, K;                 // per-batch extents; N multiple of BLOCK_N, K multiple of 64, M multiple of 128 (rows may be padded)
@@ -56,6 +59,7 @@ struct GemmParams {
     int splits, kb_per_split;     // split-K: work item t -> (t % splits) K-range, partial sums RED-added (fp32) into splitk_ws[M][N]
     float* splitk_ws;
     int m_tiles, n_tiles, num_tiles;   // persistent tile loop: tile t -> n_blk = t % n_tiles, m_blk = (t / n_tiles) % m_tiles, z = t / (n_tiles * m_tiles)
+    __half* aux;                 // QuickGELU modes: pre-activation, same layout as out
 };
 
 // ----------------------------------------------------------------------------------------------------------------
@@ -116,6 +120,8 @@ template <int BLOCK_N> struct Cfg {
 };
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
+__device__ __forceinline__ float quick_gelu(float x) { return x / (1.f + __expf(-1.702f * x)); }
+__device__ __forceinline__ float quick_gelu_grad(float x) { const float s = 1.f / (1.f + __expf(-1.702f * x)); return s * (1.f + 1.702f * x * (1.f - s)); }
 
 // acc (+)= A[64 x 16] . B[BLOCK_N x 16]^T ; TB = 1: B is MN-major
 template <int BLOCK_N, int TB>
@@ -126,7 +132,8 @@ __device__ __forceinline__ void mma_tile(float (&acc)[BLOCK_N / 2], uint64_t da,
     else wg::wgmma_f16_n256<0, TB>(acc, da, db, accumulate);
 }
 
-template <int BLOCK_N>
+// kQuickGelu: the instantiation that also carries the EPI_QUICKGELU* epilogues (the other modes compile exactly as without them)
+template <int BLOCK_N, bool kQuickGelu = false>
 __global__ void __launch_bounds__(kThreads, Cfg<BLOCK_N>::kMinBlocks)
 k_tc_gemm(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmParams p) {
     using C = Cfg<BLOCK_N>;
@@ -250,6 +257,14 @@ k_tc_gemm(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
                     } else if (p.epi_mode == EPI_TRANSPOSED) {
                         __half* o = p.out + zoff + (size_t)n * p.ldc + m;
                         o[0] = __float2half_rn(f0); o[p.ldc] = __float2half_rn(f1);
+                    } else if (kQuickGelu && p.epi_mode == EPI_QUICKGELU) {
+                        const size_t o = zoff + (size_t)m * p.ldc + n;
+                        if (p.aux) *reinterpret_cast<__half2*>(p.aux + o) = __floats2half2_rn(f0, f1);
+                        *reinterpret_cast<__half2*>(p.out + o) = __floats2half2_rn(quick_gelu(f0), quick_gelu(f1));
+                    } else if (kQuickGelu && p.epi_mode == EPI_QUICKGELU_BWD) {
+                        const size_t o = zoff + (size_t)m * p.ldc + n;
+                        const __half2 pre = *reinterpret_cast<const __half2*>(p.aux + o);
+                        *reinterpret_cast<__half2*>(p.out + o) = __floats2half2_rn(f0 * quick_gelu_grad(__low2float(pre)), f1 * quick_gelu_grad(__high2float(pre)));
                     } else {
                         if (p.residual) {
                             const __half2 rv = *reinterpret_cast<const __half2*>(p.residual + zoff + (size_t)m * p.ld_res + n);

@@ -10,8 +10,9 @@ Weights: parameters are enumerated by diffusers' state_dict names; real SD-2.0-b
 `load_diffusers_state_dict(unet_state, vae_state)` (which also pushes them into the engine); offline (no network, no weights on disk) they are seeded random tensors with PyTorch's default
 initialisers -- which is what the benchmark and the parity tests use (`data: synthetic`).
 The "denoise" side branch (nerf/sd.py:153-159: DDIM step t -> t-1, VAE decode, CLIP losses) is built on the same engine (`mi3d_sd_ddim_step`,
-`mi3d_sd_decode`); the CLIP losses run on a caller-provided clip_model (the reference passes it in too) and are skipped without one.
-What is NOT built (SURVEY.md 8f rank 3): the CLIP text encoder behind `get_text_embeds` (deterministic stand-in) and CLIP itself.
+`mi3d_sd_decode`); the CLIP losses run on the caller-provided clip_model (the reference passes it in too) and are skipped without one.
+A native `nerf.clip.CLIP` computes them on the CLIP engine (csrc/clip_engine.cu, aug included); any other model is called as before.
+What is NOT built (SURVEY.md 8f rank 3): the OpenCLIP text encoder behind `get_text_embeds` (deterministic stand-in).
 """
 import contextlib
 import ctypes as C
@@ -23,6 +24,7 @@ import torch
 import torch.nn as nn
 
 from .. import _lib as L
+from .clip import CLIP
 
 
 class UNetCfg(C.Structure):
@@ -315,7 +317,10 @@ class StableDiffusion(nn.Module):
         de_latents = self.ddim_prev_sample(noise_pred, latents_noisy, self._t)
         imgs = self.decode_latents(de_latents)
         loss = 0
-        if clip_model is not None:
+        if isinstance(clip_model, CLIP):
+            img_loss, text_loss = clip_model.losses(imgs, ref_rgb, ref_text)
+            loss = 10 * img_loss + 10 * text_loss
+        elif clip_model is not None:
             aug = getattr(self, "aug", None)
             loss = 10 * self.img_clip_loss(clip_model, imgs, ref_rgb, aug) + 10 * self.img_text_clip_loss(clip_model, imgs, ref_text, aug)
         return loss, imgs
