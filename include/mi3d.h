@@ -506,6 +506,34 @@ int mi3d_clip_encode_image_backward(mi3d_clip_t h, const float* dfeats, int n_gr
  * [B,embed_dim] (encode_text, causal attention).  Ids outside [0, vocab) are clamped into it. */
 int mi3d_clip_encode_text(mi3d_clip_t h, const long long* tokens, int B, float* feats, mi3d_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------
+ * B5: refine-stage point renderer  (replaces pytorch3d's rasterize_points + alpha_composite as render_point drives them,
+ * nerf/refine_utils.py:306-333, and the Python loop of z_buffer, refine_utils.py:167-208)
+ * ------------------------------------------------------------------------------------------------------ */
+/* HOST: workspace bytes of mi3d_points_render_forward for P points rasterised at H x W with NDC radius `radius` (0: invalid
+ * arguments).  The bin lists are sized from a bound on the screen tiles one point can touch, so they cannot overflow. */
+size_t mi3d_points_workspace_bytes(uint32_t P, uint32_t H, uint32_t W, double radius);
+/* points [P,3], feats [P,C] (C in 1..32) fp32; cam_k [9] (row-major K) and world2cam [12] (rows 0..2 of the pose, R | t) are DEVICE
+ * fp32 buffers.  Projection: c = R p + t, q = K c, u = q.x / q.z, x_ndc = -(u / proj_w * 2 - 1) (same for y with proj_h), z = q.z.
+ * Naive pytorch3d rasterisation of an H x W image (H == W, else MI3D_ERR_ARG): pixel (y, x) has the NDC centre
+ * (-1 + (2(W-1-x)+1)/W, -1 + (2(H-1-y)+1)/H); a point with z >= 0 covers it when dist2 < r*r (fp32 r = radius); each pixel keeps the
+ * K (1..16) covering points with the smallest (z, index), ascending, empty slots -1.  alpha = 1 - sqrt(clamp(0.1 dist2 / fp32(radius^2),
+ * 1e-3, 1)); image [1,C,H,W] = front-to-back alpha composite over the slots, background 0.
+ * Outputs [H,W,K]: idx (required), w = T * alpha (the backward's weights; required with image), zbuf / dist2 (nullable, -1 when empty).
+ * image == NULL rasterises only (feats unused).  workspace: mi3d_points_workspace_bytes() bytes. */
+int mi3d_points_render_forward(const float* points, const float* feats, uint32_t P, uint32_t C, const float* cam_k, const float* world2cam,
+                               float proj_w, float proj_h, uint32_t H, uint32_t W, double radius, uint32_t K, float* image, int* idx,
+                               float* w, float* zbuf, float* dist2, void* workspace, size_t workspace_bytes, mi3d_stream_t stream);
+/* grad_feats [P,C] (overwritten) = sum over the (pixel, slot) pairs holding each point of grad_image[c, pixel] * w; idx / w from the
+ * forward with the same points and camera.  No gradient for points, radius or background (the reference requests none). */
+int mi3d_points_render_backward(const float* points, uint32_t P, uint32_t C, const float* cam_k, const float* world2cam, float proj_w,
+                                float proj_h, uint32_t H, uint32_t W, double radius, uint32_t K, const int* idx, const float* w,
+                                const float* grad_image, float* grad_feats, mi3d_stream_t stream);
+/* z_buffer visibility in fp64: project points [P,3] with DEVICE cam_k [9] / world2cam [12], (x, y) = rint(u, v) (half to even);
+ * mask[i] (uint8) = in image && !(z_i - min z of the in-image points in that pixel > 1/H).  zbuf: DEVICE scratch of H*W uint64. */
+int mi3d_points_zbuffer_visible(const double* points, uint32_t P, const double* cam_k, const double* world2cam, uint32_t H, uint32_t W,
+                                unsigned long long* zbuf, uint8_t* mask, mi3d_stream_t stream);
+
 /* unit-test entry for the hand-written wgmma tf32 tiles of the field forward (3-term split, K-major operands):
  * mode 0 (the only one): d[128,N] = a[128,K] . b[N,K]^T, N in {16, 32, 64}, K in {32, 64, 96, 128}.  fp32 in/out. */
 int mi3d_tf32_tile_test(const float* a, const float* b, float* d, int N, int K, int mode, mi3d_stream_t stream);
