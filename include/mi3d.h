@@ -534,6 +534,41 @@ int mi3d_points_render_backward(const float* points, uint32_t P, uint32_t C, con
 int mi3d_points_zbuffer_visible(const double* points, uint32_t P, const double* cam_k, const double* world2cam, uint32_t H, uint32_t W,
                                 unsigned long long* zbuf, uint8_t* mask, mi3d_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------
+ * B6: refine-stage contextual loss  (replaces the contextual_loss package's ContextualLoss(use_vgg=True, vgg_layer='relu5_4',
+ * loss_type='cosine'), nerf/utils.py:36, 455-457, 810, 882)
+ * ------------------------------------------------------------------------------------------------------ */
+typedef struct {
+    int N, H, W;               /* images per call (1..16) and their size (16..4096 each): the plan is static for this shape */
+} mi3d_cx_cfg;
+
+typedef struct mi3d_cx* mi3d_cx_t;
+
+/* HOST: bytes of device workspace the engine needs (0: invalid configuration); create plans inside it, NULL on failure */
+size_t mi3d_cx_workspace_bytes(const mi3d_cx_cfg* cfg);
+mi3d_cx_t mi3d_cx_create(const mi3d_cx_cfg* cfg, void* workspace, size_t workspace_bytes);
+void mi3d_cx_destroy(mi3d_cx_t h);
+/* Parameters carry the package's state_dict names, "vgg_model.slice1.0.weight" .. "vgg_model.slice5.34.bias" (a '#dgrad' suffix
+ * marks a derived copy, written when its base tensor is loaded).  load: src = fp32 DEVICE tensor in torch's layout. */
+int mi3d_cx_num_params(mi3d_cx_t h);
+const char* mi3d_cx_param_name(mi3d_cx_t h, int i);
+int mi3d_cx_param_shape(mi3d_cx_t h, int i, int* shape4); /* returns rank */
+int mi3d_cx_load_param(mi3d_cx_t h, int i, const float* src, mi3d_stream_t stream);
+/* CUDA-graph replay of the static launch lists, from a list's third call on (`stream` must then be capturable); off by default.
+ * mi3d_cx_graph_replays: lists currently instantiated. */
+int mi3d_cx_set_graph_replay(mi3d_cx_t h, int enable);
+int mi3d_cx_graph_replays(mi3d_cx_t h);
+/* x, y fp32 [N,3,H,W] -> loss: DEVICE fp32 scalar.  ImageNet normalisation, VGG19 features[0:36] of x and y in one batched pass
+ * (fp16 storage, fp32 accumulation), then in fp32: centring by y's channel mean over batch and positions, L2 normalisation,
+ * d = 1 - cos, d / (min_j d + 1e-5), w = exp((1 - .) / band_width), cx = w / sum_j w, loss = mean_n -log(mean_j max_i cx + 1e-5).
+ * need_grad != 0 keeps the tape for mi3d_cx_backward; any forward replaces it. */
+int mi3d_cx_forward(mi3d_cx_t h, const float* x, const float* y, float band_width, int need_grad, float* loss, mi3d_stream_t stream);
+/* dx fp32 [N,3,H,W] (overwritten) = dloss * d loss / d x of the last forward; dloss: DEVICE fp32 scalar.  No gradient for y or the
+ * weights.  MI3D_ERR_ARG without a tape. */
+int mi3d_cx_backward(mi3d_cx_t h, const float* dloss, float* dx, mi3d_stream_t stream);
+/* debug tap: device pointer + size of a named intermediate ("relu5_4": fp16 NHWC [2N,H/16,W/16,512], the x images first) */
+int mi3d_cx_debug_tensor(mi3d_cx_t h, const char* name, void** ptr, size_t* bytes);
+
 /* unit-test entry for the hand-written wgmma tf32 tiles of the field forward (3-term split, K-major operands):
  * mode 0 (the only one): d[128,N] = a[128,K] . b[N,K]^T, N in {16, 32, 64}, K in {32, 64, 96, 128}.  fp32 in/out. */
 int mi3d_tf32_tile_test(const float* a, const float* b, float* d, int N, int K, int mode, mi3d_stream_t stream);

@@ -1,4 +1,4 @@
-// engine_plan.cuh -- the op-builder layer shared by the planned engines (sd_engine.cu, clip_engine.cu).
+// engine_plan.cuh -- the op-builder layer shared by the planned engines (sd_engine.cu, clip_engine.cu, cx_engine.cu).
 //
 // An engine is built twice: a dry run sizes the caller's workspace, the real run carves parameters and activations out of it
 // (bump allocation, nothing is ever freed or reused) and records one closure per launch into static launch lists.  What lives
@@ -31,6 +31,12 @@ struct Param {
     void* dst = nullptr;      // primary storage
     void* dst2 = nullptr;     // secondary (transposed / flipped copy for the input-gradient pass)
     std::string partner;      // GEGLU: weight <-> bias handled together
+};
+
+struct T4 {  // NHWC fp16 activation
+    __half* p = nullptr; int n = 0, h = 0, w = 0, c = 0;
+    size_t numel() const { return (size_t)n * h * w * c; }
+    long long rows() const { return (long long)n * h * w; }
 };
 
 struct Builder {
@@ -129,6 +135,67 @@ struct Builder {
         gemm(a, b, N, o, e);
     }
 
+    T4 act(int n, int h, int w, int c) { T4 t; t.n = n; t.h = h; t.w = w; t.c = c; t.p = alloc16(t.numel()); return t; }
+
+    // 3x3 stride-1 pad-1 conv via implicit GEMM; w [Cout][3][3][Cin] fp16
+    void conv3(const T4& x, const __half* w, int Cout, const T4& y, const float* bias, const float* row_bias = nullptr,
+               const __half* residual = nullptr) {
+        if (dry) return;
+        const long long M = x.rows();
+        int bw = x.w < 128 ? x.w : 128, bh = 128 / bw; if (bh > x.h) bh = x.h; const int bn_img = 128 / (bw * bh);
+        if (M % 128 || x.c % 64 || bw * bh * bn_img != 128 || x.w % bw || x.h % bh || x.n % bn_img) { err = MI3D_ERR_ARG; return; }
+        int bn = tc::pick_block_n(Cout, M / 128, num_sms);
+        if (!bn) { err = MI3D_ERR_ARG; return; }
+        int splits = 1;
+        if ((size_t)M * Cout <= splitk_elems) {
+            if (Cout % 128 == 0 && (M / 128) * (Cout / 128) * 2 <= num_sms) bn = 128;
+            splits = tc::plan_splits((M / 128) * (Cout / bn), 9 * (x.c / 64), num_sms);
+        }
+        CUtensorMap ma, mb;
+        int r = tc::make_map_nhwc(&ma, x.p, x.c, x.w, x.h, x.n, bw, bh, bn_img);
+        if (!r) r = tc::make_map_matrix(&mb, w, 9ull * x.c, Cout, 9ull * x.c, bn);
+        if (r) { err = r; return; }
+        tc::GemmParams p = {};
+        p.M = (int)M; p.N = Cout; p.K = 9 * x.c; p.num_k_blocks = 9 * (x.c / 64); p.conv = 1;
+        p.conv_H = x.h; p.conv_W = x.w; p.conv_bw = bw; p.conv_bh = bh; p.cin_blocks = x.c / 64;
+        p.a_z1 = 1; p.b_z1 = 1; p.b_batched = 0; p.out = y.p; p.ldc = Cout; p.out_z1 = 1;
+        p.bias = bias; p.row_bias = row_bias; p.rows_per_group = x.h * x.w; p.residual = residual; p.ld_res = Cout;
+        p.epi_mode = tc::EPI_PLAIN; p.alpha = 1.f; p.m_valid = (int)M; p.splits = splits;
+        push([this, ma, mb, p, bn](cudaStream_t st) { return timed_launch(ma, mb, p, bn, 1, st); });
+    }
+
+    // dgrad of a stride-1 3x3 conv: dx = conv3(dy, W_flipped^T)  (+ residual accumulation)
+    void conv3_dgrad(const T4& dy, const std::string& wname, int cin, const T4& dx, const __half* add = nullptr) {
+        Param& w = params[pindex[wname]];
+        conv3(dy, (const __half*)w.dst2, cin, dx, nullptr, nullptr, add);
+    }
+
+    // The same conv for any H x W (VGG's levels): each 128-row tile is a bw x bh block of one image (the shape that wastes the
+    // fewest rows over the image edge), overhanging tiles load zeros and store only in-image pixels.  mode: EPI_PLAIN, EPI_RELU, or
+    // EPI_RELU_BWD with aux = the mask source.  No split-K (its fp32 RED order varies run to run).
+    void conv3_block(const T4& x, const __half* w, int Cout, const T4& y, const float* bias, int mode, const __half* aux = nullptr) {
+        if (dry) return;
+        if (x.c % 64 || Cout % 64 || y.n != x.n || y.h != x.h || y.w != x.w || y.c != Cout) { err = MI3D_ERR_ARG; return; }
+        int bw = 128, bh = 1; long long best = -1;
+        for (int cw = 8; cw <= 128; cw *= 2) {
+            const long long area = (long long)((x.w + cw - 1) / cw) * cw * ((x.h + 128 / cw - 1) / (128 / cw)) * (128 / cw);
+            if (best < 0 || area < best) { best = area; bw = cw; bh = 128 / cw; }
+        }
+        const long long tiles = (long long)x.n * ((x.w + bw - 1) / bw) * ((x.h + bh - 1) / bh);
+        const int bn = tc::pick_block_n(Cout, tiles, num_sms);
+        if (!bn) { err = MI3D_ERR_ARG; return; }
+        CUtensorMap ma, mb;
+        int r = tc::make_map_nhwc(&ma, x.p, x.c, x.w, x.h, x.n, bw, bh, 1);
+        if (!r) r = tc::make_map_matrix(&mb, w, 9ull * x.c, Cout, 9ull * x.c, bn);
+        if (r) { err = r; return; }
+        tc::GemmParams p = {};
+        p.M = (int)(tiles * 128); p.N = Cout; p.K = 9 * x.c; p.num_k_blocks = 9 * (x.c / 64); p.conv = 2;
+        p.conv_H = x.h; p.conv_W = x.w; p.conv_bw = bw; p.conv_bh = bh; p.cin_blocks = x.c / 64;
+        p.a_z1 = 1; p.b_z1 = 1; p.b_batched = 0; p.out = y.p; p.ldc = Cout; p.out_z1 = 1;
+        p.bias = bias; p.rows_per_group = 1; p.epi_mode = mode; p.alpha = 1.f; p.m_valid = (int)x.rows(); p.splits = 1; p.aux = const_cast<__half*>(aux);
+        push([this, ma, mb, p, bn](cudaStream_t st) { return timed_launch(ma, mb, p, bn, 1, st); });
+    }
+
     void layernorm(const __half* x, long long rows, int C, const std::string& pname, __half* y) {
         const float* ga = pf(pname + ".weight", {C}); const float* be = pf(pname + ".bias", {C});
         push([=](cudaStream_t st) {
@@ -148,6 +215,9 @@ struct Builder {
             return (int)cudaGetLastError();
         });
     }
+    // persistent grids of the small direct convolutions: as many CTAs per SM as their weight staging area allows
+    int small_cin_grid(size_t outputs, size_t smem) const { const int per_sm = (int)std::max<size_t>(1, std::min<size_t>(8, (200 * 1024) / std::max<size_t>(smem, 1))); return (int)std::min<size_t>((outputs / 8 + 255) / 256, (size_t)num_sms * per_sm); }
+    int small_cout_grid(size_t pixels, int cin) const { const int ppw = cin <= 128 ? 2 : 1; return (int)std::min<size_t>((pixels / ppw + 7) / 8 + 1, (size_t)num_sms * 8); }
     static int blocks_for(size_t n) { return (int)std::min<size_t>((n + 255) / 256, 132 * 16); }
 
     // multi-head attention core on token matrices (attn.cuh).  q: [B*T, ldq] (head h at column h*64), k / v likewise

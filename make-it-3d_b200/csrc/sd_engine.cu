@@ -16,12 +16,6 @@ namespace sd {
 
 using namespace plan;
 
-struct T4 {  // NHWC fp16 activation
-    __half* p = nullptr; int n = 0, h = 0, w = 0, c = 0;
-    size_t numel() const { return (size_t)n * h * w * c; }
-    long long rows() const { return (long long)n * h * w; }
-};
-
 struct Engine : Builder {
     mi3d_unet_cfg ucfg; mi3d_vae_cfg vcfg;
     std::vector<Op> unet_ops, enc_ops, enc_bwd_ops;
@@ -44,34 +38,6 @@ struct Engine : Builder {
     T4 vae_in; float* vae_moments = nullptr; float* vae_gmoments = nullptr; __half* vae_gin = nullptr;
     T4 dec_in; float* dec_out = nullptr; std::vector<Op> dec_ops;          // VAE decoder (denoise side branch, nerf/sd.py:201-210)
     int ctx_pad = 128;
-    T4 act(int n, int h, int w, int c) { T4 t; t.n = n; t.h = h; t.w = w; t.c = c; t.p = alloc16(t.numel()); return t; }
-
-    // 3x3 stride-1 pad-1 conv via implicit GEMM; w [Cout][3][3][Cin] fp16
-    void conv3(const T4& x, const __half* w, int Cout, const T4& y, const float* bias, const float* row_bias = nullptr,
-               const __half* residual = nullptr) {
-        if (dry) return;
-        const long long M = x.rows();
-        int bw = x.w < 128 ? x.w : 128, bh = 128 / bw; if (bh > x.h) bh = x.h; const int bn_img = 128 / (bw * bh);
-        if (M % 128 || x.c % 64 || bw * bh * bn_img != 128 || x.w % bw || x.h % bh || x.n % bn_img) { err = MI3D_ERR_ARG; return; }
-        int bn = tc::pick_block_n(Cout, M / 128, num_sms);
-        if (!bn) { err = MI3D_ERR_ARG; return; }
-        int splits = 1;
-        if ((size_t)M * Cout <= splitk_elems) {
-            if (Cout % 128 == 0 && (M / 128) * (Cout / 128) * 2 <= num_sms) bn = 128;
-            splits = tc::plan_splits((M / 128) * (Cout / bn), 9 * (x.c / 64), num_sms);
-        }
-        CUtensorMap ma, mb;
-        int r = tc::make_map_nhwc(&ma, x.p, x.c, x.w, x.h, x.n, bw, bh, bn_img);
-        if (!r) r = tc::make_map_matrix(&mb, w, 9ull * x.c, Cout, 9ull * x.c, bn);
-        if (r) { err = r; return; }
-        tc::GemmParams p = {};
-        p.M = (int)M; p.N = Cout; p.K = 9 * x.c; p.num_k_blocks = 9 * (x.c / 64); p.conv = 1;
-        p.conv_H = x.h; p.conv_W = x.w; p.conv_bw = bw; p.conv_bh = bh; p.cin_blocks = x.c / 64;
-        p.a_z1 = 1; p.b_z1 = 1; p.b_batched = 0; p.out = y.p; p.ldc = Cout; p.out_z1 = 1;
-        p.bias = bias; p.row_bias = row_bias; p.rows_per_group = x.h * x.w; p.residual = residual; p.ld_res = Cout;
-        p.epi_mode = tc::EPI_PLAIN; p.alpha = 1.f; p.m_valid = (int)M; p.splits = splits;
-        push([this, ma, mb, p, bn](cudaStream_t st) { return timed_launch(ma, mb, p, bn, 1, st); });
-    }
 
     struct GN { double* stats; const float* gamma; const float* beta; float eps; int silu; T4 x; int G; };
     GN groupnorm(const T4& x, const std::string& pname, float eps, int silu, const T4& y) {
@@ -114,9 +80,6 @@ struct Engine : Builder {
             return (int)cudaGetLastError();
         });
     }
-    // persistent grids of the small direct convolutions: as many CTAs per SM as their weight staging area allows
-    int small_cin_grid(size_t outputs, size_t smem) const { const int per_sm = (int)std::max<size_t>(1, std::min<size_t>(8, (200 * 1024) / std::max<size_t>(smem, 1))); return (int)std::min<size_t>((outputs / 8 + 255) / 256, (size_t)num_sms * per_sm); }
-    int small_cout_grid(size_t pixels, int cin) const { const int ppw = cin <= 128 ? 2 : 1; return (int)std::min<size_t>((pixels / ppw + 7) / 8 + 1, (size_t)num_sms * 8); }
 
     // ------------------------------------------------------------------------------------------------------
     // U-Net pieces (diffusers naming)
@@ -564,12 +527,6 @@ struct Engine : Builder {
             });
         }
         cur = nullptr;
-    }
-
-    // dgrad of a stride-1 3x3 conv: dx = conv3(dy, W_flipped^T)  (+ residual accumulation)
-    void conv3_dgrad(const T4& dy, const std::string& wname, int cin, const T4& dx, const __half* add = nullptr) {
-        Param& w = params[pindex[wname]];
-        conv3(dy, (const __half*)w.dst2, cin, dx, nullptr, nullptr, add);
     }
 
     void build_vae_bwd() {

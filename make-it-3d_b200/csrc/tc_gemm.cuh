@@ -13,6 +13,9 @@
 //   CONV3 : implicit GEMM for a 3x3 stride-1 pad-1 convolution over an NHWC activation: A is a (C, W, H, N) tensor
 //           map, the K loop runs over 9 taps x C/64 channel blocks, each stage is ONE 4-D TMA box shifted by the tap
 //           offset; out-of-bounds rows/columns are zero-filled by the TMA unit (that is the padding).
+//   CONV3_BLOCK (conv = 2, k_tc_gemm_vgg only): the same implicit conv for any H x W: a 128-row M tile is a conv_bw x conv_bh spatial
+//           block of one image (m_blk -> image, block row, block column); the box may overhang the right / bottom edge (zero-filled
+//           loads) and the epilogue stores only the in-image pixels, at NHWC row (n * H + y) * W + x.
 //
 // Warp roles (384 threads): warp 0 = TMA producer (warps 1..3 idle), warpgroups 1 and 2 = MMA + epilogue for tile rows 0..63 / 64..127.
 #pragma once
@@ -32,12 +35,14 @@ constexpr int kThreads = 384;
 // EPI_QUICKGELU: out = y * sigmoid(1.702 y) (CLIP's MLP activation), y = alpha * acc + bias; the pre-activation y is also stored to aux
 //                when aux is set (the input-gradient pass needs it).
 // EPI_QUICKGELU_BWD: out = y * QuickGELU'(aux), aux = the saved pre-activation (same layout as out).
-enum EpiMode : int { EPI_PLAIN = 0, EPI_GEGLU = 1, EPI_TRANSPOSED = 2, EPI_QUICKGELU = 3, EPI_QUICKGELU_BWD = 4 };
+// EPI_RELU: out = max(y, 0) (VGG's convs).  EPI_RELU_BWD: out = y * (aux > 0), aux = the saved post-ReLU input of the conv whose
+//                input gradient this is (same layout as out).  Both only in k_tc_gemm_vgg.
+enum EpiMode : int { EPI_PLAIN = 0, EPI_GEGLU = 1, EPI_TRANSPOSED = 2, EPI_QUICKGELU = 3, EPI_QUICKGELU_BWD = 4, EPI_RELU = 5, EPI_RELU_BWD = 6 };
 
 struct GemmParams {
     int M, N, K;                 // per-batch extents; N multiple of BLOCK_N, K multiple of 64, M multiple of 128 (rows may be padded)
     int num_k_blocks;
-    int conv;                    // 0 plain, 1 implicit 3x3 conv
+    int conv;                    // 0 plain, 1 implicit 3x3 conv, 2 implicit 3x3 conv over spatial blocks (k_tc_gemm_vgg)
     int conv_H, conv_W, conv_bw, conv_bh, cin_blocks;
     int a_z1, b_z1;              // batch decomposition of blockIdx.z for A and B maps; b_batched = 0 -> weights shared
     int b_batched;
@@ -59,7 +64,7 @@ struct GemmParams {
     int splits, kb_per_split;     // split-K: work item t -> (t % splits) K-range, partial sums RED-added (fp32) into splitk_ws[M][N]
     float* splitk_ws;
     int m_tiles, n_tiles, num_tiles;   // persistent tile loop: tile t -> n_blk = t % n_tiles, m_blk = (t / n_tiles) % m_tiles, z = t / (n_tiles * m_tiles)
-    __half* aux;                 // QuickGELU modes: pre-activation, same layout as out
+    __half* aux;                 // QuickGELU modes: pre-activation, same layout as out; EPI_RELU_BWD: the ReLU mask source
 };
 
 // ----------------------------------------------------------------------------------------------------------------
@@ -132,10 +137,10 @@ __device__ __forceinline__ void mma_tile(float (&acc)[BLOCK_N / 2], uint64_t da,
     else wg::wgmma_f16_n256<0, TB>(acc, da, db, accumulate);
 }
 
-// kQuickGelu: the instantiation that also carries the EPI_QUICKGELU* epilogues (the other modes compile exactly as without them)
-template <int BLOCK_N, bool kQuickGelu = false>
-__global__ void __launch_bounds__(kThreads, Cfg<BLOCK_N>::kMinBlocks)
-k_tc_gemm(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmParams p) {
+// The kernel body.  kQuickGelu: the instantiation that also carries the EPI_QUICKGELU* epilogues; kVgg: the one that carries the
+// CONV3_BLOCK mode and the EPI_RELU* epilogues.  Each is a compile-time switch, so the other modes compile exactly as without them.
+template <int BLOCK_N, bool kQuickGelu, bool kVgg>
+__device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUtensorMap& map_b, const GemmParams& p) {
     using C = Cfg<BLOCK_N>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // offset arithmetic keeps the shared address space (STS / LDS, not generic ST / LD)
@@ -162,7 +167,11 @@ k_tc_gemm(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
             const int kb0 = sp * p.kb_per_split, kb1 = min(p.num_k_blocks, kb0 + p.kb_per_split);
             const int m0 = m_blk * BLOCK_M, n0 = n_blk * BLOCK_N;
             int cw = 0, ch = 0, cn = 0;
-            if (p.conv) {
+            if (kVgg && p.conv == 2) {
+                const int bx = (p.conv_W + p.conv_bw - 1) / p.conv_bw, by = (p.conv_H + p.conv_bh - 1) / p.conv_bh;
+                cn = m_blk / (bx * by); const int rem = m_blk - cn * bx * by;
+                ch = rem / bx * p.conv_bh; cw = (rem % bx) * p.conv_bw;
+            } else if (p.conv) {
                 const int hw = p.conv_H * p.conv_W;
                 cn = m0 / hw; const int rem = m0 - cn * hw;
                 ch = rem / p.conv_W; cw = rem - ch * p.conv_W;
@@ -235,7 +244,15 @@ k_tc_gemm(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
             const size_t zoff = (size_t)(z % p.out_z1) * p.out_s_lo + (size_t)(z / p.out_z1) * p.out_s_hi;
             #pragma unroll
             for (int hh = 0; hh < 2; hh++) {
-                const int m = m_blk * BLOCK_M + g * 64 + wl * 16 + (lane >> 2) + 8 * hh;
+                int m = m_blk * BLOCK_M + g * 64 + wl * 16 + (lane >> 2) + 8 * hh;
+                if (kVgg && p.conv == 2) {
+                    // tile row -> pixel of the spatial block; rows over the right / bottom edge are not stored
+                    const int bx = (p.conv_W + p.conv_bw - 1) / p.conv_bw, by = (p.conv_H + p.conv_bh - 1) / p.conv_bh;
+                    const int r = m - m_blk * BLOCK_M, n = m_blk / (bx * by), rem = m_blk - n * bx * by;
+                    const int y = rem / bx * p.conv_bh + r / p.conv_bw, x = (rem % bx) * p.conv_bw + r % p.conv_bw;
+                    if (x >= p.conv_W || y >= p.conv_H) continue;
+                    m = (n * p.conv_H + y) * p.conv_W + x;
+                }
                 const bool row_ok = m < p.m_valid;
                 if (!row_ok) continue;
                 const float* rb = p.row_bias ? p.row_bias + (size_t)(((long long)z * p.M + m) / p.rows_per_group) * p.N : nullptr;
@@ -265,6 +282,12 @@ k_tc_gemm(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
                         const size_t o = zoff + (size_t)m * p.ldc + n;
                         const __half2 pre = *reinterpret_cast<const __half2*>(p.aux + o);
                         *reinterpret_cast<__half2*>(p.out + o) = __floats2half2_rn(f0 * quick_gelu_grad(__low2float(pre)), f1 * quick_gelu_grad(__high2float(pre)));
+                    } else if (kVgg && p.epi_mode == EPI_RELU) {
+                        *reinterpret_cast<__half2*>(p.out + zoff + (size_t)m * p.ldc + n) = __floats2half2_rn(fmaxf(f0, 0.f), fmaxf(f1, 0.f));
+                    } else if (kVgg && p.epi_mode == EPI_RELU_BWD) {
+                        const size_t o = zoff + (size_t)m * p.ldc + n;
+                        const __half2 a = *reinterpret_cast<const __half2*>(p.aux + o);
+                        *reinterpret_cast<__half2*>(p.out + o) = __floats2half2_rn(__low2float(a) > 0.f ? f0 : 0.f, __high2float(a) > 0.f ? f1 : 0.f);
                     } else {
                         if (p.residual) {
                             const __half2 rv = *reinterpret_cast<const __half2*>(p.residual + zoff + (size_t)m * p.ld_res + n);
@@ -277,6 +300,19 @@ k_tc_gemm(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
             }
         }
     }
+}
+
+template <int BLOCK_N, bool kQuickGelu = false>
+__global__ void __launch_bounds__(kThreads, Cfg<BLOCK_N>::kMinBlocks)
+k_tc_gemm(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmParams p) {
+    tc_gemm_body<BLOCK_N, kQuickGelu, false>(map_a, map_b, p);
+}
+
+// VGG19's convs (cx_engine.cu): CONV3_BLOCK tiles, EPI_RELU / EPI_RELU_BWD epilogues
+template <int BLOCK_N>
+__global__ void __launch_bounds__(kThreads, Cfg<BLOCK_N>::kMinBlocks)
+k_tc_gemm_vgg(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmParams p) {
+    tc_gemm_body<BLOCK_N, false, true>(map_a, map_b, p);
 }
 
 // split-K epilogue: out = alpha * ws + bias + row_bias (+ residual) -> fp16 ; 8 elements per thread

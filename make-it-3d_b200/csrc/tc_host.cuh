@@ -62,11 +62,12 @@ inline int pick_block_n(int N, long long m_tiles_times_batch, int num_sms) {
     return 0;
 }
 
-template <int BN, bool kQuickGelu = false>
+template <int BN, bool kQuickGelu = false, bool kVgg = false>
 inline int launch_bn(const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams& p, int batch, cudaStream_t st) {
     static bool attr = false;
+    auto kernel = [] { if constexpr (kVgg) return k_tc_gemm_vgg<BN>; else return k_tc_gemm<BN, kQuickGelu>; }();
     if (!attr) {
-        MI3D_CHECK(cudaFuncSetAttribute(k_tc_gemm<BN, kQuickGelu>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg<BN>::kSmemBytes));
+        MI3D_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg<BN>::kSmemBytes));
         attr = true;
     }
     GemmParams q = p;
@@ -77,7 +78,7 @@ inline int launch_bn(const CUtensorMap& ma, const CUtensorMap& mb, const GemmPar
     if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
     const int resident = (Cfg<BN>::kSmemBytes <= 110 * 1024) ? 2 : 1;       // persistent grid: one (or two) CTAs per SM loop over the tiles
     const int grid = q.num_tiles < sms * resident ? q.num_tiles : sms * resident;
-    k_tc_gemm<BN, kQuickGelu><<<grid, kThreads, Cfg<BN>::kSmemBytes, st>>>(ma, mb, q);
+    kernel<<<grid, kThreads, Cfg<BN>::kSmemBytes, st>>>(ma, mb, q);
     return (int)cudaGetLastError();
 }
 
@@ -85,6 +86,15 @@ inline int launch(const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams
     if (p.K % BLOCK_K || p.N % block_n || p.out_z1 < 1) return MI3D_ERR_ARG;
     if (p.b_mn && block_n % 64) return MI3D_ERR_ARG;                                   // MN-major B is loaded in 64-column boxes
     if (((uintptr_t)p.bias | (uintptr_t)p.row_bias | (uintptr_t)p.splitk_ws) & 15) return MI3D_ERR_ARG;     // read / RED-added 16 bytes at a time
+    if (p.conv == 2 || p.epi_mode == EPI_RELU || p.epi_mode == EPI_RELU_BWD) {
+        if (p.splits > 1 || (p.epi_mode == EPI_RELU_BWD && !p.aux)) return MI3D_ERR_ARG;
+        switch (block_n) {
+            case 64: return launch_bn<64, false, true>(ma, mb, p, batch, st);
+            case 128: return launch_bn<128, false, true>(ma, mb, p, batch, st);
+            case 256: return launch_bn<256, false, true>(ma, mb, p, batch, st);
+        }
+        return MI3D_ERR_ARG;
+    }
     if (p.epi_mode == EPI_QUICKGELU || p.epi_mode == EPI_QUICKGELU_BWD) {
         if (p.splits > 1) return MI3D_ERR_ARG;
         switch (block_n) {
