@@ -569,6 +569,45 @@ int mi3d_cx_backward(mi3d_cx_t h, const float* dloss, float* dx, mi3d_stream_t s
 /* debug tap: device pointer + size of a named intermediate ("relu5_4": fp16 NHWC [2N,H/16,W/16,512], the x images first) */
 int mi3d_cx_debug_tensor(mi3d_cx_t h, const char* name, void** ptr, size_t* bytes);
 
+/* ------------------------------------------------------------------------------------------------------
+ * B7: refine-stage gated U-Net  (replaces the reference's nerf/unet.py UNet(num_input_channels=3+16) with its defaults:
+ * feature_scale 4, bilinear upsampling, sigmoid output, gated blocks; nerf/utils.py:808, 863, 937)
+ * ------------------------------------------------------------------------------------------------------ */
+typedef struct {
+    int N, H, W;               /* images per call (1..16) and the finest level's size (4..4096 each, multiples of 4): the plan is static */
+} mi3d_unet_shape;
+
+typedef struct mi3d_unet* mi3d_unet_t;
+
+/* HOST: bytes of device workspace the engine needs (0: invalid configuration); create plans inside it, NULL on failure */
+size_t mi3d_unet_workspace_bytes(const mi3d_unet_shape* cfg);
+mi3d_unet_t mi3d_unet_create(const mi3d_unet_shape* cfg, void* workspace, size_t workspace_bytes);
+void mi3d_unet_destroy(mi3d_unet_t h);
+/* The registry lists the reference's 41 state_dict entries in its order ("start.block.conv_f.weight" .. "final.0.0.bias"), parameters
+ * and BatchNorm buffers alike (shape rank 0: num_batches_tracked). */
+int mi3d_unet_num_params(mi3d_unet_t h);
+const char* mi3d_unet_param_name(mi3d_unet_t h, int i);
+int mi3d_unet_param_shape(mi3d_unet_t h, int i, int* shape4); /* returns rank */
+/* CUDA-graph replay of the static launch lists, from a list's third call on (`stream` must then be capturable); off by default.
+ * mi3d_unet_graph_replays: lists currently instantiated. */
+int mi3d_unet_set_graph_replay(mi3d_unet_t h, int enable);
+int mi3d_unet_graph_replays(mi3d_unet_t h);
+/* x0 [N,19,H,W], x1 [N,19,H/2,W/2], x2 [N,19,H/4,W/4] fp32 -> out [N,3,H,W] fp32.  state: one DEVICE pointer per registry entry, in
+ * registry order, in torch's layouts: the fp32 parameters are read on every call (no reload after an optimizer step).  train != 0:
+ * BatchNorm with batch statistics, and the fp32 running_mean / running_var and the int64 num_batches_tracked given are updated
+ * once (momentum 0.1, unbiased variance); a NULL buffer pointer skips its update; MI3D_ERR_ARG when N x H/4 x W/4 < 2 (one value
+ * per channel).  train == 0: the running statistics are read.
+ * need_grad != 0 keeps the tape for mi3d_unet_backward; any forward replaces it. */
+int mi3d_unet_forward(mi3d_unet_t h, const float* x0, const float* x1, const float* x2, void* const* state, int train, int need_grad,
+                      float* out, mi3d_stream_t stream);
+/* dout fp32 [N,3,H,W] -> dx0, dx1, dx2 (overwritten) and, for every parameter entry whose grads[i] is not NULL, its fp32 gradient
+ * (overwritten; buffer entries are ignored), for the last forward.  May run any number of times per forward.  MI3D_ERR_ARG without
+ * a tape. */
+int mi3d_unet_backward(mi3d_unet_t h, const float* dout, float* dx0, float* dx1, float* dx2, float* const* grads, mi3d_stream_t stream);
+/* debug tap: device pointer + size of a named fp32 NCHW intermediate ("cat1", "cat2", "d2", "up2", "up1", "out"; "in64" is a
+ * channel slice of "cat1") */
+int mi3d_unet_debug_tensor(mi3d_unet_t h, const char* name, void** ptr, size_t* bytes);
+
 /* unit-test entry for the hand-written wgmma tf32 tiles of the field forward (3-term split, K-major operands):
  * mode 0 (the only one): d[128,N] = a[128,K] . b[N,K]^T, N in {16, 32, 64}, K in {32, 64, 96, 128}.  fp32 in/out. */
 int mi3d_tf32_tile_test(const float* a, const float* b, float* d, int N, int K, int mode, mi3d_stream_t stream);

@@ -111,6 +111,8 @@ SYMBOLS = [
     "mi3d_points_workspace_bytes", "mi3d_points_render_forward", "mi3d_points_render_backward", "mi3d_points_zbuffer_visible",
     "mi3d_cx_workspace_bytes", "mi3d_cx_create", "mi3d_cx_destroy", "mi3d_cx_num_params", "mi3d_cx_param_name", "mi3d_cx_param_shape",
     "mi3d_cx_load_param", "mi3d_cx_set_graph_replay", "mi3d_cx_graph_replays", "mi3d_cx_forward", "mi3d_cx_backward", "mi3d_cx_debug_tensor",
+    "mi3d_unet_workspace_bytes", "mi3d_unet_create", "mi3d_unet_destroy", "mi3d_unet_num_params", "mi3d_unet_param_name", "mi3d_unet_param_shape",
+    "mi3d_unet_set_graph_replay", "mi3d_unet_graph_replays", "mi3d_unet_forward", "mi3d_unet_backward", "mi3d_unet_debug_tensor",
 ]
 
 
