@@ -467,6 +467,37 @@ int mi3d_sd_graph_replays(mi3d_sd_t h);
 int mi3d_sd_debug_tensor(mi3d_sd_t h, const char* name, void** ptr, size_t* bytes);
 
 /* ------------------------------------------------------------------------------------------------------
+ * B3': Stable Diffusion 2 text encoder  (replaces transformers' CLIPTextModel behind get_text_embeds, nerf/sd.py:68-85: OpenCLIP
+ * ViT-H/14's text tower truncated to 23 layers, as every SD-2.x checkpoint ships it)
+ * ------------------------------------------------------------------------------------------------------ */
+typedef struct {
+    int width, layers, heads;  /* 1024, 23, 16 (head_dim 64; MLP width 4 x width, exact-erf GELU) */
+    int context_len, vocab;    /* 77, 49408 */
+    int max_batch;             /* prompts per call (1..8); 2 encodes [negative, positive] in one pass */
+} mi3d_sd_text_cfg;
+
+typedef struct mi3d_sd_text* mi3d_sd_text_t;
+
+/* HOST: bytes of device workspace the engine needs (0: invalid configuration); create plans inside it, NULL on failure */
+size_t mi3d_sd_text_workspace_bytes(const mi3d_sd_text_cfg* cfg);
+mi3d_sd_text_t mi3d_sd_text_create(const mi3d_sd_text_cfg* cfg, void* workspace, size_t workspace_bytes);
+void mi3d_sd_text_destroy(mi3d_sd_text_t h);
+/* Parameters are enumerated by transformers' CLIPTextModel state_dict names, in its order ("text_model.embeddings.token_embedding.weight"
+ * .. "text_model.final_layer_norm.bias"; no position_ids).  The separate q / k / v projections are stored as row slices of one packed
+ * weight.  load: src = fp32 DEVICE tensor in torch's layout; it may be freed once the stream has passed the call. */
+int mi3d_sd_text_num_params(mi3d_sd_text_t h);
+const char* mi3d_sd_text_param_name(mi3d_sd_text_t h, int i);
+int mi3d_sd_text_param_shape(mi3d_sd_text_t h, int i, int* shape4); /* returns rank */
+int mi3d_sd_text_load_param(mi3d_sd_text_t h, int i, const float* src, mi3d_stream_t stream);
+/* CUDA-graph replay of the static launch lists, from a list's third call on (`stream` must then be capturable); off by default.
+ * mi3d_sd_text_graph_replays: lists currently instantiated. */
+int mi3d_sd_text_set_graph_replay(mi3d_sd_text_t h, int enable);
+int mi3d_sd_text_graph_replays(mi3d_sd_text_t h);
+/* ids int64 [B,context_len] (DEVICE) -> out fp32 [B,context_len,width] (DEVICE): last_hidden_state, final_layer_norm applied to every
+ * position.  Causal attention, no padding mask.  Ids outside [0, vocab) are clamped into it.  B <= max_batch. */
+int mi3d_sd_text_encode(mi3d_sd_text_t h, const long long* ids, int B, float* out, mi3d_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------------
  * B4: CLIP losses  (replaces openai CLIP's encode_image / encode_text behind the per-step CLIP losses, nerf/utils.py:436-453, 561-563,
  * and the denoise branch's, nerf/sd.py:97-114, 157-158)
  * ------------------------------------------------------------------------------------------------------ */

@@ -105,6 +105,8 @@ SYMBOLS = [
     "mi3d_sd_workspace_bytes", "mi3d_sd_create", "mi3d_sd_destroy", "mi3d_sd_num_params", "mi3d_sd_param_name", "mi3d_sd_param_numel",
     "mi3d_sd_param_shape", "mi3d_sd_load_param", "mi3d_sd_encode", "mi3d_sd_encode_backward", "mi3d_sd_unet_sds", "mi3d_sd_debug_tensor", "mi3d_sd_profile",
     "mi3d_sd_profile_dump", "mi3d_sd_set_graph_replay", "mi3d_sd_graph_replays", "mi3d_sd_ddim_step", "mi3d_sd_decode",
+    "mi3d_sd_text_workspace_bytes", "mi3d_sd_text_create", "mi3d_sd_text_destroy", "mi3d_sd_text_num_params", "mi3d_sd_text_param_name",
+    "mi3d_sd_text_param_shape", "mi3d_sd_text_load_param", "mi3d_sd_text_set_graph_replay", "mi3d_sd_text_graph_replays", "mi3d_sd_text_encode",
     "mi3d_clip_workspace_bytes", "mi3d_clip_create", "mi3d_clip_destroy", "mi3d_clip_num_params", "mi3d_clip_param_name",
     "mi3d_clip_param_shape", "mi3d_clip_load_param", "mi3d_clip_set_graph_replay", "mi3d_clip_graph_replays", "mi3d_clip_encode_image",
     "mi3d_clip_encode_image_backward", "mi3d_clip_encode_text",

@@ -2,33 +2,23 @@
 //
 // Replaces what openai CLIP's encode_image / encode_text run for the per-step CLIP losses of the training step
 // (nerf/utils.py:436-453, nerf/sd.py:97-114): a statically planned list of launches over the tile GEMM (tc_gemm.cuh) and the fused
-// attention (attn.cuh), built with the op builders shared with the SD engine (engine_plan.cuh), plus the kernels of clip_kernels.cuh.
+// attention (attn.cuh), built with the op builders shared with the SD engine (engine_plan.cuh) and the transformer block shared with
+// the SD-2 text encoder (transformer_plan.cuh), plus the kernels of clip_kernels.cuh.
 // Token rows: every image / prompt owns Tpad = roundup(T, 64) rows (197 -> 256 image tokens, 77 -> 128 text tokens); rows past T are
 // zero at the embedding, carry finite values through the blocks, are masked out as keys and never reach a valid row, so every
 // attention product of the input-gradient pass has K a multiple of 64.  Activations fp16, statistics and accumulation fp32, weights
 // fp16 copies (plus transposed copies for the input-gradient GEMMs) of the fp32 openai parameters.  The CLIP weights are frozen: the
 // backward computes the input gradient only.  No split-K and no atomics: results are bit-reproducible run to run and under graph replay.
-#include "engine_plan.cuh"
-#include "clip_kernels.cuh"
+#include "transformer_plan.cuh"
 
 namespace clip {
 
 using namespace plan;
 
-struct Tower { int C = 0, L = 0, heads = 0, T = 0, Tpad = 0; };
-
-struct BlockW {
-    std::string pre;
-    const float *ln1, *ln2, *b_in, *b_out, *b_fc, *b_proj;
-    const __half *w_in, *w_out, *w_fc, *w_proj;           // [out][in]: forward
-    const __half *t_in, *t_out, *t_fc, *t_proj;           // [in][out]: input-gradient GEMMs (image tower only)
-};
-// one block's activations, sized for max_batch; every launch list of the tower (any batch) uses the same buffers
-struct BlockA { __half *x, *ln1, *qkv, *qkvT, *S, *ao, *h, *ln2, *pre, *act, *out; };
 // scratch of the reverse walk, shared by all blocks (they run one after the other)
 struct BwdA { __half *dpre, *dln2, *dh, *dao, *daoT, *dS, *PT, *dST, *dqkv, *dln1; };
 
-struct Engine : Builder {
+struct Engine : TowerBuilder {
     mi3d_clip_cfg cfg;
     Tower vt, tt;
     int np = 0, G = 0, KP = 0;
@@ -48,21 +38,19 @@ struct Engine : Builder {
     // the tape of the last image forward
     bool tape_valid = false; int tape_B = 0, tape_H = 0, tape_W = 0, tape_aug = 0;
 
-    static int pad64(int t) { return (t + 63) / 64 * 64; }
-
     void block_params(const std::string& pre, int C, bool both, BlockW& w) {
         const PKind k = both ? PK_LINEAR_BOTH : PK_LINEAR;
-        w.pre = pre;
         auto lin = [&](const std::string& n, int o, int i, const __half** fw, const __half** bw_) {
             Param& P = param(pre + n, {o, i}, k); *fw = (const __half*)P.dst; *bw_ = (const __half*)P.dst2;
         };
-        w.ln1 = pf(pre + ".ln_1.weight", {C}); pf(pre + ".ln_1.bias", {C});
+        w.ln1 = pf(pre + ".ln_1.weight", {C}); w.ln1_b = pf(pre + ".ln_1.bias", {C});
         lin(".attn.in_proj_weight", 3 * C, C, &w.w_in, &w.t_in); w.b_in = pf(pre + ".attn.in_proj_bias", {3 * C});
         lin(".attn.out_proj.weight", C, C, &w.w_out, &w.t_out); w.b_out = pf(pre + ".attn.out_proj.bias", {C});
-        w.ln2 = pf(pre + ".ln_2.weight", {C}); pf(pre + ".ln_2.bias", {C});
+        w.ln2 = pf(pre + ".ln_2.weight", {C}); w.ln2_b = pf(pre + ".ln_2.bias", {C});
         lin(".mlp.c_fc.weight", 4 * C, C, &w.w_fc, &w.t_fc); w.b_fc = pf(pre + ".mlp.c_fc.bias", {4 * C});
         lin(".mlp.c_proj.weight", C, 4 * C, &w.w_proj, &w.t_proj); w.b_proj = pf(pre + ".mlp.c_proj.bias", {C});
     }
+    // one block's activations, sized for max_batch; every launch list of the tower (any batch) uses the same buffers
     BlockA block_bufs(const Tower& t, __half* x) {
         const size_t M = (size_t)cfg.max_batch * t.Tpad, C = t.C;
         BlockA a; a.x = x;
@@ -70,62 +58,6 @@ struct Engine : Builder {
         a.S = alloc16((size_t)cfg.max_batch * t.heads * t.Tpad * t.Tpad); a.ao = alloc16(M * C); a.h = alloc16(M * C);
         a.ln2 = alloc16(M * C); a.pre = alloc16(M * 4 * C); a.act = alloc16(M * 4 * C); a.out = alloc16(M * C);
         return a;
-    }
-
-    // ---- batched per-(image, head) products on token rows: z = b * heads + h ----
-    // head h of section s (0 q, 1 k, 2 v) of a [b][Tpad][ld] token matrix, K = 64 contiguous
-    Mat heads_rows(const __half* p, long long ld, const Tower& t) const {
-        Mat m{p, ld, t.Tpad, 64}; m.z1 = t.heads; m.sz1 = 64; m.z2 = 0; m.sz2 = (long long)t.Tpad * ld; return m;
-    }
-    // the same head as an operand with K = tokens: per-image transposed copy [b][ldT][Tpad], head rows at h*64 (+ section offset in p)
-    Mat heads_cols(const __half* p, long long ldT, const Tower& t) const {
-        Mat m{p, t.Tpad, 64, t.Tpad}; m.z1 = t.heads; m.sz1 = 64LL * t.Tpad; m.z2 = 0; m.sz2 = ldT * t.Tpad; return m;
-    }
-    // [b * heads][Tpad][Tpad] score-shaped operand
-    Mat scores(const __half* p, const Tower& t) const {
-        Mat m{p, t.Tpad, t.Tpad, t.Tpad}; m.z1 = t.heads; m.sz1 = (long long)t.Tpad * t.Tpad; m.z2 = 0; m.sz2 = (long long)t.heads * t.Tpad * t.Tpad; return m;
-    }
-    void bgemm(Mat a, Mat b, int N, __half* out, long long ldc, long long s_lo, long long s_hi, int out_z1, int B, const Tower& t) {
-        a.z2 = B; b.z2 = B;
-        Out o; o.p16 = out; o.ldc = ldc; o.z1 = out_z1; o.s_lo = s_lo; o.s_hi = s_hi;
-        Epi e;
-        gemm(a, b, N, o, e, B * t.heads, true);
-    }
-
-    // attention with the score matrix materialised: S = Q K^T, (causal) softmax, O = P V; P stays in a.S for the backward
-    void attention_materialised(const Tower& t, const BlockA& a, int B, bool causal) {
-        const int C = t.C, Tp = t.Tpad;
-        transpose(a.qkv, a.qkvT, B, Tp, 3 * C);                                          // [b][3C][Tpad]
-        bgemm(heads_rows(a.qkv, 3 * C, t), heads_rows(a.qkv + C, 3 * C, t), Tp, a.S, Tp, 0, (long long)Tp * Tp, 1, B, t);
-        const size_t rows = (size_t)B * t.heads * Tp;
-        if (causal) {
-            __half* s = a.S; const int T = t.T;
-            push([=](cudaStream_t st) {
-                clipk::k_softmax_causal<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(s, rows, Tp, T, Tp, 0.125f);
-                return (int)cudaGetLastError();
-            });
-        } else {
-            softmax(a.S, rows, Tp, t.T, 0.125f);
-        }
-        bgemm(scores(a.S, t), heads_cols(a.qkvT + 2LL * C * Tp, 3 * C, t), 64, a.ao, C, 64, (long long)Tp * C, t.heads, B, t);
-    }
-
-    // mode 0: fused attention (no tape); 1: materialised, tape kept for the backward; 2: materialised causal (text tower)
-    void block_fwd(const Tower& t, const BlockW& w, const BlockA& a, int B, int mode) {
-        const int C = t.C; const long long M = (long long)B * t.Tpad;
-        layernorm(a.x, M, C, w.pre + ".ln_1", a.ln1);
-        linear(a.ln1, M, C, w.w_in, 3 * C, a.qkv, w.b_in);
-        if (mode == 0) attention_core(a.qkv, 3 * C, a.qkv + C, 3 * C, a.qkv + 2 * C, 3 * C, B, t.Tpad, t.Tpad, t.T, t.heads, 64, a.ao, C);
-        else attention_materialised(t, a, B, mode == 2);
-        linear(a.ao, M, C, w.w_out, C, a.h, w.b_out, a.x);
-        layernorm(a.h, M, C, w.pre + ".ln_2", a.ln2);
-        {
-            Mat x{a.ln2, C, M, C}; Mat wm{w.w_fc, C, 4 * C, C};
-            Out o; o.p16 = a.act; o.ldc = 4 * C;
-            Epi e; e.bias = w.b_fc; e.mode = tc::EPI_QUICKGELU; e.aux = mode == 1 ? a.pre : nullptr;
-            gemm(x, wm, 4 * C, o, e);
-        }
-        linear(a.act, M, 4 * C, w.w_proj, C, a.out, w.b_proj, a.h);
     }
 
     // dx = LayerNorm input gradient of dy (+ add)
@@ -214,7 +146,7 @@ struct Engine : Builder {
                       return (int)cudaGetLastError();
                   }); }
                 layernorm(x0, M, C, "visual.ln_pre", r0);
-                for (int i = 0; i < t.L; i++) block_fwd(t, vw[i], va[i], B, tape);
+                for (int i = 0; i < t.L; i++) block_fwd(t, vw[i], va[i], B, tape, tc::EPI_QUICKGELU);
                 gather_rows(r_last, (size_t)t.Tpad * C, cls, C, C, B);
                 layernorm(cls, B, C, "visual.ln_post", clsn);
                 Mat a{clsn, C, B, C}; Mat wm{w_proj, C, c.embed_dim, C};
@@ -278,7 +210,7 @@ struct Engine : Builder {
                 clipk::k_text_embed<<<blocks_for((size_t)B * Tp * C / 8), 256, 0, st>>>(tk, tok, pos, xx, B, T, Tp, C, V);
                 return (int)cudaGetLastError();
             });
-            for (int i = 0; i < t.L; i++) block_fwd(t, tw[i], ta[i], B, 2);
+            for (int i = 0; i < t.L; i++) block_fwd(t, tw[i], ta[i], B, 2, tc::EPI_QUICKGELU);
             __half* rows = eot;
             push([=](cudaStream_t st) {
                 clipk::k_text_eot_rows<<<B, 128, 0, st>>>(tk, r_last, rows, T, Tp, C);

@@ -10,6 +10,7 @@
 #include "sd_kernels.cuh"
 
 namespace clipk {
+namespace {   // internal linkage: the CLIP engine and the SD-2 text encoder both include these kernels
 
 // openai CLIP's Normalize constants
 __device__ __forceinline__ float norm_mean(int c) { return c == 0 ? 0.48145466f : (c == 1 ? 0.4578275f : 0.40821073f); }
@@ -248,4 +249,5 @@ __global__ void k_softmax_causal(__half* __restrict__ s, size_t rows, int cols, 
     }
 }
 
+}  // namespace
 }  // namespace clipk

@@ -94,6 +94,16 @@ struct Builder {
         return params.back();
     }
     const float* pf(const std::string& name, std::vector<int> shape) { return (const float*)param(name, shape, PK_F32).dst; }
+    // a parameter stored in memory the engine carved itself (a row slice of a packed weight): registered, not allocated
+    Param& param_view(const std::string& name, std::vector<int> shape, PKind kind, void* dst) {
+        auto it = pindex.find(name);
+        if (it != pindex.end()) return params[it->second];
+        Param P; P.name = name; P.shape = shape; P.kind = kind; P.numel = 1; P.dst = dst;
+        for (int s : shape) P.numel *= (size_t)s;
+        pindex[name] = (int)params.size();
+        params.push_back(P);
+        return params.back();
+    }
 
     // ------------------------------------------------------------------------------------------------------
     // op builders
@@ -198,6 +208,9 @@ struct Builder {
 
     void layernorm(const __half* x, long long rows, int C, const std::string& pname, __half* y) {
         const float* ga = pf(pname + ".weight", {C}); const float* be = pf(pname + ".bias", {C});
+        layernorm(x, rows, C, ga, be, y);
+    }
+    void layernorm(const __half* x, long long rows, int C, const float* ga, const float* be, __half* y) {
         push([=](cudaStream_t st) {
             sdk::k_layernorm<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(x, y, ga, be, (int)rows, C, 1e-5f);
             return (int)cudaGetLastError();

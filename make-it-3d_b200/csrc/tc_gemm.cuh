@@ -37,7 +37,10 @@ constexpr int kThreads = 384;
 // EPI_QUICKGELU_BWD: out = y * QuickGELU'(aux), aux = the saved pre-activation (same layout as out).
 // EPI_RELU: out = max(y, 0) (VGG's convs).  EPI_RELU_BWD: out = y * (aux > 0), aux = the saved post-ReLU input of the conv whose
 //                input gradient this is (same layout as out).  Both only in k_tc_gemm_vgg.
-enum EpiMode : int { EPI_PLAIN = 0, EPI_GEGLU = 1, EPI_TRANSPOSED = 2, EPI_QUICKGELU = 3, EPI_QUICKGELU_BWD = 4, EPI_RELU = 5, EPI_RELU_BWD = 6 };
+// EPI_GELU: out = 0.5 y (1 + erf(y / sqrt 2)) (exact GELU, the SD-2 text encoder's MLP activation), y = alpha * acc + bias, in fp32,
+//                stored fp16.  Forward only; only in k_tc_gemm_gelu.
+enum EpiMode : int { EPI_PLAIN = 0, EPI_GEGLU = 1, EPI_TRANSPOSED = 2, EPI_QUICKGELU = 3, EPI_QUICKGELU_BWD = 4, EPI_RELU = 5, EPI_RELU_BWD = 6,
+                     EPI_GELU = 7 };
 
 struct GemmParams {
     int M, N, K;                 // per-batch extents; N multiple of BLOCK_N, K multiple of 64, M multiple of 128 (rows may be padded)
@@ -138,8 +141,9 @@ __device__ __forceinline__ void mma_tile(float (&acc)[BLOCK_N / 2], uint64_t da,
 }
 
 // The kernel body.  kQuickGelu: the instantiation that also carries the EPI_QUICKGELU* epilogues; kVgg: the one that carries the
-// CONV3_BLOCK mode and the EPI_RELU* epilogues.  Each is a compile-time switch, so the other modes compile exactly as without them.
-template <int BLOCK_N, bool kQuickGelu, bool kVgg>
+// CONV3_BLOCK mode and the EPI_RELU* epilogues; kGelu: the one that carries EPI_GELU.  Each is a compile-time switch, so the other
+// modes compile exactly as without them.
+template <int BLOCK_N, bool kQuickGelu, bool kVgg, bool kGelu = false>
 __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUtensorMap& map_b, const GemmParams& p) {
     using C = Cfg<BLOCK_N>;
     extern __shared__ uint8_t smem_raw[];
@@ -288,6 +292,8 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUt
                         const size_t o = zoff + (size_t)m * p.ldc + n;
                         const __half2 a = *reinterpret_cast<const __half2*>(p.aux + o);
                         *reinterpret_cast<__half2*>(p.out + o) = __floats2half2_rn(__low2float(a) > 0.f ? f0 : 0.f, __high2float(a) > 0.f ? f1 : 0.f);
+                    } else if (kGelu && p.epi_mode == EPI_GELU) {
+                        *reinterpret_cast<__half2*>(p.out + zoff + (size_t)m * p.ldc + n) = __floats2half2_rn(gelu_erf(f0), gelu_erf(f1));
                     } else {
                         if (p.residual) {
                             const __half2 rv = *reinterpret_cast<const __half2*>(p.residual + zoff + (size_t)m * p.ld_res + n);
@@ -313,6 +319,13 @@ template <int BLOCK_N>
 __global__ void __launch_bounds__(kThreads, Cfg<BLOCK_N>::kMinBlocks)
 k_tc_gemm_vgg(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmParams p) {
     tc_gemm_body<BLOCK_N, false, true>(map_a, map_b, p);
+}
+
+// the SD-2 text encoder's MLP input GEMM (sd_text_engine.cu): EPI_GELU epilogue
+template <int BLOCK_N>
+__global__ void __launch_bounds__(kThreads, Cfg<BLOCK_N>::kMinBlocks)
+k_tc_gemm_gelu(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmParams p) {
+    tc_gemm_body<BLOCK_N, false, false, true>(map_a, map_b, p);
 }
 
 // split-K epilogue: out = alpha * ws + bias + row_bias (+ residual) -> fp16 ; 8 elements per thread

@@ -62,10 +62,14 @@ inline int pick_block_n(int N, long long m_tiles_times_batch, int num_sms) {
     return 0;
 }
 
-template <int BN, bool kQuickGelu = false, bool kVgg = false>
+template <int BN, bool kQuickGelu = false, bool kVgg = false, bool kGelu = false>
 inline int launch_bn(const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams& p, int batch, cudaStream_t st) {
     static bool attr = false;
-    auto kernel = [] { if constexpr (kVgg) return k_tc_gemm_vgg<BN>; else return k_tc_gemm<BN, kQuickGelu>; }();
+    auto kernel = [] {
+        if constexpr (kVgg) return k_tc_gemm_vgg<BN>;
+        else if constexpr (kGelu) return k_tc_gemm_gelu<BN>;
+        else return k_tc_gemm<BN, kQuickGelu>;
+    }();
     if (!attr) {
         MI3D_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg<BN>::kSmemBytes));
         attr = true;
@@ -101,6 +105,15 @@ inline int launch(const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams
             case 64: return launch_bn<64, true>(ma, mb, p, batch, st);
             case 128: return launch_bn<128, true>(ma, mb, p, batch, st);
             case 256: return launch_bn<256, true>(ma, mb, p, batch, st);
+        }
+        return MI3D_ERR_ARG;
+    }
+    if (p.epi_mode == EPI_GELU) {
+        if (p.splits > 1 || p.conv || !p.out) return MI3D_ERR_ARG;
+        switch (block_n) {
+            case 64: return launch_bn<64, false, false, true>(ma, mb, p, batch, st);
+            case 128: return launch_bn<128, false, false, true>(ma, mb, p, batch, st);
+            case 256: return launch_bn<256, false, false, true>(ma, mb, p, batch, st);
         }
         return MI3D_ERR_ARG;
     }

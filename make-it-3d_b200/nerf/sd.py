@@ -12,7 +12,9 @@ initialisers -- which is what the benchmark and the parity tests use (`data: syn
 The "denoise" side branch (nerf/sd.py:153-159: DDIM step t -> t-1, VAE decode, CLIP losses) is built on the same engine (`mi3d_sd_ddim_step`,
 `mi3d_sd_decode`); the CLIP losses run on the caller-provided clip_model (the reference passes it in too) and are skipped without one.
 A native `nerf.clip.CLIP` computes them on the CLIP engine (csrc/clip_engine.cu, aug included); any other model is called as before.
-What is NOT built (SURVEY.md 8f rank 3): the OpenCLIP text encoder behind `get_text_embeds` (deterministic stand-in).
+`get_text_embeds` runs the SD-2 text encoder (nerf/sd_text.py, csrc/sd_text_engine.cu) once its weights are loaded with
+`load_diffusers_state_dict(text_encoder_state=...)`; prompts given as strings go through the `tokenizer` passed to the constructor.
+Without text-encoder weights it returns a deterministic stand-in keyed by the prompt strings.
 """
 import contextlib
 import ctypes as C
@@ -25,6 +27,7 @@ import torch.nn as nn
 
 from .. import _lib as L
 from .clip import CLIP
+from .sd_text import TextEncoder, cfg_from_state_dict
 
 
 class UNetCfg(C.Structure):
@@ -199,8 +202,13 @@ class _EncodeImgs(torch.autograd.Function):
 
 class StableDiffusion(nn.Module):
     def __init__(self, device, sd_version='2.0', hf_key=None, step_range=[0.2, 0.6], unet_cfg=None, vae_cfg=None, seed=0,
-                 unet_state=None, vae_state=None, graph_replay=True, defer_backward=False):
+                 unet_state=None, vae_state=None, graph_replay=True, defer_backward=False, tokenizer=None):
         super().__init__()
+        # tokenizer: a callable with CLIPTokenizer.__call__'s contract (e.g. CLIPTokenizer.from_pretrained(model_key, subfolder="tokenizer")),
+        # used by get_text_embeds for prompts given as strings.  The text encoder itself is created when its weights are loaded.
+        self.tokenizer = tokenizer
+        self.text_encoder = None
+        self.graph_replay = graph_replay
         # defer_backward (additive option, default off = the reference's behaviour): train_step does not call latents.backward
         # itself (nerf/sd.py:171) but returns the surrogate loss  sum(stopgrad(dL/d pred_rgb) * pred_rgb), whose gradient w.r.t.
         # pred_rgb IS the SDS gradient.  The Trainer adds it to its regularisers and its single loss.backward() (nerf/utils.py:983)
@@ -242,8 +250,17 @@ class StableDiffusion(nn.Module):
         self.alphas = alphas_cumprod().to(self.device)
         self._t = torch.zeros(1, dtype=torch.long, device=self.device)
 
-    def load_diffusers_state_dict(self, unet_state=None, vae_state=None):
-        """copy tensors named like diffusers' UNet2DConditionModel / AutoencoderKL state_dict()s and push them to the engine."""
+    def load_diffusers_state_dict(self, unet_state=None, vae_state=None, text_encoder_state=None):
+        """copy tensors named like diffusers' UNet2DConditionModel / AutoencoderKL state_dict()s and push them to the engine;
+        text_encoder_state (transformers' CLIPTextModel.state_dict()) goes into the SD-2 text encoder, created on first use."""
+        if text_encoder_state is not None:
+            if self.text_encoder is None:
+                self.text_encoder = TextEncoder(self.device, cfg=cfg_from_state_dict(text_encoder_state), state_dict=text_encoder_state,
+                                                graph_replay=self.graph_replay)
+            else:
+                self.text_encoder.load_state_dict(text_encoder_state)
+            if unet_state is None and vae_state is None:
+                return
         with torch.no_grad():
             for store, sd in ((self.unet, unet_state), (self.vae, vae_state)):
                 if sd is None:
@@ -258,16 +275,40 @@ class StableDiffusion(nn.Module):
         self.engine.load(tensors)
 
     def get_text_embeds(self, prompt, negative_prompt):
-        """nerf/sd.py:68-85.  The CLIP text encoder is outside the hot path and its weights are not available offline; a
-        deterministic stand-in keyed by the prompt strings keeps the call surface ([2,77,D], uncond first)."""
-        D = self.unet_cfg["cross_dim"]
-        out = []
-        for s in (negative_prompt, prompt):
-            s = s[0] if isinstance(s, (list, tuple)) else s
-            # stable digest (python's hash() is salted per process: every rank would get different text conditioning)
-            g = torch.Generator().manual_seed(int.from_bytes(hashlib.sha256(("mi3d:" + s).encode()).digest()[:4], "little"))
-            out.append(torch.randn(1, 77, D, generator=g))
-        return torch.cat(out).to(self.device)
+        """nerf/sd.py:68-85: [uncond, cond] text embeddings [2,77,D].  prompt / negative_prompt: a string, a list of one string, or
+        int64 token ids [1,77] / [77].  With text-encoder weights loaded both run through the SD-2 text encoder in one batch of 2;
+        strings need the tokenizer (the prompt is truncated to 77 tokens, the negative prompt is not, as in the reference).
+        Without them a deterministic stand-in keyed by the prompt strings keeps the call surface."""
+        if self.text_encoder is None:
+            D = self.unet_cfg["cross_dim"]
+            out = []
+            for s in (negative_prompt, prompt):
+                s = s[0] if isinstance(s, (list, tuple)) else s
+                # stable digest (python's hash() is salted per process: every rank would get different text conditioning)
+                g = torch.Generator().manual_seed(int.from_bytes(hashlib.sha256(("mi3d:" + s).encode()).digest()[:4], "little"))
+                out.append(torch.randn(1, 77, D, generator=g))
+            return torch.cat(out).to(self.device)
+        ids = torch.cat([self._token_ids(negative_prompt, truncation=False), self._token_ids(prompt, truncation=True)])
+        with torch.no_grad():
+            return self.text_encoder(ids)[0]
+
+    def _token_ids(self, text, truncation):
+        T = self.text_encoder.cfg["context_len"]
+        if torch.is_tensor(text):
+            ids = text
+        else:
+            if self.tokenizer is None:
+                raise L.Mi3dError("get_text_embeds got a string but StableDiffusion has no tokenizer: pass tokenizer=CLIPTokenizer.from_pretrained("
+                                  "model_key, subfolder='tokenizer') to the constructor, or pass int64 token ids [1,77]")
+            kw = dict(padding="max_length", max_length=T, return_tensors="pt")
+            if truncation:
+                kw["truncation"] = True
+            tok = self.tokenizer(text if isinstance(text, (list, tuple)) else [text], **kw)
+            ids = tok.input_ids if hasattr(tok, "input_ids") else tok["input_ids"]
+            ids = torch.as_tensor(ids)
+        if ids.dtype != torch.long or ids.shape[-1] != T or ids.dim() not in (1, 2) or (ids.dim() == 2 and ids.shape[0] != 1):
+            raise L.Mi3dError(f"text embeddings take one prompt's int64 token ids [1,{T}] or [{T}]; got {ids.dtype} {tuple(ids.shape)}")
+        return ids.reshape(1, T).to(self.device)
 
     def encode_imgs(self, imgs, eps=None):
         """nerf/sd.py:212-220 (the 512x512 interpolation of :124 is folded in: pass the render-resolution image)."""
