@@ -639,6 +639,31 @@ int mi3d_unet_backward(mi3d_unet_t h, const float* dout, float* dx0, float* dx1,
  * channel slice of "cat1") */
 int mi3d_unet_debug_tensor(mi3d_unet_t h, const char* name, void** ptr, size_t* bytes);
 
+/* ------------------------------------------------------------------------------------------------------
+ * B8: DPT-Hybrid depth model  (replaces the reference's DPT/dpt DPTDepthModel(backbone="vitb_rn50_384", non_negative=True) and timm
+ * behind the reference image's depth prior, main.py:111-127, 196-214: ResNet-50v2 trunk, ViT-B/16 on 577 tokens, RefineNet decoder)
+ * ------------------------------------------------------------------------------------------------------ */
+typedef struct mi3d_dpt* mi3d_dpt_t;
+
+/* HOST: bytes of device workspace the engine needs (one shape: a [1,3,384,384] image); create plans inside it (the workspace must be
+ * zero-filled: padding rows and channels are never written), NULL on failure */
+size_t mi3d_dpt_workspace_bytes(void);
+mi3d_dpt_t mi3d_dpt_create(void* workspace, size_t workspace_bytes);
+void mi3d_dpt_destroy(mi3d_dpt_t h);
+/* Parameters are enumerated by the reference's DPTDepthModel.state_dict() names ("pretrained.model.cls_token" ..
+ * "scratch.output_conv.4.bias"), every tensor the forward reads and nothing else (not pretrained.model.norm.*, pretrained.model.head.*
+ * or scratch.refinenet4.resConfUnit1.*).  The trunk's convs are weight-standardised at load.  load: src = fp32 DEVICE tensor in torch's
+ * layout; it may be freed once the stream has passed the call. */
+int mi3d_dpt_num_params(mi3d_dpt_t h);
+const char* mi3d_dpt_param_name(mi3d_dpt_t h, int i);
+int mi3d_dpt_param_shape(mi3d_dpt_t h, int i, int* shape4); /* returns rank */
+int mi3d_dpt_load_param(mi3d_dpt_t h, int i, const float* src, mi3d_stream_t stream);
+/* img fp32 [1,3,384,384] (resized and normalised, DEVICE) -> out fp32 [1,384,384] inverse depth (DEVICE) */
+int mi3d_dpt_forward(mi3d_dpt_t h, const float* img, float* out, mi3d_stream_t stream);
+/* the last forward's reassembled backbone features layer_1 .. layer_4 (i = 0..3) as fp32 NCHW: [1,256,96,96], [1,512,48,48],
+ * [1,768,24,24], [1,768,12,12] */
+int mi3d_dpt_tap(mi3d_dpt_t h, int i, float* dst, mi3d_stream_t stream);
+
 /* unit-test entry for the hand-written wgmma tf32 tiles of the field forward (3-term split, K-major operands):
  * mode 0 (the only one): d[128,N] = a[128,K] . b[N,K]^T, N in {16, 32, 64}, K in {32, 64, 96, 128}.  fp32 in/out. */
 int mi3d_tf32_tile_test(const float* a, const float* b, float* d, int N, int K, int mode, mi3d_stream_t stream);

@@ -115,6 +115,8 @@ SYMBOLS = [
     "mi3d_cx_load_param", "mi3d_cx_set_graph_replay", "mi3d_cx_graph_replays", "mi3d_cx_forward", "mi3d_cx_backward", "mi3d_cx_debug_tensor",
     "mi3d_unet_workspace_bytes", "mi3d_unet_create", "mi3d_unet_destroy", "mi3d_unet_num_params", "mi3d_unet_param_name", "mi3d_unet_param_shape",
     "mi3d_unet_set_graph_replay", "mi3d_unet_graph_replays", "mi3d_unet_forward", "mi3d_unet_backward", "mi3d_unet_debug_tensor",
+    "mi3d_dpt_workspace_bytes", "mi3d_dpt_create", "mi3d_dpt_destroy", "mi3d_dpt_num_params", "mi3d_dpt_param_name", "mi3d_dpt_param_shape",
+    "mi3d_dpt_load_param", "mi3d_dpt_forward", "mi3d_dpt_tap",
 ]
 
 

@@ -24,7 +24,8 @@ using Op = std::function<int(cudaStream_t)>;
 
 // How a parameter is stored in the workspace.  The engines' load functions turn the fp32 source tensor into this form.
 enum PKind { PK_F32 = 0, PK_LINEAR, PK_LINEAR_T, PK_LINEAR_BOTH, PK_CONV3, PK_CONV3_BOTH, PK_CONV1, PK_CONV1_BOTH, PK_GEGLU_W, PK_GEGLU_B,
-             PK_CONV_F32_OHWI, PK_CONV_SMALL_COUT, PK_CONV_SMALL_COUT_BOTH };
+             PK_CONV_F32_OHWI, PK_CONV_SMALL_COUT, PK_CONV_SMALL_COUT_BOTH,
+             PK_CONV_WS };   // weight-standardised conv (dpt_engine.cu): OIHW fp32 -> standardised [O][kh][kw][I] fp16
 
 struct Param {
     std::string name; std::vector<int> shape; size_t numel = 0; PKind kind = PK_F32;
@@ -85,7 +86,8 @@ struct Builder {
         switch (kind) {
             case PK_F32: case PK_GEGLU_B: P.dst = alloc(P.numel * 4); break;
             case PK_CONV_F32_OHWI: P.dst = alloc((size_t)std::max(shape[0], shape[1]) * 9 * 8 * 4); break;   // input channels padded to <= 8
-            case PK_LINEAR: case PK_CONV3: case PK_CONV1: case PK_GEGLU_W: case PK_LINEAR_T: case PK_CONV_SMALL_COUT: P.dst = alloc(P.numel * 2); break;
+            case PK_LINEAR: case PK_CONV3: case PK_CONV1: case PK_GEGLU_W: case PK_LINEAR_T: case PK_CONV_SMALL_COUT: case PK_CONV_WS:
+                P.dst = alloc(P.numel * 2); break;
             case PK_LINEAR_BOTH: case PK_CONV3_BOTH: case PK_CONV1_BOTH: case PK_CONV_SMALL_COUT_BOTH:
                 P.dst = alloc(P.numel * 2); P.dst2 = alloc(P.numel * 2); break;
         }
@@ -181,9 +183,10 @@ struct Builder {
     }
 
     // The same conv for any H x W (VGG's levels): each 128-row tile is a bw x bh block of one image (the shape that wastes the
-    // fewest rows over the image edge), overhanging tiles load zeros and store only in-image pixels.  mode: EPI_PLAIN, EPI_RELU, or
-    // EPI_RELU_BWD with aux = the mask source.  No split-K (its fp32 RED order varies run to run).
-    void conv3_block(const T4& x, const __half* w, int Cout, const T4& y, const float* bias, int mode, const __half* aux = nullptr) {
+    // fewest rows over the image edge), overhanging tiles load zeros and store only in-image pixels.  mode: EPI_PLAIN (optionally
+    // + residual, same layout as y), EPI_RELU, or EPI_RELU_BWD with aux = the mask source.  No split-K (its fp32 RED order varies run to run).
+    void conv3_block(const T4& x, const __half* w, int Cout, const T4& y, const float* bias, int mode, const __half* aux = nullptr,
+                     const __half* residual = nullptr) {
         if (dry) return;
         if (x.c % 64 || Cout % 64 || y.n != x.n || y.h != x.h || y.w != x.w || y.c != Cout) { err = MI3D_ERR_ARG; return; }
         int bw = 128, bh = 1; long long best = -1;
@@ -203,6 +206,7 @@ struct Builder {
         p.conv_H = x.h; p.conv_W = x.w; p.conv_bw = bw; p.conv_bh = bh; p.cin_blocks = x.c / 64;
         p.a_z1 = 1; p.b_z1 = 1; p.b_batched = 0; p.out = y.p; p.ldc = Cout; p.out_z1 = 1;
         p.bias = bias; p.rows_per_group = 1; p.epi_mode = mode; p.alpha = 1.f; p.m_valid = (int)x.rows(); p.splits = 1; p.aux = const_cast<__half*>(aux);
+        p.residual = residual; p.ld_res = Cout;
         push([this, ma, mb, p, bn](cudaStream_t st) { return timed_launch(ma, mb, p, bn, 1, st); });
     }
 
@@ -210,9 +214,9 @@ struct Builder {
         const float* ga = pf(pname + ".weight", {C}); const float* be = pf(pname + ".bias", {C});
         layernorm(x, rows, C, ga, be, y);
     }
-    void layernorm(const __half* x, long long rows, int C, const float* ga, const float* be, __half* y) {
+    void layernorm(const __half* x, long long rows, int C, const float* ga, const float* be, __half* y, float eps = 1e-5f) {
         push([=](cudaStream_t st) {
-            sdk::k_layernorm<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(x, y, ga, be, (int)rows, C, 1e-5f);
+            sdk::k_layernorm<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(x, y, ga, be, (int)rows, C, eps);
             return (int)cudaGetLastError();
         });
     }

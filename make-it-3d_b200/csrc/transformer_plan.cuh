@@ -1,5 +1,5 @@
-// transformer_plan.cuh -- the pre-LN transformer block shared by the CLIP towers (clip_engine.cu) and the SD-2 text encoder
-// (sd_text_engine.cu), built on the op builders of engine_plan.cuh.
+// transformer_plan.cuh -- the pre-LN transformer block shared by the CLIP towers (clip_engine.cu), the SD-2 text encoder
+// (sd_text_engine.cu) and DPT's ViT-B/16 (dpt_engine.cu), built on the op builders of engine_plan.cuh.
 //
 // Token rows: every sequence owns Tpad = roundup(T, 64) rows; rows past T carry finite values, are masked out as keys and never reach a
 // valid row.  Per-head products run as batched tile GEMMs over z = b * heads + h; head_dim is 64.
@@ -9,7 +9,7 @@
 
 namespace plan {
 
-struct Tower { int C = 0, L = 0, heads = 0, T = 0, Tpad = 0; };
+struct Tower { int C = 0, L = 0, heads = 0, T = 0, Tpad = 0; float ln_eps = 1e-5f; };   // ln_eps: 1e-6 in timm's ViTs (DPT)
 
 struct BlockW {
     const float *ln1, *ln1_b, *ln2, *ln2_b, *b_in, *b_out, *b_fc, *b_proj;
@@ -64,12 +64,12 @@ struct TowerBuilder : Builder {
     // act: the MLP activation epilogue of the tile GEMM (tc::EPI_QUICKGELU for CLIP, tc::EPI_GELU for the SD-2 text encoder).
     void block_fwd(const Tower& t, const BlockW& w, const BlockA& a, int B, int mode, int act) {
         const int C = t.C; const long long M = (long long)B * t.Tpad;
-        layernorm(a.x, M, C, w.ln1, w.ln1_b, a.ln1);
+        layernorm(a.x, M, C, w.ln1, w.ln1_b, a.ln1, t.ln_eps);
         linear(a.ln1, M, C, w.w_in, 3 * C, a.qkv, w.b_in);
         if (mode == 0) attention_core(a.qkv, 3 * C, a.qkv + C, 3 * C, a.qkv + 2 * C, 3 * C, B, t.Tpad, t.Tpad, t.T, t.heads, 64, a.ao, C);
         else attention_materialised(t, a, B, mode == 2);
         linear(a.ao, M, C, w.w_out, C, a.h, w.b_out, a.x);
-        layernorm(a.h, M, C, w.ln2, w.ln2_b, a.ln2);
+        layernorm(a.h, M, C, w.ln2, w.ln2_b, a.ln2, t.ln_eps);
         {
             Mat x{a.ln2, C, M, C}; Mat wm{w.w_fc, C, 4 * C, C};
             Out o; o.p16 = a.act; o.ldc = 4 * C;
