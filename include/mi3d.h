@@ -664,6 +664,59 @@ int mi3d_dpt_forward(mi3d_dpt_t h, const float* img, float* out, mi3d_stream_t s
  * [1,768,24,24], [1,768,12,12] */
 int mi3d_dpt_tap(mi3d_dpt_t h, int i, float* dst, mi3d_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------
+ * B9: BLIP-2 captioner  (replaces transformers' Blip2ForConditionalGeneration.generate(pixel_values) with Salesforce/blip2-opt-2.7b
+ * behind the caption of the reference image when no --text is given, main.py:158-172: EVA ViT-g/14, Q-Former, greedy OPT-2.7B decode)
+ * ------------------------------------------------------------------------------------------------------ */
+typedef struct {
+    int image_size, patch;                                   /* 224, 14 */
+    int vision_width, vision_layers, vision_heads, vision_mlp;   /* 1408, 39, 16, 6144 (head_dim 88; exact GELU; LN eps 1e-6) */
+    int qformer_width, qformer_layers, qformer_heads, qformer_ffn, cross_attention_frequency;   /* 768, 12, 12, 3072, 2 */
+    int num_query_tokens;                                    /* 32 */
+    int opt_width, opt_layers, opt_heads, opt_ffn, vocab;    /* 2560, 32, 32, 10240, 50272 (head_dim 80; ReLU FFN) */
+    int max_positions;                                       /* 2048 (embed_positions has max_positions + 2 rows) */
+    int image_token_index, bos_token_id, eos_token_id;       /* 50265, 2, 50118 */
+} mi3d_blip2_cfg;
+
+typedef struct mi3d_blip2* mi3d_blip2_t;
+
+/* HOST: bytes of device workspace the engine needs (0: a configuration the kernels cannot run); create plans inside it (the
+ * workspace must be zero-filled), NULL on failure */
+size_t mi3d_blip2_workspace_bytes(const mi3d_blip2_cfg* cfg);
+mi3d_blip2_t mi3d_blip2_create(const mi3d_blip2_cfg* cfg, void* workspace, size_t workspace_bytes);
+void mi3d_blip2_destroy(mi3d_blip2_t h);
+/* Parameters are enumerated by transformers' Blip2ForConditionalGeneration.state_dict() names, in its order ("query_tokens" ..
+ * "language_model.model.decoder.layers.{L-1}.final_layer_norm.bias"), without the tied "language_model.lm_head.weight" (lm_head reads
+ * embed_tokens).  OPT's q / k / v projections are stored as row slices of one packed weight.  load: src = fp32 DEVICE tensor in
+ * torch's layout; it may be freed once the stream has passed the call. */
+int mi3d_blip2_num_params(mi3d_blip2_t h);
+const char* mi3d_blip2_param_name(mi3d_blip2_t h, int i);
+int mi3d_blip2_param_shape(mi3d_blip2_t h, int i, int* shape4); /* returns rank */
+int mi3d_blip2_load_param(mi3d_blip2_t h, int i, const float* src, mi3d_stream_t stream);
+/* CUDA-graph replay of the static launch lists, from a list's third call on (`stream` must then be capturable); off by default.
+ * mi3d_blip2_graph_replays: lists currently instantiated. */
+int mi3d_blip2_set_graph_replay(mi3d_blip2_t h, int enable);
+int mi3d_blip2_graph_replays(mi3d_blip2_t h);
+/* pixel_values fp32 [1,3,image_size,image_size] (DEVICE, processor-normalised) -> out fp32 [num_query_tokens, opt_width]
+ * (language_model_inputs = language_projection(Q-Former(vision(pixel_values)))) */
+int mi3d_blip2_encode(mi3d_blip2_t h, const float* pixel_values, float* out, mi3d_stream_t stream);
+/* Greedy caption: the prompt [image_token_index] x num_query_tokens + [bos_token_id], the query rows replaced by language_model_inputs,
+ * then max_new_tokens greedy steps (1 .. 63 - num_query_tokens), each a causal pass over a fixed 64-row window, lm_head on the last
+ * filled row only, argmax with the lowest index on ties.  After eos (< 0: none) no token is appended.  ids (DEVICE int64 [64]): the
+ * prompt and the generated tokens; count (DEVICE int32 [1]): how many of them are valid (num_query_tokens + 1 + n).
+ * forced_ids (DEVICE int64 [max_new_tokens], nullable): teacher forcing, step s appends forced_ids[s] instead of the argmax.
+ * step_logits (DEVICE fp32 [max_new_tokens, vocab], nullable): the last-row logits of every step. */
+int mi3d_blip2_generate(mi3d_blip2_t h, const float* pixel_values, int max_new_tokens, long long eos_token_id, const long long* forced_ids,
+                        long long* ids, int* count, float* step_logits, mi3d_stream_t stream);
+/* the last call's intermediates as fp32 (DEVICE): "image_embeds" [T, vision_width] (T = (image_size / patch)^2 + 1, post_layernorm
+ * applied), "query_output" [num_query_tokens, qformer_width], "language_model_inputs" [num_query_tokens, opt_width] */
+int mi3d_blip2_tap(mi3d_blip2_t h, const char* name, float* dst, mi3d_stream_t stream);
+/* The weight-streaming GEMM on its own: y[M,N] = act(x[M,K] w[N,K]^T + bias (+ residual)), M <= 64, K % 32 == 0; x, w, residual, y
+ * fp16, bias fp32 (nullable), relu != 0: ReLU.  workspace: mi3d_stream_gemm_workspace_bytes(M, N, K) bytes (fp32 partial sums). */
+size_t mi3d_stream_gemm_workspace_bytes(int M, int N, int K);
+int mi3d_stream_gemm_f16(const void* x, const void* w, const float* bias, const void* residual, int relu, void* y, int M, int N, int K,
+                         void* workspace, size_t workspace_bytes, mi3d_stream_t stream);
+
 /* unit-test entry for the hand-written wgmma tf32 tiles of the field forward (3-term split, K-major operands):
  * mode 0 (the only one): d[128,N] = a[128,K] . b[N,K]^T, N in {16, 32, 64}, K in {32, 64, 96, 128}.  fp32 in/out. */
 int mi3d_tf32_tile_test(const float* a, const float* b, float* d, int N, int K, int mode, mi3d_stream_t stream);

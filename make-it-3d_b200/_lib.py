@@ -117,6 +117,9 @@ SYMBOLS = [
     "mi3d_unet_set_graph_replay", "mi3d_unet_graph_replays", "mi3d_unet_forward", "mi3d_unet_backward", "mi3d_unet_debug_tensor",
     "mi3d_dpt_workspace_bytes", "mi3d_dpt_create", "mi3d_dpt_destroy", "mi3d_dpt_num_params", "mi3d_dpt_param_name", "mi3d_dpt_param_shape",
     "mi3d_dpt_load_param", "mi3d_dpt_forward", "mi3d_dpt_tap",
+    "mi3d_blip2_workspace_bytes", "mi3d_blip2_create", "mi3d_blip2_destroy", "mi3d_blip2_num_params", "mi3d_blip2_param_name",
+    "mi3d_blip2_param_shape", "mi3d_blip2_load_param", "mi3d_blip2_set_graph_replay", "mi3d_blip2_graph_replays", "mi3d_blip2_encode",
+    "mi3d_blip2_generate", "mi3d_blip2_tap", "mi3d_stream_gemm_workspace_bytes", "mi3d_stream_gemm_f16",
 ]
 
 
