@@ -717,6 +717,31 @@ size_t mi3d_stream_gemm_workspace_bytes(int M, int N, int K);
 int mi3d_stream_gemm_f16(const void* x, const void* w, const float* bias, const void* residual, int relu, void* y, int M, int N, int K,
                          void* workspace, size_t workspace_bytes, mi3d_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------
+ * B10: mesh export  (replaces PyMCubes' marching_cubes and the xatlas / nvdiffrast texel pass of NeRFRenderer.export_mesh,
+ * nerf/renderer.py:157-330; csrc/mesh.cu, oracle/mesh_ref.py)
+ * ------------------------------------------------------------------------------------------------------ */
+/* Marching cubes (Bourke / Bloyd 256-case table) over volume fp32 [nx,ny,nz] (C order, (i,j,k) <-> (x,y,z)).  A corner is inside iff
+ * sigma > iso_eff with iso_eff = iso, or min(iso, *iso_dev) when iso_dev (DEVICE scalar) is given.  One vertex per crossing grid edge,
+ * owned by its lower end point p, at p + t e_a, t = (iso_eff - s_p) / (s_{p+e_a} - s_p) in fp32 without contraction; numbered by grid
+ * point (C order), then axis x < y < z.  Faces: cells in C order, triangles in table order, right-hand normal pointing out of the
+ * solid (toward sigma <= iso_eff).  Output order depends on the data only (no atomics decide it).
+ * workspace: mi3d_mc_workspace_bytes(nx, ny, nz) bytes; 0 (and MI3D_ERR_ARG from the calls) when a dimension is below 2 or a vertex
+ * or face count could overflow int32 (3 nx ny nz or 5 (nx-1)(ny-1)(nz-1) above INT32_MAX).
+ * mi3d_mc_count writes counts = (V, F) (DEVICE int32 [2]) and fills the workspace; mi3d_mc_emit, on the same workspace, volume and
+ * threshold, writes vertices fp32 [V,3] = position * scale + offset and faces int32 [F,3]. */
+size_t mi3d_mc_workspace_bytes(uint32_t nx, uint32_t ny, uint32_t nz);
+int mi3d_mc_count(const float* volume, uint32_t nx, uint32_t ny, uint32_t nz, float iso, const float* iso_dev, void* workspace,
+                  int* counts, mi3d_stream_t stream);
+int mi3d_mc_emit(const float* volume, uint32_t nx, uint32_t ny, uint32_t nz, float iso, const float* iso_dev, const void* workspace,
+                 float scale, float offset, float* vertices, int* faces, mi3d_stream_t stream);
+/* Texel pass of the per-face texture atlas (layout: T x T texels, cells of c x c texels, n cells per row, faces 2p / 2p+1 in cell p;
+ * nerf/mesh.py::atlas_layout).  points fp32 [T*T,3]: each owned texel centre mapped through its face's affine UV -> xyz map and clamped
+ * to [-bound, bound] (0 for unowned texels); owner int32 [T*T]: the face (-1: none); vt fp32 [3F,2]: UVs in [0,1] of the faces' corners
+ * (u along texel columns, v along rows). */
+int mi3d_mesh_atlas_texels(const float* vertices, const int* faces, uint32_t F, uint32_t T, uint32_t c, uint32_t n, float bound,
+                           float* points, int* owner, float* vt, mi3d_stream_t stream);
+
 /* unit-test entry for the hand-written wgmma tf32 tiles of the field forward (3-term split, K-major operands):
  * mode 0 (the only one): d[128,N] = a[128,K] . b[N,K]^T, N in {16, 32, 64}, K in {32, 64, 96, 128}.  fp32 in/out. */
 int mi3d_tf32_tile_test(const float* a, const float* b, float* d, int N, int K, int mode, mi3d_stream_t stream);

@@ -295,6 +295,13 @@ class NeRFRenderer(nn.Module):
         self.mean_count = 0                            # unused under force_all_rays=True (nerf/utils.py:498)
         self.local_step = 0
 
+    @torch.no_grad()
+    def export_mesh(self, path, resolution=None, S=128):
+        """nerf/renderer.py:157-330: marching cubes over the density volume and a baked albedo atlas, written as path/mesh.obj,
+        mesh.mtl and albedo.png (nerf/mesh.py)."""
+        from . import mesh
+        mesh.export_mesh(self, path, resolution, S)
+
     def render(self, rays_o, rays_d, depth_scale=None, staged=False, max_ray_batch=4096, **kwargs):
         """nerf/renderer.py:642-677 (cuda_ray never stages)."""
         return self.run_cuda(rays_o, rays_d, depth_scale, **kwargs)
