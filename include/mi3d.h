@@ -565,6 +565,33 @@ int mi3d_points_render_backward(const float* points, uint32_t P, uint32_t C, con
 int mi3d_points_zbuffer_visible(const double* points, uint32_t P, const double* cam_k, const double* world2cam, uint32_t H, uint32_t W,
                                 unsigned long long* zbuf, uint8_t* mask, mi3d_stream_t stream);
 
+/* B5, point-cloud construction (load_views, nerf/refine_utils.py:61-152, :335-410; csrc/views.cu, oracle/views_ref.py).  Square
+ * H x W views only (H == W, else MI3D_ERR_ARG).  Images are row-major uint8 / uint16 [H,W]; depth is depth_u16 / 1000.0.
+ * HOST: workspace bytes shared by the calls below (0: invalid size). */
+size_t mi3d_views_workspace_bytes(uint32_t H, uint32_t W);
+/* out[p] (0/1) = mask eroded with erode_k x erode_k == 255 (cv2.erode, window clipped to the image), and, when canny_thresh >= 0, not
+ * within the dilate_k x dilate_k dilation of Canny(uint8(depth * eroded * 255) wrapped modulo 256, canny_thresh, canny_thresh).
+ * Nullable outputs: masked_depth fp32 [H,W] = float32(depth * out); eroded (raw min), edges (0/255), dilated (0/255).  Odd k <= 31. */
+int mi3d_views_mask(const uint16_t* depth, const uint8_t* mask, uint32_t H, uint32_t W, uint32_t erode_k, int canny_thresh, uint32_t dilate_k,
+                    uint8_t* out, float* masked_depth, uint8_t* eroded, uint8_t* edges, uint8_t* dilated, void* workspace,
+                    size_t workspace_bytes, mi3d_stream_t stream);
+/* out[p] (0/1) = alphamask[p] == 1 and not covered, where covered = the erode_k x erode_k erosion of (uint8(render * 255) / 255 > 0.9);
+ * render fp32 [H,W] (one channel of the canonical cloud rendered with unit colours).  quant (nullable) = uint8(render * 255). */
+int mi3d_views_cover_mask(const float* render, const uint8_t* alphamask, uint32_t H, uint32_t W, uint32_t erode_k, uint8_t* out, uint8_t* quant,
+                          void* workspace, size_t workspace_bytes, mi3d_stream_t stream);
+/* points fp64 [H*W,3]: the world points (inv(K) [x, y, 1] D, then c2w) of the pixels with mask != 0, in row-major pixel order, and
+ * count (DEVICE int32) of them; rows [count, H*W) are NaN.  kinv [9], c2w [12] (rows 0..2 of the pose) are DEVICE fp64.  With
+ * cano_depth (fp32 [H,W], DEVICE), cam_k [9] and cano_w2c [12]: points whose canonical projection, rounded half to even, samples
+ * (bilinear, zero padding, align_corners=False) a depth d with -0.2 <= z - d <= 1/H are dropped. */
+int mi3d_views_backproject(const uint16_t* depth, const uint8_t* mask, uint32_t H, uint32_t W, const double* kinv, const double* c2w,
+                           const double* cam_k, const double* cano_w2c, const float* cano_depth, double* points, int* count, void* workspace,
+                           size_t workspace_bytes, mi3d_stream_t stream);
+/* points_out fp64 [count,3] = points[keep != 0] in order (P <= H*W) and colours fp32 [count,3] sampled bilinearly at their projection
+ * through cam_k / world2cam (DEVICE fp64) from exactly one of img_f32 [H,W,3] or img_u8 [H,W,3] (read as u8 / 255.0).  count: DEVICE. */
+int mi3d_views_compact_colour(const double* points, uint32_t P, const uint8_t* keep, const double* cam_k, const double* world2cam,
+                              const float* img_f32, const uint8_t* img_u8, uint32_t H, uint32_t W, double* points_out, float* colours,
+                              int* count, void* workspace, size_t workspace_bytes, mi3d_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------------
  * B6: refine-stage contextual loss  (replaces the contextual_loss package's ContextualLoss(use_vgg=True, vgg_layer='relu5_4',
  * loss_type='cosine'), nerf/utils.py:36, 455-457, 810, 882)

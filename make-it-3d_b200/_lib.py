@@ -121,6 +121,7 @@ SYMBOLS = [
     "mi3d_blip2_param_shape", "mi3d_blip2_load_param", "mi3d_blip2_set_graph_replay", "mi3d_blip2_graph_replays", "mi3d_blip2_encode",
     "mi3d_blip2_generate", "mi3d_blip2_tap", "mi3d_stream_gemm_workspace_bytes", "mi3d_stream_gemm_f16",
     "mi3d_mc_workspace_bytes", "mi3d_mc_count", "mi3d_mc_emit", "mi3d_mesh_atlas_texels",
+    "mi3d_views_workspace_bytes", "mi3d_views_mask", "mi3d_views_cover_mask", "mi3d_views_backproject", "mi3d_views_compact_colour",
 ]
 
 
@@ -149,6 +150,7 @@ def lib():
         _lib.mi3d_sumsq_workspace_bytes.restype = C.c_size_t
         _lib.mi3d_render_eval_workspace_bytes.restype = C.c_size_t
         _lib.mi3d_mc_workspace_bytes.restype = C.c_size_t
+        _lib.mi3d_views_workspace_bytes.restype = C.c_size_t
         for name in ("mi3d_sd_workspace_bytes", "mi3d_sd_weight_bytes"):
             if hasattr(_lib, name):
                 getattr(_lib, name).restype = C.c_size_t
