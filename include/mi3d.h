@@ -362,6 +362,31 @@ int mi3d_adan_step(float* param, float* grad, float* exp_avg, float* exp_avg_sq,
                    const float* total_sumsq, const mi3d_adan_cfg* cfg, mi3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------
+ * Planned engines: SD (B3), the SD-2 text encoder (B3'), CLIP (B4), the contextual loss (B6), the refine U-Net (B7), DPT (B8) and
+ * BLIP-2 (B9).  Each is made by its mi3d_<engine>_workspace_bytes / mi3d_<engine>_create (HOST: bytes of device workspace the engine
+ * needs, 0 for a configuration it cannot run; create plans the launch lists inside the caller's workspace, NULL on failure), and all
+ * share one handle type and the lifecycle below.  An engine's own entry points return MI3D_ERR_ARG for another engine's handle.
+ * ------------------------------------------------------------------------------------------------------ */
+typedef struct mi3d_engine* mi3d_engine_t;
+
+void mi3d_engine_destroy(mi3d_engine_t h);
+/* The parameter registry, in the engine's state_dict order (its section names the naming).  A '#...' suffix marks a derived copy,
+ * written from the base tensor.  param_name: NULL, param_shape: -1 for an index out of range. */
+int mi3d_engine_num_params(mi3d_engine_t h);
+const char* mi3d_engine_param_name(mi3d_engine_t h, int i);
+int mi3d_engine_param_shape(mi3d_engine_t h, int i, int* shape4); /* returns rank */
+/* src = fp32 DEVICE tensor in torch's layout (for a '#' entry: the base tensor); it may be freed once the stream has passed the call.
+ * partner_src (nullable): the second tensor of a pair written together, the ".bias" of an SD GEGLU proj weight.  The refine U-Net
+ * reads its parameters on every call instead (MI3D_ERR_ARG). */
+int mi3d_engine_load_param(mi3d_engine_t h, int i, const float* src, const float* partner_src, mi3d_stream_t stream);
+/* CUDA-graph replay of the engine's static launch lists: from its third call on a list is one cudaGraphLaunch.  `stream` of the
+ * run calls must then be capturable (not the legacy default stream).  Off by default.  graph_replays: lists currently instantiated. */
+int mi3d_engine_set_graph_replay(mi3d_engine_t h, int enable);
+int mi3d_engine_graph_replays(mi3d_engine_t h);
+/* debug tap: device pointer + size of a named intermediate inside the workspace (the engine's section lists the names) */
+int mi3d_engine_debug_tensor(mi3d_engine_t h, const char* name, void** ptr, size_t* bytes);
+
+/* ------------------------------------------------------------------------------------------------------
  * B3: Stable-Diffusion guidance  (replaces the diffusers/cuDNN/cuBLAS calls behind nerf/sd.py:117-174, :212-220)
  * ------------------------------------------------------------------------------------------------------ */
 
@@ -419,52 +444,35 @@ typedef struct {
     int decoder;              /* != 0: also plan the decoder (mi3d_sd_decode; the denoise side branch of nerf/sd.py:153-159) */
 } mi3d_vae_cfg;
 
-typedef struct mi3d_sd* mi3d_sd_t;
-
-/* HOST: bytes of device workspace the engine needs (weights + activations + tapes; nothing else is ever allocated) */
+/* weights + activations + tapes; nothing else is ever allocated */
 size_t mi3d_sd_workspace_bytes(const mi3d_unet_cfg* unet, const mi3d_vae_cfg* vae);
-/* HOST: plans the launch lists inside `workspace` (device memory owned by the caller); NULL on failure */
-mi3d_sd_t mi3d_sd_create(const mi3d_unet_cfg* unet, const mi3d_vae_cfg* vae, void* workspace, size_t workspace_bytes);
-void mi3d_sd_destroy(mi3d_sd_t h);
-
+mi3d_engine_t mi3d_sd_create(const mi3d_unet_cfg* unet, const mi3d_vae_cfg* vae, void* workspace, size_t workspace_bytes);
 /* Parameters are enumerated by their diffusers state_dict names ("down_blocks.0.resnets.0.conv1.weight", VAE names are
- * prefixed as in AutoencoderKL: "encoder....", "quant_conv...."; a '#...' suffix marks a derived copy of the base tensor).
- * load: src = fp32 DEVICE tensor in the diffusers layout; partner_src = the matching ".bias" for GEGLU proj weights. */
-int mi3d_sd_num_params(mi3d_sd_t h);
-const char* mi3d_sd_param_name(mi3d_sd_t h, int i);
-long long mi3d_sd_param_numel(mi3d_sd_t h, int i);
-int mi3d_sd_param_shape(mi3d_sd_t h, int i, int* shape4); /* returns rank */
-int mi3d_sd_load_param(mi3d_sd_t h, int i, const float* src, const float* partner_src, mi3d_stream_t stream);
+ * prefixed as in AutoencoderKL: "encoder....", "quant_conv....").  Graph replay covers the three static launch lists (U-Net,
+ * VAE encode, VAE input-gradient).  Debug taps: "unet.mid", "vae.grad_in", ... */
 
 /* replaces nerf/sd.py:124 (F.interpolate to 512) + :133,212-220 (encode_imgs: vae.encode(2x-1).latent_dist.sample()*0.18215)
  * pred_rgb [1,3,H,W] fp32 in [0,1]; eps_posterior, latents [1,4,h,w] fp32 (h = image_hw/8). */
-int mi3d_sd_encode(mi3d_sd_t h, const float* pred_rgb, int H, int W, const float* eps_posterior, float* latents, mi3d_stream_t stream);
+int mi3d_sd_encode(mi3d_engine_t h, const float* pred_rgb, int H, int W, const float* eps_posterior, float* latents, mi3d_stream_t stream);
 /* the autograd half of latents.backward(gradient=grad) (nerf/sd.py:171): d latents -> d pred_rgb, weights frozen */
-int mi3d_sd_encode_backward(mi3d_sd_t h, const float* grad_latents, const float* eps_posterior, int H, int W, float* grad_pred_rgb,
+int mi3d_sd_encode_backward(mi3d_engine_t h, const float* grad_latents, const float* eps_posterior, int H, int W, float* grad_pred_rgb,
                             mi3d_stream_t stream);
 /* replaces nerf/sd.py:138-170: scheduler.add_noise, unet([x,x], t, text_embeddings).sample, CFG (text + gs*(text-uncond)),
  * w = 1 - alphas[t], grad = nan_to_num(w*(noise_pred - noise)).  t: DEVICE int64 scalar; alphas_cumprod: DEVICE fp32 [1000];
  * text_embeddings fp32 [2,77,cross_dim] (uncond first); noise_pred / grad (nullable) fp32 [1,4,h,w]. */
-int mi3d_sd_unet_sds(mi3d_sd_t h, const float* latents, const float* noise, const long long* t, const float* alphas_cumprod,
+int mi3d_sd_unet_sds(mi3d_engine_t h, const float* latents, const float* noise, const long long* t, const float* alphas_cumprod,
                      const float* text_embeddings, float guidance_scale, float* noise_pred, float* grad, mi3d_stream_t stream);
 /* The "denoise" side branch of train_step (nerf/sd.py:153-159), taken on non-large views when t <= 0.4 T:
  * replaces scheduler.step (DDIM, eta 0, t -> t-1; fp32 [1,4,h,w], n = 4*h*w elements) and decode_latents (nerf/sd.py:201-210:
  * vae.decode(latents / 0.18215) -> (x/2 + 0.5).clamp(0,1); imgs fp32 [1,3,image_hw,image_hw]).  Forward only, like the reference. */
 int mi3d_sd_ddim_step(const float* noise_pred, const float* latents_noisy, const long long* t, const float* alphas_cumprod,
                       float* prev_sample, int n, mi3d_stream_t stream);
-int mi3d_sd_decode(mi3d_sd_t h, const float* latents, float* imgs, mi3d_stream_t stream);
+int mi3d_sd_decode(mi3d_engine_t h, const float* latents, float* imgs, mi3d_stream_t stream);
 /* live timing of the tensor-core tile kernel: enable=1 starts recording CUDA events around every launch; enable=0 stops and
  * returns the summed kernel time (ms) and launch count (HOST pointers; synchronises on the recorded events). */
-int mi3d_sd_profile(mi3d_sd_t h, int enable, float* gemm_ms_host, int* launches_host);
+int mi3d_sd_profile(mi3d_engine_t h, int enable, float* gemm_ms_host, int* launches_host);
 /* same, and (enable=0) also writes one text line per timed launch to dump_path_host: "M N K block_n splits conv batch epi ms" */
-int mi3d_sd_profile_dump(mi3d_sd_t h, int enable, float* gemm_ms_host, int* launches_host, const char* dump_path_host);
-/* CUDA-graph replay of the three static launch lists (U-Net, VAE encode, VAE input-gradient): from its third call on a list is
- * one cudaGraphLaunch.  `stream` of the run calls must then be capturable (not the legacy default stream).  Off by default at the
- * C level; nerf/sd.py turns it on together with an engine-owned stream.  mi3d_sd_graph_replays: lists currently instantiated. */
-int mi3d_sd_set_graph_replay(mi3d_sd_t h, int enable);
-int mi3d_sd_graph_replays(mi3d_sd_t h);
-/* debug tap: device pointer + size of a named intermediate ("unet.mid", "vae.grad_in", ...) */
-int mi3d_sd_debug_tensor(mi3d_sd_t h, const char* name, void** ptr, size_t* bytes);
+int mi3d_sd_profile_dump(mi3d_engine_t h, int enable, float* gemm_ms_host, int* launches_host, const char* dump_path_host);
 
 /* ------------------------------------------------------------------------------------------------------
  * B3': Stable Diffusion 2 text encoder  (replaces transformers' CLIPTextModel behind get_text_embeds, nerf/sd.py:68-85: OpenCLIP
@@ -476,26 +484,14 @@ typedef struct {
     int max_batch;             /* prompts per call (1..8); 2 encodes [negative, positive] in one pass */
 } mi3d_sd_text_cfg;
 
-typedef struct mi3d_sd_text* mi3d_sd_text_t;
-
-/* HOST: bytes of device workspace the engine needs (0: invalid configuration); create plans inside it, NULL on failure */
 size_t mi3d_sd_text_workspace_bytes(const mi3d_sd_text_cfg* cfg);
-mi3d_sd_text_t mi3d_sd_text_create(const mi3d_sd_text_cfg* cfg, void* workspace, size_t workspace_bytes);
-void mi3d_sd_text_destroy(mi3d_sd_text_t h);
+mi3d_engine_t mi3d_sd_text_create(const mi3d_sd_text_cfg* cfg, void* workspace, size_t workspace_bytes);
 /* Parameters are enumerated by transformers' CLIPTextModel state_dict names, in its order ("text_model.embeddings.token_embedding.weight"
  * .. "text_model.final_layer_norm.bias"; no position_ids).  The separate q / k / v projections are stored as row slices of one packed
- * weight.  load: src = fp32 DEVICE tensor in torch's layout; it may be freed once the stream has passed the call. */
-int mi3d_sd_text_num_params(mi3d_sd_text_t h);
-const char* mi3d_sd_text_param_name(mi3d_sd_text_t h, int i);
-int mi3d_sd_text_param_shape(mi3d_sd_text_t h, int i, int* shape4); /* returns rank */
-int mi3d_sd_text_load_param(mi3d_sd_text_t h, int i, const float* src, mi3d_stream_t stream);
-/* CUDA-graph replay of the static launch lists, from a list's third call on (`stream` must then be capturable); off by default.
- * mi3d_sd_text_graph_replays: lists currently instantiated. */
-int mi3d_sd_text_set_graph_replay(mi3d_sd_text_t h, int enable);
-int mi3d_sd_text_graph_replays(mi3d_sd_text_t h);
+ * weight. */
 /* ids int64 [B,context_len] (DEVICE) -> out fp32 [B,context_len,width] (DEVICE): last_hidden_state, final_layer_norm applied to every
  * position.  Causal attention, no padding mask.  Ids outside [0, vocab) are clamped into it.  B <= max_batch. */
-int mi3d_sd_text_encode(mi3d_sd_text_t h, const long long* ids, int B, float* out, mi3d_stream_t stream);
+int mi3d_sd_text_encode(mi3d_engine_t h, const long long* ids, int B, float* out, mi3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------
  * B4: CLIP losses  (replaces openai CLIP's encode_image / encode_text behind the per-step CLIP losses, nerf/utils.py:436-453, 561-563,
@@ -510,32 +506,20 @@ typedef struct {
     int max_batch;             /* images / prompts per call (1..8); 2 encodes [rendered, reference] in one pass */
 } mi3d_clip_cfg;
 
-typedef struct mi3d_clip* mi3d_clip_t;
-
-/* HOST: bytes of device workspace the engine needs (0: invalid configuration); create plans inside it, NULL on failure */
 size_t mi3d_clip_workspace_bytes(const mi3d_clip_cfg* cfg);
-mi3d_clip_t mi3d_clip_create(const mi3d_clip_cfg* cfg, void* workspace, size_t workspace_bytes);
-void mi3d_clip_destroy(mi3d_clip_t h);
+mi3d_engine_t mi3d_clip_create(const mi3d_clip_cfg* cfg, void* workspace, size_t workspace_bytes);
 /* Parameters are enumerated by openai CLIP's state_dict names ("visual.conv1.weight", "transformer.resblocks.0.attn.in_proj_weight",
- * "visual.proj", ...; a '#...' suffix marks a derived copy of the base tensor).  load: src = fp32 DEVICE tensor in openai's layout. */
-int mi3d_clip_num_params(mi3d_clip_t h);
-const char* mi3d_clip_param_name(mi3d_clip_t h, int i);
-int mi3d_clip_param_shape(mi3d_clip_t h, int i, int* shape4); /* returns rank */
-int mi3d_clip_load_param(mi3d_clip_t h, int i, const float* src, mi3d_stream_t stream);
-/* CUDA-graph replay of the static launch lists, from a list's third call on (`stream` must then be capturable); off by default.
- * mi3d_clip_graph_replays: lists currently instantiated. */
-int mi3d_clip_set_graph_replay(mi3d_clip_t h, int enable);
-int mi3d_clip_graph_replays(mi3d_clip_t h);
+ * "visual.proj", ...), in openai's layout. */
 /* img fp32 [B,3,H,W] -> feats fp32 [B,embed_dim] (encode_image).  aug != 0: the reference's aug first (Resize((res,res)): bilinear,
  * align_corners=False, no antialiasing; then Normalize with CLIP's mean / std); aug = 0: img is already augmented and res x res.
  * need_grad != 0 keeps a tape for mi3d_clip_encode_image_backward; any image forward replaces the previous tape.  B <= max_batch. */
-int mi3d_clip_encode_image(mi3d_clip_t h, const float* img, int B, int H, int W, int aug, int need_grad, float* feats, mi3d_stream_t stream);
+int mi3d_clip_encode_image(mi3d_engine_t h, const float* img, int B, int H, int W, int aug, int need_grad, float* feats, mi3d_stream_t stream);
 /* input gradient of the first n_grad images of the last (taped) image forward: dfeats fp32 [n_grad,embed_dim] -> dimg fp32
  * [n_grad,3,H,W] (overwritten).  Weights frozen.  MI3D_ERR_ARG without a tape or with n_grad outside 1..B of that forward. */
-int mi3d_clip_encode_image_backward(mi3d_clip_t h, const float* dfeats, int n_grad, float* dimg, mi3d_stream_t stream);
+int mi3d_clip_encode_image_backward(mi3d_engine_t h, const float* dfeats, int n_grad, float* dimg, mi3d_stream_t stream);
 /* tokens int64 [B,context_len] (clip.tokenize ids; the features are taken at each row's argmax, the EOT token) -> feats fp32
  * [B,embed_dim] (encode_text, causal attention).  Ids outside [0, vocab) are clamped into it. */
-int mi3d_clip_encode_text(mi3d_clip_t h, const long long* tokens, int B, float* feats, mi3d_stream_t stream);
+int mi3d_clip_encode_text(mi3d_engine_t h, const long long* tokens, int B, float* feats, mi3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------
  * B5: refine-stage point renderer  (replaces pytorch3d's rasterize_points + alpha_composite as render_point drives them,
@@ -600,32 +584,19 @@ typedef struct {
     int N, H, W;               /* images per call (1..16) and their size (16..4096 each): the plan is static for this shape */
 } mi3d_cx_cfg;
 
-typedef struct mi3d_cx* mi3d_cx_t;
-
-/* HOST: bytes of device workspace the engine needs (0: invalid configuration); create plans inside it, NULL on failure */
 size_t mi3d_cx_workspace_bytes(const mi3d_cx_cfg* cfg);
-mi3d_cx_t mi3d_cx_create(const mi3d_cx_cfg* cfg, void* workspace, size_t workspace_bytes);
-void mi3d_cx_destroy(mi3d_cx_t h);
-/* Parameters carry the package's state_dict names, "vgg_model.slice1.0.weight" .. "vgg_model.slice5.34.bias" (a '#dgrad' suffix
- * marks a derived copy, written when its base tensor is loaded).  load: src = fp32 DEVICE tensor in torch's layout. */
-int mi3d_cx_num_params(mi3d_cx_t h);
-const char* mi3d_cx_param_name(mi3d_cx_t h, int i);
-int mi3d_cx_param_shape(mi3d_cx_t h, int i, int* shape4); /* returns rank */
-int mi3d_cx_load_param(mi3d_cx_t h, int i, const float* src, mi3d_stream_t stream);
-/* CUDA-graph replay of the static launch lists, from a list's third call on (`stream` must then be capturable); off by default.
- * mi3d_cx_graph_replays: lists currently instantiated. */
-int mi3d_cx_set_graph_replay(mi3d_cx_t h, int enable);
-int mi3d_cx_graph_replays(mi3d_cx_t h);
+mi3d_engine_t mi3d_cx_create(const mi3d_cx_cfg* cfg, void* workspace, size_t workspace_bytes);
+/* Parameters carry the package's state_dict names, "vgg_model.slice1.0.weight" .. "vgg_model.slice5.34.bias" (the '#dgrad' copy of
+ * conv1_1 is written when its base tensor is loaded; loading the '#dgrad' entry itself does nothing).  Debug tap: "relu5_4", fp16
+ * NHWC [2N,H/16,W/16,512], the x images first. */
 /* x, y fp32 [N,3,H,W] -> loss: DEVICE fp32 scalar.  ImageNet normalisation, VGG19 features[0:36] of x and y in one batched pass
  * (fp16 storage, fp32 accumulation), then in fp32: centring by y's channel mean over batch and positions, L2 normalisation,
  * d = 1 - cos, d / (min_j d + 1e-5), w = exp((1 - .) / band_width), cx = w / sum_j w, loss = mean_n -log(mean_j max_i cx + 1e-5).
  * need_grad != 0 keeps the tape for mi3d_cx_backward; any forward replaces it. */
-int mi3d_cx_forward(mi3d_cx_t h, const float* x, const float* y, float band_width, int need_grad, float* loss, mi3d_stream_t stream);
+int mi3d_cx_forward(mi3d_engine_t h, const float* x, const float* y, float band_width, int need_grad, float* loss, mi3d_stream_t stream);
 /* dx fp32 [N,3,H,W] (overwritten) = dloss * d loss / d x of the last forward; dloss: DEVICE fp32 scalar.  No gradient for y or the
  * weights.  MI3D_ERR_ARG without a tape. */
-int mi3d_cx_backward(mi3d_cx_t h, const float* dloss, float* dx, mi3d_stream_t stream);
-/* debug tap: device pointer + size of a named intermediate ("relu5_4": fp16 NHWC [2N,H/16,W/16,512], the x images first) */
-int mi3d_cx_debug_tensor(mi3d_cx_t h, const char* name, void** ptr, size_t* bytes);
+int mi3d_cx_backward(mi3d_engine_t h, const float* dloss, float* dx, mi3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------
  * B7: refine-stage gated U-Net  (replaces the reference's nerf/unet.py UNet(num_input_channels=3+16) with its defaults:
@@ -635,61 +606,39 @@ typedef struct {
     int N, H, W;               /* images per call (1..16) and the finest level's size (4..4096 each, multiples of 4): the plan is static */
 } mi3d_unet_shape;
 
-typedef struct mi3d_unet* mi3d_unet_t;
-
-/* HOST: bytes of device workspace the engine needs (0: invalid configuration); create plans inside it, NULL on failure */
 size_t mi3d_unet_workspace_bytes(const mi3d_unet_shape* cfg);
-mi3d_unet_t mi3d_unet_create(const mi3d_unet_shape* cfg, void* workspace, size_t workspace_bytes);
-void mi3d_unet_destroy(mi3d_unet_t h);
+mi3d_engine_t mi3d_unet_create(const mi3d_unet_shape* cfg, void* workspace, size_t workspace_bytes);
 /* The registry lists the reference's 41 state_dict entries in its order ("start.block.conv_f.weight" .. "final.0.0.bias"), parameters
- * and BatchNorm buffers alike (shape rank 0: num_batches_tracked). */
-int mi3d_unet_num_params(mi3d_unet_t h);
-const char* mi3d_unet_param_name(mi3d_unet_t h, int i);
-int mi3d_unet_param_shape(mi3d_unet_t h, int i, int* shape4); /* returns rank */
-/* CUDA-graph replay of the static launch lists, from a list's third call on (`stream` must then be capturable); off by default.
- * mi3d_unet_graph_replays: lists currently instantiated. */
-int mi3d_unet_set_graph_replay(mi3d_unet_t h, int enable);
-int mi3d_unet_graph_replays(mi3d_unet_t h);
+ * and BatchNorm buffers alike (shape rank 0: num_batches_tracked); they are passed to every call (state), not loaded.  Debug taps:
+ * fp32 NCHW "cat1", "cat2", "d2", "up2", "up1", "out"; "in64" is a channel slice of "cat1". */
 /* x0 [N,19,H,W], x1 [N,19,H/2,W/2], x2 [N,19,H/4,W/4] fp32 -> out [N,3,H,W] fp32.  state: one DEVICE pointer per registry entry, in
  * registry order, in torch's layouts: the fp32 parameters are read on every call (no reload after an optimizer step).  train != 0:
  * BatchNorm with batch statistics, and the fp32 running_mean / running_var and the int64 num_batches_tracked given are updated
  * once (momentum 0.1, unbiased variance); a NULL buffer pointer skips its update; MI3D_ERR_ARG when N x H/4 x W/4 < 2 (one value
  * per channel).  train == 0: the running statistics are read.
  * need_grad != 0 keeps the tape for mi3d_unet_backward; any forward replaces it. */
-int mi3d_unet_forward(mi3d_unet_t h, const float* x0, const float* x1, const float* x2, void* const* state, int train, int need_grad,
+int mi3d_unet_forward(mi3d_engine_t h, const float* x0, const float* x1, const float* x2, void* const* state, int train, int need_grad,
                       float* out, mi3d_stream_t stream);
 /* dout fp32 [N,3,H,W] -> dx0, dx1, dx2 (overwritten) and, for every parameter entry whose grads[i] is not NULL, its fp32 gradient
  * (overwritten; buffer entries are ignored), for the last forward.  May run any number of times per forward.  MI3D_ERR_ARG without
  * a tape. */
-int mi3d_unet_backward(mi3d_unet_t h, const float* dout, float* dx0, float* dx1, float* dx2, float* const* grads, mi3d_stream_t stream);
-/* debug tap: device pointer + size of a named fp32 NCHW intermediate ("cat1", "cat2", "d2", "up2", "up1", "out"; "in64" is a
- * channel slice of "cat1") */
-int mi3d_unet_debug_tensor(mi3d_unet_t h, const char* name, void** ptr, size_t* bytes);
+int mi3d_unet_backward(mi3d_engine_t h, const float* dout, float* dx0, float* dx1, float* dx2, float* const* grads, mi3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------
  * B8: DPT-Hybrid depth model  (replaces the reference's DPT/dpt DPTDepthModel(backbone="vitb_rn50_384", non_negative=True) and timm
  * behind the reference image's depth prior, main.py:111-127, 196-214: ResNet-50v2 trunk, ViT-B/16 on 577 tokens, RefineNet decoder)
  * ------------------------------------------------------------------------------------------------------ */
-typedef struct mi3d_dpt* mi3d_dpt_t;
-
-/* HOST: bytes of device workspace the engine needs (one shape: a [1,3,384,384] image); create plans inside it (the workspace must be
- * zero-filled: padding rows and channels are never written), NULL on failure */
+/* one shape: a [1,3,384,384] image; the workspace must be zero-filled (padding rows and channels are never written) */
 size_t mi3d_dpt_workspace_bytes(void);
-mi3d_dpt_t mi3d_dpt_create(void* workspace, size_t workspace_bytes);
-void mi3d_dpt_destroy(mi3d_dpt_t h);
+mi3d_engine_t mi3d_dpt_create(void* workspace, size_t workspace_bytes);
 /* Parameters are enumerated by the reference's DPTDepthModel.state_dict() names ("pretrained.model.cls_token" ..
  * "scratch.output_conv.4.bias"), every tensor the forward reads and nothing else (not pretrained.model.norm.*, pretrained.model.head.*
- * or scratch.refinenet4.resConfUnit1.*).  The trunk's convs are weight-standardised at load.  load: src = fp32 DEVICE tensor in torch's
- * layout; it may be freed once the stream has passed the call. */
-int mi3d_dpt_num_params(mi3d_dpt_t h);
-const char* mi3d_dpt_param_name(mi3d_dpt_t h, int i);
-int mi3d_dpt_param_shape(mi3d_dpt_t h, int i, int* shape4); /* returns rank */
-int mi3d_dpt_load_param(mi3d_dpt_t h, int i, const float* src, mi3d_stream_t stream);
+ * or scratch.refinenet4.resConfUnit1.*).  The trunk's convs are weight-standardised at load.  The forward always runs eagerly. */
 /* img fp32 [1,3,384,384] (resized and normalised, DEVICE) -> out fp32 [1,384,384] inverse depth (DEVICE) */
-int mi3d_dpt_forward(mi3d_dpt_t h, const float* img, float* out, mi3d_stream_t stream);
+int mi3d_dpt_forward(mi3d_engine_t h, const float* img, float* out, mi3d_stream_t stream);
 /* the last forward's reassembled backbone features layer_1 .. layer_4 (i = 0..3) as fp32 NCHW: [1,256,96,96], [1,512,48,48],
  * [1,768,24,24], [1,768,12,12] */
-int mi3d_dpt_tap(mi3d_dpt_t h, int i, float* dst, mi3d_stream_t stream);
+int mi3d_dpt_tap(mi3d_engine_t h, int i, float* dst, mi3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------
  * B9: BLIP-2 captioner  (replaces transformers' Blip2ForConditionalGeneration.generate(pixel_values) with Salesforce/blip2-opt-2.7b
@@ -705,39 +654,26 @@ typedef struct {
     int image_token_index, bos_token_id, eos_token_id;       /* 50265, 2, 50118 */
 } mi3d_blip2_cfg;
 
-typedef struct mi3d_blip2* mi3d_blip2_t;
-
-/* HOST: bytes of device workspace the engine needs (0: a configuration the kernels cannot run); create plans inside it (the
- * workspace must be zero-filled), NULL on failure */
+/* the workspace must be zero-filled */
 size_t mi3d_blip2_workspace_bytes(const mi3d_blip2_cfg* cfg);
-mi3d_blip2_t mi3d_blip2_create(const mi3d_blip2_cfg* cfg, void* workspace, size_t workspace_bytes);
-void mi3d_blip2_destroy(mi3d_blip2_t h);
+mi3d_engine_t mi3d_blip2_create(const mi3d_blip2_cfg* cfg, void* workspace, size_t workspace_bytes);
 /* Parameters are enumerated by transformers' Blip2ForConditionalGeneration.state_dict() names, in its order ("query_tokens" ..
  * "language_model.model.decoder.layers.{L-1}.final_layer_norm.bias"), without the tied "language_model.lm_head.weight" (lm_head reads
- * embed_tokens).  OPT's q / k / v projections are stored as row slices of one packed weight.  load: src = fp32 DEVICE tensor in
- * torch's layout; it may be freed once the stream has passed the call. */
-int mi3d_blip2_num_params(mi3d_blip2_t h);
-const char* mi3d_blip2_param_name(mi3d_blip2_t h, int i);
-int mi3d_blip2_param_shape(mi3d_blip2_t h, int i, int* shape4); /* returns rank */
-int mi3d_blip2_load_param(mi3d_blip2_t h, int i, const float* src, mi3d_stream_t stream);
-/* CUDA-graph replay of the static launch lists, from a list's third call on (`stream` must then be capturable); off by default.
- * mi3d_blip2_graph_replays: lists currently instantiated. */
-int mi3d_blip2_set_graph_replay(mi3d_blip2_t h, int enable);
-int mi3d_blip2_graph_replays(mi3d_blip2_t h);
+ * embed_tokens).  OPT's q / k / v projections are stored as row slices of one packed weight. */
 /* pixel_values fp32 [1,3,image_size,image_size] (DEVICE, processor-normalised) -> out fp32 [num_query_tokens, opt_width]
  * (language_model_inputs = language_projection(Q-Former(vision(pixel_values)))) */
-int mi3d_blip2_encode(mi3d_blip2_t h, const float* pixel_values, float* out, mi3d_stream_t stream);
+int mi3d_blip2_encode(mi3d_engine_t h, const float* pixel_values, float* out, mi3d_stream_t stream);
 /* Greedy caption: the prompt [image_token_index] x num_query_tokens + [bos_token_id], the query rows replaced by language_model_inputs,
  * then max_new_tokens greedy steps (1 .. 63 - num_query_tokens), each a causal pass over a fixed 64-row window, lm_head on the last
  * filled row only, argmax with the lowest index on ties.  After eos (< 0: none) no token is appended.  ids (DEVICE int64 [64]): the
  * prompt and the generated tokens; count (DEVICE int32 [1]): how many of them are valid (num_query_tokens + 1 + n).
  * forced_ids (DEVICE int64 [max_new_tokens], nullable): teacher forcing, step s appends forced_ids[s] instead of the argmax.
  * step_logits (DEVICE fp32 [max_new_tokens, vocab], nullable): the last-row logits of every step. */
-int mi3d_blip2_generate(mi3d_blip2_t h, const float* pixel_values, int max_new_tokens, long long eos_token_id, const long long* forced_ids,
+int mi3d_blip2_generate(mi3d_engine_t h, const float* pixel_values, int max_new_tokens, long long eos_token_id, const long long* forced_ids,
                         long long* ids, int* count, float* step_logits, mi3d_stream_t stream);
 /* the last call's intermediates as fp32 (DEVICE): "image_embeds" [T, vision_width] (T = (image_size / patch)^2 + 1, post_layernorm
  * applied), "query_output" [num_query_tokens, qformer_width], "language_model_inputs" [num_query_tokens, opt_width] */
-int mi3d_blip2_tap(mi3d_blip2_t h, const char* name, float* dst, mi3d_stream_t stream);
+int mi3d_blip2_tap(mi3d_engine_t h, const char* name, float* dst, mi3d_stream_t stream);
 /* The weight-streaming GEMM on its own: y[M,N] = act(x[M,K] w[N,K]^T + bias (+ residual)), M <= 64, K % 32 == 0; x, w, residual, y
  * fp16, bias fp32 (nullable), relu != 0: ReLU.  workspace: mi3d_stream_gemm_workspace_bytes(M, N, K) bytes (fp32 partial sums). */
 size_t mi3d_stream_gemm_workspace_bytes(int M, int N, int K);

@@ -2,6 +2,7 @@
 
 The product path has NO fallback: if the shared library is missing, or a call returns non-zero, we raise.
 """
+import contextlib
 import ctypes as C
 import os
 import subprocess
@@ -102,24 +103,18 @@ SYMBOLS = [
     "mi3d_density_grid_workspace_bytes", "mi3d_density_grid_update", "mi3d_version",
     "mi3d_sumsq_workspace_bytes", "mi3d_sumsq", "mi3d_adan_step",
     "mi3d_gemm_f16", "mi3d_gemm_f16_splitk", "mi3d_flash_attn_f16", "mi3d_conv3x3_f16", "mi3d_tf32_tile_test", "mi3d_gemm_f16_bt",
-    "mi3d_sd_workspace_bytes", "mi3d_sd_create", "mi3d_sd_destroy", "mi3d_sd_num_params", "mi3d_sd_param_name", "mi3d_sd_param_numel",
-    "mi3d_sd_param_shape", "mi3d_sd_load_param", "mi3d_sd_encode", "mi3d_sd_encode_backward", "mi3d_sd_unet_sds", "mi3d_sd_debug_tensor", "mi3d_sd_profile",
-    "mi3d_sd_profile_dump", "mi3d_sd_set_graph_replay", "mi3d_sd_graph_replays", "mi3d_sd_ddim_step", "mi3d_sd_decode",
-    "mi3d_sd_text_workspace_bytes", "mi3d_sd_text_create", "mi3d_sd_text_destroy", "mi3d_sd_text_num_params", "mi3d_sd_text_param_name",
-    "mi3d_sd_text_param_shape", "mi3d_sd_text_load_param", "mi3d_sd_text_set_graph_replay", "mi3d_sd_text_graph_replays", "mi3d_sd_text_encode",
-    "mi3d_clip_workspace_bytes", "mi3d_clip_create", "mi3d_clip_destroy", "mi3d_clip_num_params", "mi3d_clip_param_name",
-    "mi3d_clip_param_shape", "mi3d_clip_load_param", "mi3d_clip_set_graph_replay", "mi3d_clip_graph_replays", "mi3d_clip_encode_image",
-    "mi3d_clip_encode_image_backward", "mi3d_clip_encode_text",
+    "mi3d_engine_destroy", "mi3d_engine_num_params", "mi3d_engine_param_name", "mi3d_engine_param_shape", "mi3d_engine_load_param",
+    "mi3d_engine_set_graph_replay", "mi3d_engine_graph_replays", "mi3d_engine_debug_tensor",
+    "mi3d_sd_workspace_bytes", "mi3d_sd_create", "mi3d_sd_encode", "mi3d_sd_encode_backward", "mi3d_sd_unet_sds", "mi3d_sd_profile",
+    "mi3d_sd_profile_dump", "mi3d_sd_ddim_step", "mi3d_sd_decode",
+    "mi3d_sd_text_workspace_bytes", "mi3d_sd_text_create", "mi3d_sd_text_encode",
+    "mi3d_clip_workspace_bytes", "mi3d_clip_create", "mi3d_clip_encode_image", "mi3d_clip_encode_image_backward", "mi3d_clip_encode_text",
     "mi3d_points_workspace_bytes", "mi3d_points_render_forward", "mi3d_points_render_backward", "mi3d_points_zbuffer_visible",
-    "mi3d_cx_workspace_bytes", "mi3d_cx_create", "mi3d_cx_destroy", "mi3d_cx_num_params", "mi3d_cx_param_name", "mi3d_cx_param_shape",
-    "mi3d_cx_load_param", "mi3d_cx_set_graph_replay", "mi3d_cx_graph_replays", "mi3d_cx_forward", "mi3d_cx_backward", "mi3d_cx_debug_tensor",
-    "mi3d_unet_workspace_bytes", "mi3d_unet_create", "mi3d_unet_destroy", "mi3d_unet_num_params", "mi3d_unet_param_name", "mi3d_unet_param_shape",
-    "mi3d_unet_set_graph_replay", "mi3d_unet_graph_replays", "mi3d_unet_forward", "mi3d_unet_backward", "mi3d_unet_debug_tensor",
-    "mi3d_dpt_workspace_bytes", "mi3d_dpt_create", "mi3d_dpt_destroy", "mi3d_dpt_num_params", "mi3d_dpt_param_name", "mi3d_dpt_param_shape",
-    "mi3d_dpt_load_param", "mi3d_dpt_forward", "mi3d_dpt_tap",
-    "mi3d_blip2_workspace_bytes", "mi3d_blip2_create", "mi3d_blip2_destroy", "mi3d_blip2_num_params", "mi3d_blip2_param_name",
-    "mi3d_blip2_param_shape", "mi3d_blip2_load_param", "mi3d_blip2_set_graph_replay", "mi3d_blip2_graph_replays", "mi3d_blip2_encode",
-    "mi3d_blip2_generate", "mi3d_blip2_tap", "mi3d_stream_gemm_workspace_bytes", "mi3d_stream_gemm_f16",
+    "mi3d_cx_workspace_bytes", "mi3d_cx_create", "mi3d_cx_forward", "mi3d_cx_backward",
+    "mi3d_unet_workspace_bytes", "mi3d_unet_create", "mi3d_unet_forward", "mi3d_unet_backward",
+    "mi3d_dpt_workspace_bytes", "mi3d_dpt_create", "mi3d_dpt_forward", "mi3d_dpt_tap",
+    "mi3d_blip2_workspace_bytes", "mi3d_blip2_create", "mi3d_blip2_encode", "mi3d_blip2_generate", "mi3d_blip2_tap",
+    "mi3d_stream_gemm_workspace_bytes", "mi3d_stream_gemm_f16",
     "mi3d_mc_workspace_bytes", "mi3d_mc_count", "mi3d_mc_emit", "mi3d_mesh_atlas_texels",
     "mi3d_views_workspace_bytes", "mi3d_views_mask", "mi3d_views_cover_mask", "mi3d_views_backproject", "mi3d_views_compact_colour",
 ]
@@ -141,21 +136,14 @@ def lib():
             raise Mi3dError(f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
                             "(there is no CPU / PyTorch fallback for the hot path)")
         _lib = C.CDLL(LIB_PATH)
-        _lib.mi3d_version.restype = C.c_char_p
-        _lib.mi3d_march_rays_train_workspace_bytes.restype = C.c_size_t
-        _lib.mi3d_density_grid_workspace_bytes.restype = C.c_size_t
-        _lib.mi3d_field_backward_workspace_bytes.restype = C.c_size_t
-        _lib.mi3d_field_enc_cache_bytes.restype = C.c_size_t
-        _lib.mi3d_render_workspace_bytes.restype = C.c_size_t
-        _lib.mi3d_sumsq_workspace_bytes.restype = C.c_size_t
-        _lib.mi3d_render_eval_workspace_bytes.restype = C.c_size_t
-        _lib.mi3d_mc_workspace_bytes.restype = C.c_size_t
-        _lib.mi3d_views_workspace_bytes.restype = C.c_size_t
-        for name in ("mi3d_sd_workspace_bytes", "mi3d_sd_weight_bytes"):
-            if hasattr(_lib, name):
+        for name in SYMBOLS:
+            if name.endswith("_workspace_bytes"):
                 getattr(_lib, name).restype = C.c_size_t
-        if hasattr(_lib, "mi3d_sd_create"):
-            _lib.mi3d_sd_create.restype = C.c_void_p
+            elif name.endswith("_create"):
+                getattr(_lib, name).restype = C.c_void_p           # mi3d_engine_t
+        _lib.mi3d_field_enc_cache_bytes.restype = C.c_size_t
+        _lib.mi3d_engine_param_name.restype = C.c_char_p
+        _lib.mi3d_version.restype = C.c_char_p
     return _lib
 
 
@@ -189,3 +177,98 @@ def require_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:
             raise Mi3dError("mi3d operators run on sm_90a only; got a CPU tensor and there is no CPU fallback")
+
+
+class Engine:
+    """A planned engine of libmi3d.so (mi3d_<kind>_create): the device workspace it is carved from (zeroed: padding rows and channels
+    are never written), its handle, its parameter registry (`names`, `shapes`) and, with graph_replay, the stream its launch lists
+    run on so that they can replay as CUDA graphs (torch's legacy default stream cannot be captured; graph_replay=False keeps plain
+    launches on the caller's stream).  Subclasses add their configuration struct, their compute calls and their state_dict policy."""
+
+    debug_dtype = torch.float16          # element type of the workspace's intermediates (debug_tensor's default view)
+
+    def __init__(self, kind, cfg_args, device, graph_replay, what):
+        """cfg_args: the arguments mi3d_<kind>_workspace_bytes takes (and mi3d_<kind>_create before the workspace); what: the
+        configuration, for the error message when the engine cannot run it"""
+        lib_ = lib()
+        nbytes = getattr(lib_, f"mi3d_{kind}_workspace_bytes")(*cfg_args)
+        if nbytes == 0:
+            raise Mi3dError(f"unsupported {what}")
+        self.nbytes = nbytes
+        self.workspace = torch.zeros(nbytes, dtype=torch.uint8, device=device)
+        h = getattr(lib_, f"mi3d_{kind}_create")(*cfg_args, ptr(self.workspace), C.c_size_t(nbytes))
+        if not h:
+            raise Mi3dError(f"mi3d_{kind}_create failed (TMA descriptor encoding error)")
+        self.h = C.c_void_p(h)
+        self.names, self.shapes = [], []
+        shp = (C.c_int * 4)()
+        for i in range(lib_.mi3d_engine_num_params(self.h)):
+            self.names.append(lib_.mi3d_engine_param_name(self.h, C.c_int(i)).decode())
+            r = lib_.mi3d_engine_param_shape(self.h, C.c_int(i), shp)
+            self.shapes.append(tuple(shp[k] for k in range(r)))
+        self.stream = torch.cuda.Stream(device) if graph_replay else None
+        check(lib_.mi3d_engine_set_graph_replay(self.h, C.c_int(1 if graph_replay else 0)), f"{kind}: set_graph_replay")
+
+    def graph_replays(self):
+        """number of launch lists currently instantiated as CUDA graphs"""
+        return int(lib().mi3d_engine_graph_replays(self.h))
+
+    @contextlib.contextmanager
+    def on_stream(self):
+        """Engine calls inside run on self.stream, ordered after the caller's pending work; the caller's stream then waits for them."""
+        if self.stream is None:
+            yield
+            return
+        cur = torch.cuda.current_stream()
+        self.stream.wait_stream(cur)
+        with torch.cuda.stream(self.stream):
+            yield
+        cur.wait_stream(self.stream)
+
+    def partner(self, name, tensors):
+        """the second tensor of a pair the engine writes together with entry `name` (None: none)"""
+        return None
+
+    def load(self, tensors):
+        """tensors: name -> tensor (any float dtype, any device) for every registry entry; an entry 'base#suffix' is a derived copy
+        and is written from tensors[base]"""
+        lib_ = lib()
+        dev = self.workspace.device
+        for i, name in enumerate(self.names):
+            base = name.split("#")[0]
+            if base not in tensors:
+                raise Mi3dError(f"missing parameter {base}")
+            src = tensors[base].detach().to(dev, torch.float32).contiguous()
+            partner = self.partner(name, tensors)
+            if partner is not None:
+                partner = partner.detach().to(dev, torch.float32).contiguous()
+            # the caching allocator reuses src's memory only after the load kernel queued behind it on this stream
+            check(lib_.mi3d_engine_load_param(self.h, C.c_int(i), ptr(src), ptr(partner), stream()), f"load_param({name})")
+        torch.cuda.synchronize(dev)
+
+    def load_strict(self, state_dict, ignored=lambda key: False):
+        """load() after checking that state_dict holds every registry entry with its shape and no other key but those `ignored` accepts"""
+        known = set(self.names)
+        missing = [n for n in self.names if n not in state_dict]
+        unexpected = [k for k in state_dict if k not in known and not ignored(k)]
+        if missing or unexpected:
+            raise Mi3dError(f"{type(self).__name__} state_dict mismatch: missing {missing[:4]}, unexpected {unexpected[:4]}")
+        for name, shape in zip(self.names, self.shapes):
+            if tuple(state_dict[name].shape) != shape:
+                raise Mi3dError(f"{name}: shape {tuple(state_dict[name].shape)}, expected {shape}")
+        self.load(state_dict)
+        return self
+
+    def debug_tensor(self, name, dtype=None):
+        """a named intermediate, as a view of the workspace"""
+        p, n = C.c_void_p(), C.c_size_t()
+        check(lib().mi3d_engine_debug_tensor(self.h, name.encode(), C.byref(p), C.byref(n)), f"debug_tensor({name})")
+        off = p.value - self.workspace.data_ptr()
+        return self.workspace[off:off + n.value].view(dtype or self.debug_dtype)
+
+    def __del__(self):
+        try:
+            if getattr(self, "h", None):
+                lib().mi3d_engine_destroy(self.h)
+        except Exception:
+            pass

@@ -50,6 +50,7 @@ struct OptW { const __half *w_qkv, *w_out, *w_fc1, *w_fc2; const float *b_qkv, *
 
 struct Engine : Builder {
     mi3d_blip2_cfg cfg;
+    explicit Engine(const mi3d_blip2_cfg& c) : cfg(c) {}
     int Tv = 0, Tvp = 0, np = 0, Kpatch = 0, Vpad = 0, max_new = 0;
     std::map<int, int> padk;                 // param index -> padded K (the patch conv's weight)
     // device buffers
@@ -333,6 +334,14 @@ struct Engine : Builder {
         if (err) { dec.erase(n); return nullptr; }
         return &L;
     }
+
+    int load_param(const Param& P, const float* src, const float* partner, cudaStream_t st) override {
+        auto pk = padk.find((int)(&P - params.data()));
+        if (pk == padk.end()) return Builder::load_param(P, src, partner, st);
+        const int N = P.shape[0], K = (int)(P.numel / N);
+        b2k::k_f32_to_f16_padk<<<blocks_for((size_t)N * pk->second), 256, 0, st>>>(src, (__half*)P.dst, N, K, pk->second);
+        return (int)cudaGetLastError();
+    }
 };
 
 bool valid_cfg(const mi3d_blip2_cfg& c) {
@@ -348,69 +357,20 @@ bool valid_cfg(const mi3d_blip2_cfg& c) {
 
 }  // namespace blip2
 
-struct mi3d_blip2 { blip2::Engine e; };
-
 extern "C" {
 
 size_t mi3d_blip2_workspace_bytes(const mi3d_blip2_cfg* cfg) {
-    if (!cfg || !blip2::valid_cfg(*cfg)) return 0;
-    blip2::Engine e; e.cfg = *cfg;
-    if (e.build(true)) return 0;
-    return e.off + (1 << 20);
+    return cfg && blip2::valid_cfg(*cfg) ? plan::workspace_bytes<blip2::Engine>(*cfg) : 0;
 }
 
-mi3d_blip2_t mi3d_blip2_create(const mi3d_blip2_cfg* cfg, void* workspace, size_t workspace_bytes) {
-    if (!cfg || !workspace || !blip2::valid_cfg(*cfg)) return nullptr;
-    mi3d_blip2* h = new mi3d_blip2();
-    h->e.cfg = *cfg; h->e.base = (uint8_t*)workspace; h->e.cap = workspace_bytes;
-    int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&h->e.num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (h->e.build(false) != 0) { delete h; return nullptr; }
-    return h;
+mi3d_engine_t mi3d_blip2_create(const mi3d_blip2_cfg* cfg, void* workspace, size_t workspace_bytes) {
+    return cfg && blip2::valid_cfg(*cfg) ? plan::create<blip2::Engine>(workspace, workspace_bytes, *cfg) : nullptr;
 }
 
-void mi3d_blip2_destroy(mi3d_blip2_t h) { delete h; }
-
-int mi3d_blip2_num_params(mi3d_blip2_t h) { return h ? (int)h->e.params.size() : 0; }
-const char* mi3d_blip2_param_name(mi3d_blip2_t h, int i) {
-    if (!h || i < 0 || i >= (int)h->e.params.size()) return nullptr;
-    return h->e.params[i].name.c_str();
-}
-int mi3d_blip2_param_shape(mi3d_blip2_t h, int i, int* shape4) {
-    if (!h || !shape4 || i < 0 || i >= (int)h->e.params.size()) return -1;
-    const auto& s = h->e.params[i].shape;
-    for (int k = 0; k < 4; k++) shape4[k] = k < (int)s.size() ? s[k] : 0;
-    return (int)s.size();
-}
-
-int mi3d_blip2_load_param(mi3d_blip2_t h, int i, const float* src, mi3d_stream_t stream) {
-    if (!h || i < 0 || i >= (int)h->e.params.size() || !src) return MI3D_ERR_ARG;
-    cudaStream_t st = (cudaStream_t)stream;
-    const plan::Param& P = h->e.params[i];
-    auto pk = h->e.padk.find(i);
-    if (pk != h->e.padk.end()) {
-        const int N = P.shape[0], K = (int)(P.numel / N);
-        b2k::k_f32_to_f16_padk<<<plan::Builder::blocks_for((size_t)N * pk->second), 256, 0, st>>>(src, (__half*)P.dst, N, K, pk->second);
-        return (int)cudaGetLastError();
-    }
-    switch (P.kind) {
-        case plan::PK_F32: MI3D_CHECK(cudaMemcpyAsync(P.dst, src, P.numel * 4, cudaMemcpyDeviceToDevice, st)); break;
-        case plan::PK_LINEAR: sdk::k_f32_to_f16<<<plan::Builder::blocks_for(P.numel), 256, 0, st>>>(src, (__half*)P.dst, P.numel); break;
-        default: return MI3D_ERR_ARG;
-    }
-    return (int)cudaGetLastError();
-}
-
-int mi3d_blip2_set_graph_replay(mi3d_blip2_t h, int enable) {
-    if (!h) return MI3D_ERR_ARG;
-    h->e.use_graph = enable != 0;
-    return MI3D_OK;
-}
-
-int mi3d_blip2_graph_replays(mi3d_blip2_t h) { return h ? h->e.graph_replays() : -1; }
-
-int mi3d_blip2_encode(mi3d_blip2_t h, const float* pixel_values, float* out, mi3d_stream_t stream) {
-    if (!h || !pixel_values) return MI3D_ERR_ARG;
-    blip2::Engine& e = h->e; const mi3d_blip2_cfg& c = e.cfg;
+int mi3d_blip2_encode(mi3d_engine_t h, const float* pixel_values, float* out, mi3d_stream_t stream) {
+    blip2::Engine* ep = plan::engine_of<blip2::Engine>(h);
+    if (!ep || !pixel_values) return MI3D_ERR_ARG;
+    blip2::Engine& e = *ep; const mi3d_blip2_cfg& c = e.cfg;
     cudaStream_t st = (cudaStream_t)stream;
     MI3D_CHECK(cudaMemcpyAsync(e.pixels, pixel_values, (size_t)3 * c.image_size * c.image_size * 4, cudaMemcpyDeviceToDevice, st));
     int r = e.run(e.enc, st); if (r) return r;
@@ -422,10 +382,11 @@ int mi3d_blip2_encode(mi3d_blip2_t h, const float* pixel_values, float* out, mi3
     return MI3D_OK;
 }
 
-int mi3d_blip2_generate(mi3d_blip2_t h, const float* pixel_values, int max_new_tokens, long long eos_token_id, const long long* forced_ids,
+int mi3d_blip2_generate(mi3d_engine_t h, const float* pixel_values, int max_new_tokens, long long eos_token_id, const long long* forced_ids,
                         long long* ids, int* count, float* step_logits, mi3d_stream_t stream) {
-    if (!h || !pixel_values || !ids || !count) return MI3D_ERR_ARG;
-    blip2::Engine& e = h->e; const mi3d_blip2_cfg& c = e.cfg;
+    blip2::Engine* ep = plan::engine_of<blip2::Engine>(h);
+    if (!ep || !pixel_values || !ids || !count) return MI3D_ERR_ARG;
+    blip2::Engine& e = *ep; const mi3d_blip2_cfg& c = e.cfg;
     if (max_new_tokens < 1 || max_new_tokens > e.max_new) return MI3D_ERR_ARG;
     cudaStream_t st = (cudaStream_t)stream;
     std::vector<plan::Op>* L = e.decode_list(max_new_tokens);
@@ -444,10 +405,11 @@ int mi3d_blip2_generate(mi3d_blip2_t h, const float* pixel_values, int max_new_t
     return MI3D_OK;
 }
 
-int mi3d_blip2_tap(mi3d_blip2_t h, const char* name, float* dst, mi3d_stream_t stream) {
-    if (!h || !name || !dst) return MI3D_ERR_ARG;
-    auto it = h->e.named.find(name);
-    if (it == h->e.named.end()) return MI3D_ERR_ARG;
+int mi3d_blip2_tap(mi3d_engine_t h, const char* name, float* dst, mi3d_stream_t stream) {
+    blip2::Engine* ep = plan::engine_of<blip2::Engine>(h);
+    if (!ep || !name || !dst) return MI3D_ERR_ARG;
+    auto it = ep->named.find(name);
+    if (it == ep->named.end()) return MI3D_ERR_ARG;
     const size_t n = it->second.second / 2;
     b2k::k_f16_to_f32<<<plan::Builder::blocks_for(n), 256, 0, (cudaStream_t)stream>>>((const __half*)it->second.first, dst, n);
     return (int)cudaGetLastError();

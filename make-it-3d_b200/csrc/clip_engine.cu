@@ -20,6 +20,7 @@ struct BwdA { __half *dpre, *dln2, *dh, *dao, *daoT, *dS, *PT, *dST, *dqkv, *dln
 
 struct Engine : TowerBuilder {
     mi3d_clip_cfg cfg;
+    explicit Engine(const mi3d_clip_cfg& c) : cfg(c) {}
     Tower vt, tt;
     int np = 0, G = 0, KP = 0;
     std::vector<BlockW> vw, tw;
@@ -245,70 +246,20 @@ bool valid_cfg(const mi3d_clip_cfg& c) {
 
 }  // namespace clip
 
-struct mi3d_clip { clip::Engine e; };
-
 extern "C" {
 
 size_t mi3d_clip_workspace_bytes(const mi3d_clip_cfg* cfg) {
-    if (!cfg || !clip::valid_cfg(*cfg)) return 0;
-    clip::Engine e; e.cfg = *cfg;
-    e.build(true);
-    return e.off + (1 << 20);
+    return cfg && clip::valid_cfg(*cfg) ? plan::workspace_bytes<clip::Engine>(*cfg) : 0;
 }
 
-mi3d_clip_t mi3d_clip_create(const mi3d_clip_cfg* cfg, void* workspace, size_t workspace_bytes) {
-    if (!cfg || !workspace || !clip::valid_cfg(*cfg)) return nullptr;
-    mi3d_clip* h = new mi3d_clip();
-    h->e.cfg = *cfg; h->e.base = (uint8_t*)workspace; h->e.cap = workspace_bytes;
-    int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&h->e.num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (h->e.build(false) != 0) { delete h; return nullptr; }
-    return h;
+mi3d_engine_t mi3d_clip_create(const mi3d_clip_cfg* cfg, void* workspace, size_t workspace_bytes) {
+    return cfg && clip::valid_cfg(*cfg) ? plan::create<clip::Engine>(workspace, workspace_bytes, *cfg) : nullptr;
 }
 
-void mi3d_clip_destroy(mi3d_clip_t h) { delete h; }
-
-int mi3d_clip_num_params(mi3d_clip_t h) { return h ? (int)h->e.params.size() : 0; }
-const char* mi3d_clip_param_name(mi3d_clip_t h, int i) {
-    if (!h || i < 0 || i >= (int)h->e.params.size()) return nullptr;
-    return h->e.params[i].name.c_str();
-}
-int mi3d_clip_param_shape(mi3d_clip_t h, int i, int* shape4) {
-    if (!h || !shape4 || i < 0 || i >= (int)h->e.params.size()) return -1;
-    const auto& s = h->e.params[i].shape;
-    for (int k = 0; k < 4; k++) shape4[k] = k < (int)s.size() ? s[k] : 0;
-    return (int)s.size();
-}
-
-// src: fp32 device tensor in openai CLIP's layout, named by mi3d_clip_param_name (a '#' suffix marks a derived copy: pass the base tensor)
-int mi3d_clip_load_param(mi3d_clip_t h, int i, const float* src, mi3d_stream_t stream) {
-    if (!h || i < 0 || i >= (int)h->e.params.size() || !src) return MI3D_ERR_ARG;
-    cudaStream_t st = (cudaStream_t)stream;
-    const plan::Param& P = h->e.params[i];
-    const int nb = plan::Builder::blocks_for(P.numel);
-    const int O = P.shape.empty() ? 1 : P.shape[0], I = (int)(P.numel / (size_t)O);     // conv1 [C,3,P,P] is the matrix [C][3*P*P]
-    switch (P.kind) {
-        case plan::PK_F32: MI3D_CHECK(cudaMemcpyAsync(P.dst, src, P.numel * 4, cudaMemcpyDeviceToDevice, st)); break;
-        case plan::PK_LINEAR: sdk::k_f32_to_f16<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.numel); break;
-        case plan::PK_LINEAR_T: sdk::k_transpose_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst, O, I); break;
-        case plan::PK_LINEAR_BOTH:
-            sdk::k_f32_to_f16<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.numel);
-            sdk::k_transpose_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst2, O, I); break;
-        default: return MI3D_ERR_ARG;
-    }
-    return (int)cudaGetLastError();
-}
-
-int mi3d_clip_set_graph_replay(mi3d_clip_t h, int enable) {
-    if (!h) return MI3D_ERR_ARG;
-    h->e.use_graph = enable != 0;
-    return MI3D_OK;
-}
-
-int mi3d_clip_graph_replays(mi3d_clip_t h) { return h ? h->e.graph_replays() : -1; }
-
-int mi3d_clip_encode_image(mi3d_clip_t h, const float* img, int B, int H, int W, int aug, int need_grad, float* feats, mi3d_stream_t stream) {
-    if (!h || h->e.cfg.layers == 0 || !img || !feats) return MI3D_ERR_ARG;
-    clip::Engine& e = h->e; const mi3d_clip_cfg& c = e.cfg;
+int mi3d_clip_encode_image(mi3d_engine_t h, const float* img, int B, int H, int W, int aug, int need_grad, float* feats, mi3d_stream_t stream) {
+    clip::Engine* ep = plan::engine_of<clip::Engine>(h);
+    if (!ep || ep->cfg.layers == 0 || !img || !feats) return MI3D_ERR_ARG;
+    clip::Engine& e = *ep; const mi3d_clip_cfg& c = e.cfg;
     if (B < 1 || B > c.max_batch || H < 1 || W < 1 || (!aug && (H != c.image_res || W != c.image_res))) return MI3D_ERR_ARG;
     cudaStream_t st = (cudaStream_t)stream;
     e.tape_valid = false;
@@ -321,9 +272,10 @@ int mi3d_clip_encode_image(mi3d_clip_t h, const float* img, int B, int H, int W,
     return MI3D_OK;
 }
 
-int mi3d_clip_encode_image_backward(mi3d_clip_t h, const float* dfeats, int n_grad, float* dimg, mi3d_stream_t stream) {
-    if (!h || !dfeats || !dimg) return MI3D_ERR_ARG;
-    clip::Engine& e = h->e; const mi3d_clip_cfg& c = e.cfg;
+int mi3d_clip_encode_image_backward(mi3d_engine_t h, const float* dfeats, int n_grad, float* dimg, mi3d_stream_t stream) {
+    clip::Engine* ep = plan::engine_of<clip::Engine>(h);
+    if (!ep || !dfeats || !dimg) return MI3D_ERR_ARG;
+    clip::Engine& e = *ep; const mi3d_clip_cfg& c = e.cfg;
     if (!e.tape_valid || n_grad < 1 || n_grad > e.tape_B) return MI3D_ERR_ARG;
     cudaStream_t st = (cudaStream_t)stream;
     clipk::k_grad_in<<<1, 256, 0, st>>>(dfeats, n_grad * c.embed_dim, e.dfeat16, e.gscale);
@@ -334,9 +286,10 @@ int mi3d_clip_encode_image_backward(mi3d_clip_t h, const float* dfeats, int n_gr
     return (int)cudaGetLastError();
 }
 
-int mi3d_clip_encode_text(mi3d_clip_t h, const long long* tokens, int B, float* feats, mi3d_stream_t stream) {
-    if (!h || h->e.cfg.text_layers == 0 || !tokens || !feats) return MI3D_ERR_ARG;
-    clip::Engine& e = h->e; const mi3d_clip_cfg& c = e.cfg;
+int mi3d_clip_encode_text(mi3d_engine_t h, const long long* tokens, int B, float* feats, mi3d_stream_t stream) {
+    clip::Engine* ep = plan::engine_of<clip::Engine>(h);
+    if (!ep || ep->cfg.text_layers == 0 || !tokens || !feats) return MI3D_ERR_ARG;
+    clip::Engine& e = *ep; const mi3d_clip_cfg& c = e.cfg;
     if (B < 1 || B > c.max_batch) return MI3D_ERR_ARG;
     cudaStream_t st = (cudaStream_t)stream;
     MI3D_CHECK(cudaMemcpyAsync(e.tokens, tokens, (size_t)B * c.context_len * sizeof(long long), cudaMemcpyDeviceToDevice, st));

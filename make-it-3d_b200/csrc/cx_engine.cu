@@ -23,6 +23,7 @@ struct Layer {
 
 struct Engine : Builder {
     mi3d_cx_cfg cfg;
+    explicit Engine(const mi3d_cx_cfg& c) : cfg(c) {}
     std::vector<Layer> layers;
     T4 img4, feat;
     int P = 0, C5 = 0;
@@ -63,8 +64,8 @@ struct Engine : Builder {
                 L.w = conv_name(idx); L.in = x; L.out = act(B, x.h, x.w, cout);
                 const float* bias = pf(L.w + ".bias", {cout});
                 if (idx == 0) {
-                    const float* w = (const float*)param(L.w + ".weight", {cout, cin, 3, 3}, PK_CONV_F32_OHWI).dst;
-                    param(L.w + ".weight#dgrad", {4, cout, 3, 3}, PK_CONV_SMALL_COUT);
+                    const float* w = (const float*)param(L.w + ".weight", {cout, cin, 3, 3}, PK_CX_CONV_IN).dst;
+                    param(L.w + ".weight#dgrad", {4, cout, 3, 3}, PK_CX_CONV_IN_DGRAD);
                     const T4 a = L.in, o = L.out;
                     const size_t sm = (size_t)cout * 9 * 4 * sizeof(float);
                     const int grid = small_cin_grid(o.numel(), sm);
@@ -158,81 +159,39 @@ struct Engine : Builder {
         cur = nullptr;
         return err;
     }
+
+    int load_param(const Param& P, const float* src, const float* partner, cudaStream_t st) override {
+        switch (P.kind) {
+            case PK_CX_CONV_IN: {
+                // conv1_1: the fp32 forward weights and, in the same pass, the flipped fp16 copy of its '#dgrad' entry
+                const Param& D = params[pindex[P.name + "#dgrad"]];
+                cxk::k_conv1_w<<<1, 256, 0, st>>>(src, (float*)P.dst, (__half*)D.dst, P.shape[0]);
+                return (int)cudaGetLastError();
+            }
+            case PK_CX_CONV_IN_DGRAD: return MI3D_OK;      // written with its base tensor
+            default: return Builder::load_param(P, src, partner, st);
+        }
+    }
 };
 
 bool valid_cfg(const mi3d_cx_cfg& c) { return c.N >= 1 && c.N <= 16 && c.H >= 16 && c.W >= 16 && c.H <= 4096 && c.W <= 4096; }
 
 }  // namespace cx
 
-struct mi3d_cx { cx::Engine e; };
-
 extern "C" {
 
 size_t mi3d_cx_workspace_bytes(const mi3d_cx_cfg* cfg) {
-    if (!cfg || !cx::valid_cfg(*cfg)) return 0;
-    cx::Engine e; e.cfg = *cfg;
-    e.build(true);
-    return e.off + (1 << 20);
+    return cfg && cx::valid_cfg(*cfg) ? plan::workspace_bytes<cx::Engine>(*cfg) : 0;
 }
 
-mi3d_cx_t mi3d_cx_create(const mi3d_cx_cfg* cfg, void* workspace, size_t workspace_bytes) {
-    if (!cfg || !workspace || !cx::valid_cfg(*cfg)) return nullptr;
-    mi3d_cx* h = new mi3d_cx();
-    h->e.cfg = *cfg; h->e.base = (uint8_t*)workspace; h->e.cap = workspace_bytes;
-    int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&h->e.num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (h->e.build(false) != 0) { delete h; return nullptr; }
-    return h;
+mi3d_engine_t mi3d_cx_create(const mi3d_cx_cfg* cfg, void* workspace, size_t workspace_bytes) {
+    return cfg && cx::valid_cfg(*cfg) ? plan::create<cx::Engine>(workspace, workspace_bytes, *cfg) : nullptr;
 }
 
-void mi3d_cx_destroy(mi3d_cx_t h) { delete h; }
-
-int mi3d_cx_num_params(mi3d_cx_t h) { return h ? (int)h->e.params.size() : 0; }
-const char* mi3d_cx_param_name(mi3d_cx_t h, int i) {
-    if (!h || i < 0 || i >= (int)h->e.params.size()) return nullptr;
-    return h->e.params[i].name.c_str();
-}
-int mi3d_cx_param_shape(mi3d_cx_t h, int i, int* shape4) {
-    if (!h || !shape4 || i < 0 || i >= (int)h->e.params.size()) return -1;
-    const auto& s = h->e.params[i].shape;
-    for (int k = 0; k < 4; k++) shape4[k] = k < (int)s.size() ? s[k] : 0;
-    return (int)s.size();
-}
-
-// src: fp32 device tensor in torch's layout (OIHW weights, [O] biases), named by mi3d_cx_param_name; for a '#dgrad' copy pass the base tensor
-int mi3d_cx_load_param(mi3d_cx_t h, int i, const float* src, mi3d_stream_t stream) {
-    if (!h || i < 0 || i >= (int)h->e.params.size() || !src) return MI3D_ERR_ARG;
-    cudaStream_t st = (cudaStream_t)stream;
-    const plan::Param& P = h->e.params[i];
-    const int nb = plan::Builder::blocks_for(P.numel);
-    switch (P.kind) {
-        case plan::PK_F32: MI3D_CHECK(cudaMemcpyAsync(P.dst, src, P.numel * 4, cudaMemcpyDeviceToDevice, st)); break;
-        case plan::PK_CONV3_BOTH:
-            sdk::k_conv_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.shape[0], P.shape[1], 0);
-            sdk::k_conv_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst2, P.shape[0], P.shape[1], 1);
-            break;
-        case plan::PK_CONV_F32_OHWI: {
-            // conv1_1: the fp32 forward weights and, in the same pass, the flipped fp16 copy of its '#dgrad' entry
-            const plan::Param& D = h->e.params[h->e.pindex[P.name + "#dgrad"]];
-            cxk::k_conv1_w<<<1, 256, 0, st>>>(src, (float*)P.dst, (__half*)D.dst, P.shape[0]);
-            break;
-        }
-        case plan::PK_CONV_SMALL_COUT: break;      // written with its base tensor
-        default: return MI3D_ERR_ARG;
-    }
-    return (int)cudaGetLastError();
-}
-
-int mi3d_cx_set_graph_replay(mi3d_cx_t h, int enable) {
-    if (!h) return MI3D_ERR_ARG;
-    h->e.use_graph = enable != 0;
-    return MI3D_OK;
-}
-
-int mi3d_cx_graph_replays(mi3d_cx_t h) { return h ? h->e.graph_replays() : -1; }
-
-int mi3d_cx_forward(mi3d_cx_t h, const float* x, const float* y, float band_width, int need_grad, float* loss, mi3d_stream_t stream) {
-    if (!h || !x || !y || !loss || !(band_width > 0.f)) return MI3D_ERR_ARG;
-    cx::Engine& e = h->e; const mi3d_cx_cfg& c = e.cfg;
+int mi3d_cx_forward(mi3d_engine_t h, const float* x, const float* y, float band_width, int need_grad, float* loss, mi3d_stream_t stream) {
+    cx::Engine* ep = plan::engine_of<cx::Engine>(h);
+    if (!ep || !x || !y || !loss || !(band_width > 0.f)) return MI3D_ERR_ARG;
+    cx::Engine& e = *ep; const mi3d_cx_cfg& c = e.cfg;
     cudaStream_t st = (cudaStream_t)stream;
     e.tape_valid = false;
     cxk::k_prep<<<plan::Builder::blocks_for((size_t)2 * c.N * c.H * c.W), 256, 0, st>>>(x, y, c.N, c.H, c.W, e.img4.p);
@@ -244,23 +203,16 @@ int mi3d_cx_forward(mi3d_cx_t h, const float* x, const float* y, float band_widt
     return MI3D_OK;
 }
 
-int mi3d_cx_backward(mi3d_cx_t h, const float* dloss, float* dx, mi3d_stream_t stream) {
-    if (!h || !dloss || !dx) return MI3D_ERR_ARG;
-    cx::Engine& e = h->e; const mi3d_cx_cfg& c = e.cfg;
+int mi3d_cx_backward(mi3d_engine_t h, const float* dloss, float* dx, mi3d_stream_t stream) {
+    cx::Engine* ep = plan::engine_of<cx::Engine>(h);
+    if (!ep || !dloss || !dx) return MI3D_ERR_ARG;
+    cx::Engine& e = *ep; const mi3d_cx_cfg& c = e.cfg;
     if (!e.tape_valid) return MI3D_ERR_ARG;
     cudaStream_t st = (cudaStream_t)stream;
     MI3D_CHECK(cudaMemcpyAsync(e.dloss, dloss, sizeof(float), cudaMemcpyDeviceToDevice, st));
     int r = e.run(e.bwd, st); if (r) return r;
     cxk::k_img_grad<<<plan::Builder::blocks_for((size_t)c.N * 3 * c.H * c.W), 256, 0, st>>>(e.g4, e.gscale, c.N, c.H, c.W, dx);
     return (int)cudaGetLastError();
-}
-
-int mi3d_cx_debug_tensor(mi3d_cx_t h, const char* name, void** ptr, size_t* bytes) {
-    if (!h || !name || !ptr || !bytes) return MI3D_ERR_ARG;
-    auto it = h->e.named.find(name);
-    if (it == h->e.named.end()) return MI3D_ERR_ARG;
-    *ptr = it->second.first; *bytes = it->second.second;
-    return MI3D_OK;
 }
 
 }  // extern "C"

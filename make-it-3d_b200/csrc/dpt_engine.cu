@@ -433,63 +433,26 @@ struct Engine : TowerBuilder {
         cur = nullptr;
         return err;
     }
+
+    int load_param(const Param& P, const float* src, const float* partner, cudaStream_t st) override {
+        if (P.kind != PK_CONV_WS) return Builder::load_param(P, src, partner, st);
+        dptk::k_ws_conv<<<P.shape[0], 256, 0, st>>>(src, (__half*)P.dst, P.shape[1], P.shape[2] * P.shape[3]);
+        return (int)cudaGetLastError();
+    }
 };
 
 }  // namespace dpt
 
-struct mi3d_dpt { dpt::Engine e; };
-
 extern "C" {
 
-size_t mi3d_dpt_workspace_bytes(void) {
-    dpt::Engine e;
-    e.build(true);
-    return e.off + (1 << 20);
-}
+size_t mi3d_dpt_workspace_bytes(void) { return plan::workspace_bytes<dpt::Engine>(); }
 
-mi3d_dpt_t mi3d_dpt_create(void* workspace, size_t workspace_bytes) {
-    if (!workspace) return nullptr;
-    mi3d_dpt* h = new mi3d_dpt();
-    h->e.base = (uint8_t*)workspace; h->e.cap = workspace_bytes;
-    int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&h->e.num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (h->e.build(false) != 0) { delete h; return nullptr; }
-    return h;
-}
+mi3d_engine_t mi3d_dpt_create(void* workspace, size_t workspace_bytes) { return plan::create<dpt::Engine>(workspace, workspace_bytes); }
 
-void mi3d_dpt_destroy(mi3d_dpt_t h) { delete h; }
-
-int mi3d_dpt_num_params(mi3d_dpt_t h) { return h ? (int)h->e.params.size() : 0; }
-const char* mi3d_dpt_param_name(mi3d_dpt_t h, int i) {
-    if (!h || i < 0 || i >= (int)h->e.params.size()) return nullptr;
-    return h->e.params[i].name.c_str();
-}
-int mi3d_dpt_param_shape(mi3d_dpt_t h, int i, int* shape4) {
-    if (!h || !shape4 || i < 0 || i >= (int)h->e.params.size()) return -1;
-    const auto& s = h->e.params[i].shape;
-    for (int k = 0; k < 4; k++) shape4[k] = k < (int)s.size() ? s[k] : 0;
-    return (int)s.size();
-}
-
-int mi3d_dpt_load_param(mi3d_dpt_t h, int i, const float* src, mi3d_stream_t stream) {
-    if (!h || i < 0 || i >= (int)h->e.params.size() || !src) return MI3D_ERR_ARG;
-    cudaStream_t st = (cudaStream_t)stream;
-    const plan::Param& P = h->e.params[i];
-    const int nb = plan::Builder::blocks_for(P.numel);
-    switch (P.kind) {
-        case plan::PK_F32: MI3D_CHECK(cudaMemcpyAsync(P.dst, src, P.numel * 4, cudaMemcpyDeviceToDevice, st)); break;
-        case plan::PK_LINEAR: sdk::k_f32_to_f16<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.numel); break;
-        case plan::PK_CONV3: sdk::k_conv_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.shape[0], P.shape[1], 0); break;
-        case plan::PK_CONV_WS:
-            dptk::k_ws_conv<<<P.shape[0], 256, 0, st>>>(src, (__half*)P.dst, P.shape[1], P.shape[2] * P.shape[3]);
-            break;
-        default: return MI3D_ERR_ARG;
-    }
-    return (int)cudaGetLastError();
-}
-
-int mi3d_dpt_forward(mi3d_dpt_t h, const float* img, float* out, mi3d_stream_t stream) {
-    if (!h || !img || !out) return MI3D_ERR_ARG;
-    dpt::Engine& e = h->e;
+int mi3d_dpt_forward(mi3d_engine_t h, const float* img, float* out, mi3d_stream_t stream) {
+    dpt::Engine* ep = plan::engine_of<dpt::Engine>(h);
+    if (!ep || !img || !out) return MI3D_ERR_ARG;
+    dpt::Engine& e = *ep;
     cudaStream_t st = (cudaStream_t)stream;
     MI3D_CHECK(cudaMemcpyAsync(e.img, img, (size_t)3 * dpt::kImg * dpt::kImg * sizeof(float), cudaMemcpyDeviceToDevice, st));
     int r = e.run_eager(e.fwd, st); if (r) return r;
@@ -497,9 +460,10 @@ int mi3d_dpt_forward(mi3d_dpt_t h, const float* img, float* out, mi3d_stream_t s
     return MI3D_OK;
 }
 
-int mi3d_dpt_tap(mi3d_dpt_t h, int i, float* dst, mi3d_stream_t stream) {
-    if (!h || !dst || i < 0 || i > 3) return MI3D_ERR_ARG;
-    const plan::T4& t = h->e.taps[i];
+int mi3d_dpt_tap(mi3d_engine_t h, int i, float* dst, mi3d_stream_t stream) {
+    dpt::Engine* ep = plan::engine_of<dpt::Engine>(h);
+    if (!ep || !dst || i < 0 || i > 3) return MI3D_ERR_ARG;
+    const plan::T4& t = ep->taps[i];
     const size_t n = t.numel();
     dptk::k_nhwc_to_nchw_f32<<<plan::Builder::blocks_for(n), 256, 0, (cudaStream_t)stream>>>(t.p, dst, t.h * t.w, t.c);
     return (int)cudaGetLastError();

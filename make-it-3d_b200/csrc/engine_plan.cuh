@@ -1,9 +1,10 @@
-// engine_plan.cuh -- the op-builder layer shared by the planned engines (sd_engine.cu, clip_engine.cu, cx_engine.cu).
+// engine_plan.cuh -- the op-builder layer shared by the planned engines (sd, sd_text, clip, cx, unet, dpt and blip2_engine.cu).
 //
 // An engine is built twice: a dry run sizes the caller's workspace, the real run carves parameters and activations out of it
 // (bump allocation, nothing is ever freed or reused) and records one closure per launch into static launch lists.  What lives
-// here: the parameter registry, the workspace carving, the op builders over the tile GEMM / fused attention / memory-bound
-// kernels, and the replay of a list as a CUDA graph.
+// here: the parameter registry and its weight loading, the workspace carving, the op builders over the tile GEMM / fused
+// attention / memory-bound kernels, the replay of a list as a CUDA graph, and the create / size steps every engine's C entry
+// points share (the generic mi3d_engine_* functions are in engine.cu).
 #pragma once
 #include <functional>
 #include <cstdio>
@@ -18,13 +19,19 @@
 #include "tc_host.cuh"
 #include "attn.cuh"
 
+// The opaque handle of include/mi3d.h: every planned engine is one (plan::Builder derives from it).
+struct mi3d_engine { virtual ~mi3d_engine() {} };
+
 namespace plan {
 
 using Op = std::function<int(cudaStream_t)>;
 
-// How a parameter is stored in the workspace.  The engines' load functions turn the fp32 source tensor into this form.
-enum PKind { PK_F32 = 0, PK_LINEAR, PK_LINEAR_T, PK_LINEAR_BOTH, PK_CONV3, PK_CONV3_BOTH, PK_CONV1, PK_CONV1_BOTH, PK_GEGLU_W, PK_GEGLU_B,
-             PK_CONV_F32_OHWI, PK_CONV_SMALL_COUT, PK_CONV_SMALL_COUT_BOTH,
+// How a parameter is stored in the workspace; one kind is one layout in every engine.  Builder::load_param writes the kinds all
+// engines share from the fp32 source tensor, an engine's override the kinds only it uses.
+enum PKind { PK_F32 = 0, PK_LINEAR, PK_LINEAR_T, PK_LINEAR_BOTH, PK_CONV3, PK_CONV3_BOTH, PK_CONV1, PK_CONV1_BOTH,
+             PK_CONV3_S2_BOTH,                                          // sd_engine.cu: strided 3x3 conv, dst2 = [9*I][O] (im2col dgrad)
+             PK_GEGLU_W, PK_GEGLU_B, PK_CONV_F32_OHWI, PK_CONV_SMALL_COUT, PK_CONV_SMALL_COUT_BOTH,   // sd_engine.cu
+             PK_CX_CONV_IN, PK_CX_CONV_IN_DGRAD,                        // cx_engine.cu: VGG conv1_1, fp32 forward and flipped fp16 copy
              PK_CONV_WS };   // weight-standardised conv (dpt_engine.cu): OIHW fp32 -> standardised [O][kh][kw][I] fp16
 
 struct Param {
@@ -40,7 +47,7 @@ struct T4 {  // NHWC fp16 activation
     long long rows() const { return (long long)n * h * w; }
 };
 
-struct Builder {
+struct Builder : mi3d_engine {
     uint8_t* base = nullptr; size_t cap = 0, off = 0; bool dry = true; int err = 0;
     int num_sms = 132;
     std::vector<Param> params; std::map<std::string, int> pindex;
@@ -85,10 +92,12 @@ struct Builder {
         for (int s : shape) P.numel *= (size_t)s;
         switch (kind) {
             case PK_F32: case PK_GEGLU_B: P.dst = alloc(P.numel * 4); break;
-            case PK_CONV_F32_OHWI: P.dst = alloc((size_t)std::max(shape[0], shape[1]) * 9 * 8 * 4); break;   // input channels padded to <= 8
-            case PK_LINEAR: case PK_CONV3: case PK_CONV1: case PK_GEGLU_W: case PK_LINEAR_T: case PK_CONV_SMALL_COUT: case PK_CONV_WS:
+            case PK_CONV_F32_OHWI: case PK_CX_CONV_IN:                                                         // input channels padded to <= 8
+                P.dst = alloc((size_t)std::max(shape[0], shape[1]) * 9 * 8 * 4); break;
+            case PK_LINEAR: case PK_CONV3: case PK_CONV1: case PK_GEGLU_W: case PK_LINEAR_T: case PK_CONV_SMALL_COUT: case PK_CX_CONV_IN_DGRAD:
+            case PK_CONV_WS:
                 P.dst = alloc(P.numel * 2); break;
-            case PK_LINEAR_BOTH: case PK_CONV3_BOTH: case PK_CONV1_BOTH: case PK_CONV_SMALL_COUT_BOTH:
+            case PK_LINEAR_BOTH: case PK_CONV3_BOTH: case PK_CONV1_BOTH: case PK_CONV3_S2_BOTH: case PK_CONV_SMALL_COUT_BOTH:
                 P.dst = alloc(P.numel * 2); P.dst2 = alloc(P.numel * 2); break;
         }
         pindex[name] = (int)params.size();
@@ -105,6 +114,29 @@ struct Builder {
         pindex[name] = (int)params.size();
         params.push_back(P);
         return params.back();
+    }
+
+    // Writes P from src, an fp32 device tensor in torch's layout (for a '#' entry: its base tensor).  partner: the second tensor of a
+    // pair written together (SD's GEGLU weight and bias).  The base handles the kinds every engine lays out alike; an engine overrides
+    // it for its own kinds and passes the rest on.
+    virtual int load_param(const Param& P, const float* src, const float* partner, cudaStream_t st) {
+        (void)partner;
+        const int nb = blocks_for(P.numel);
+        const int O = P.shape.empty() ? 1 : P.shape[0], I = (int)(P.numel / (size_t)O);   // a conv [O][I][kh][kw] as the matrix [O][I*kh*kw]
+        switch (P.kind) {
+            case PK_F32: MI3D_CHECK(cudaMemcpyAsync(P.dst, src, P.numel * 4, cudaMemcpyDeviceToDevice, st)); break;
+            case PK_LINEAR: case PK_CONV1: sdk::k_f32_to_f16<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.numel); break;
+            case PK_LINEAR_T: sdk::k_transpose_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst, O, I); break;
+            case PK_LINEAR_BOTH: case PK_CONV1_BOTH:
+                sdk::k_f32_to_f16<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.numel);
+                sdk::k_transpose_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst2, O, I); break;
+            case PK_CONV3: sdk::k_conv_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.shape[0], P.shape[1], 0); break;
+            case PK_CONV3_BOTH:                                                     // dst2: the flipped, transposed dgrad weights
+                sdk::k_conv_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.shape[0], P.shape[1], 0);
+                sdk::k_conv_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst2, P.shape[0], P.shape[1], 1); break;
+            default: return MI3D_ERR_ARG;
+        }
+        return (int)cudaGetLastError();
     }
 
     // ------------------------------------------------------------------------------------------------------
@@ -265,7 +297,7 @@ struct Builder {
     }
     // The launch lists are static (fixed pointers, shapes and order; every input lives in a device buffer), so a list replays as ONE
     // CUDA graph from its third call on (the lists lose their CPU launch cost and inter-kernel gaps).  Enabled per engine
-    // (mi3d_sd_set_graph_replay / mi3d_clip_set_graph_replay); needs a capturable stream (torch's legacy default stream is not: the
+    // (mi3d_engine_set_graph_replay); needs a capturable stream (torch's legacy default stream is not: the
     // Python engines run on their own stream, event-ordered against the caller's).  A list whose capture fails falls back to plain
     // launches for good.
     struct ListGraph { cudaGraphExec_t exec = nullptr; int calls = 0; bool failed = false; };
@@ -293,7 +325,25 @@ struct Builder {
         for (auto& kv : graphs) if (kv.second.exec) n++;
         return n;
     }
-    ~Builder() { for (auto& kv : graphs) if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec); }
+    ~Builder() override { for (auto& kv : graphs) if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec); }
 };
+
+// The create / size steps of every engine's C entry points.  E is constructed from the configuration arguments and has build(dry).
+// Workspace size: the dry build's carve plus 1 MiB of slack; 0 when the dry build fails.
+template <class E, class... Cfg> size_t workspace_bytes(const Cfg&... cfg) {
+    E e(cfg...);
+    return e.build(true) ? 0 : e.off + (1 << 20);
+}
+// The engine planned inside the caller's workspace (the real build, for this device's SM count); nullptr on failure.
+template <class E, class... Cfg> E* create(void* workspace, size_t bytes, const Cfg&... cfg) {
+    if (!workspace) return nullptr;
+    E* e = new E(cfg...);
+    e->base = (uint8_t*)workspace; e->cap = bytes;
+    int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&e->num_sms, cudaDevAttrMultiProcessorCount, dev);
+    if (e->build(false) != 0) { delete e; return nullptr; }
+    return e;
+}
+// The engine of type E behind a handle; nullptr for NULL or another engine's handle (its entry points then return MI3D_ERR_ARG).
+template <class E> E* engine_of(mi3d_engine_t h) { return dynamic_cast<E*>(h); }
 
 }  // namespace plan

@@ -18,6 +18,10 @@ using namespace plan;
 
 struct Engine : Builder {
     mi3d_unet_cfg ucfg; mi3d_vae_cfg vcfg;
+    // either part may be absent (NULL); a VAE-only engine takes its GroupNorm group count from the VAE
+    Engine(const mi3d_unet_cfg* u, const mi3d_vae_cfg* v) : ucfg(u ? *u : mi3d_unet_cfg{}), vcfg(v ? *v : mi3d_vae_cfg{}) {
+        if (v && !u) ucfg.groups = v->groups;
+    }
     std::vector<Op> unet_ops, enc_ops, enc_bwd_ops;
     // GroupNorm statistics of one op list live in one pool, cleared by a single memset at the head of the list
     uint8_t* pool = nullptr; size_t pool_used = 0; static constexpr size_t kPoolBytes = 256 * 1024;
@@ -190,7 +194,7 @@ struct Engine : Builder {
             sdk::k_im2col_s2<<<blocks_for((size_t)Mo * 9 * C / 8), 256, 0, st>>>(xx.p, col, xx.n, xx.h, xx.w, C, Ho, Wo, pad_lo);
             return (int)cudaGetLastError();
         });
-        Param& w = param(pre + ".conv.weight", {C, C, 3, 3}, both ? PK_CONV3_BOTH : PK_CONV3);
+        Param& w = param(pre + ".conv.weight", {C, C, 3, 3}, both ? PK_CONV3_S2_BOTH : PK_CONV3);
         T4 y = act(x.n, Ho, Wo, C);
         linear(col, Mo, 9 * C, (const __half*)w.dst, C, y.p, pf(pre + ".conv.bias", {C}));
         if (col_out) *col_out = col;
@@ -580,7 +584,7 @@ struct Engine : Builder {
                 const DownTape& d = vdown[di--];
                 const int C = d.x.c; const long long Mo = d.y.rows();
                 Param& w = params[pindex[d.pre + ".conv.weight"]];
-                // dcol[Mo, 9C] = dy[Mo, C] . Wt   with Wt = [9C][C]  (dst2 of a CONV3_BOTH strided weight = plain transpose, see load)
+                // dcol[Mo, 9C] = dy[Mo, C] . Wt   with Wt = [9C][C]  (dst2 of a PK_CONV3_S2_BOTH weight = plain transpose, see load_param)
                 __half* dcol = alloc16((size_t)Mo * 9 * C);
                 linear(dh.p, Mo, C, (const __half*)w.dst2, 9 * C, dcol);
                 T4 dx = act(d.x.n, d.x.h, d.x.w, C);
@@ -646,6 +650,66 @@ struct Engine : Builder {
         if (ucfg.n_levels > 0) build_unet();
         if (vcfg.n_levels > 0) { build_vae(); build_vae_bwd(); if (vcfg.decoder) build_vae_dec(); }
         return err;
+    }
+
+    int load_param(const Param& P, const float* src, const float* partner, cudaStream_t st) override {
+        const int nb = blocks_for(P.numel);
+        using namespace sdk;
+        switch (P.kind) {
+            case PK_CONV3_S2_BOTH:
+                // dgrad of the im2col GEMM needs the plain transpose of the [Cout][9*Cin] matrix: [9*Cin][Cout]
+                // (k_conv_w wrote [O][ky][kx][I]; transpose that fp16 matrix)
+                k_conv_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.shape[0], P.shape[1], 0);
+                k_transpose<<<dim3((9 * P.shape[1] + 31) / 32, (P.shape[0] + 31) / 32, 1), dim3(32, 8), 0, st>>>((const __half*)P.dst, (__half*)P.dst2, P.shape[0], 9 * P.shape[1]);
+                break;
+            case PK_GEGLU_W: {
+                if (!partner) return MI3D_ERR_ARG;
+                const Param& Bp = params[pindex[P.partner]];
+                k_geglu_w<<<nb, 256, 0, st>>>(src, partner, (__half*)P.dst, (float*)Bp.dst, P.shape[0] / 2, P.shape[1]);
+                break;
+            }
+            case PK_GEGLU_B: break;     // written together with the weight
+            case PK_CONV_F32_OHWI: {
+                // fp32 direct-conv weights.  Base form: OIHW [O][I][3][3] -> [O][ky][kx][Ipad] with Ipad = 4 (conv_in) ;
+                // "#dgrad_f32" form (conv_out transposed): src is conv_out OIHW [8][ch][3][3] -> [ch][2-ky][2-kx][8]
+                std::vector<float> tmp;   // host staging keeps this one-off path simple
+                const bool dg = P.name.find("#dgrad_f32") != std::string::npos;
+                const int O = dg ? P.shape[1] : P.shape[0], I = dg ? P.shape[0] : P.shape[1];
+                std::vector<float> hsrc((size_t)O * I * 9);
+                MI3D_CHECK(cudaMemcpyAsync(hsrc.data(), src, hsrc.size() * 4, cudaMemcpyDeviceToHost, st));
+                MI3D_CHECK(cudaStreamSynchronize(st));
+                if (!dg) {
+                    const int Ip = 4;
+                    tmp.assign((size_t)O * 9 * Ip, 0.f);
+                    for (int o = 0; o < O; o++) for (int c = 0; c < I; c++) for (int t = 0; t < 9; t++) tmp[((size_t)o * 9 + t) * Ip + c] = hsrc[((size_t)o * I + c) * 9 + t];
+                } else {
+                    // hsrc = conv_out [O=8][I=ch][3][3]; want w'[ci=ch][ky'][kx'][co=8] = hsrc[co][ci][2-ky'][2-kx']
+                    tmp.assign((size_t)I * 9 * O, 0.f);
+                    for (int o = 0; o < O; o++) for (int c = 0; c < I; c++) for (int t = 0; t < 9; t++) tmp[((size_t)c * 9 + (8 - t)) * O + o] = hsrc[((size_t)o * I + c) * 9 + t];
+                }
+                MI3D_CHECK(cudaMemcpyAsync(P.dst, tmp.data(), std::min(tmp.size(), dg ? P.numel : tmp.size()) * 4, cudaMemcpyHostToDevice, st));
+                MI3D_CHECK(cudaStreamSynchronize(st));
+                break;
+            }
+            case PK_CONV_SMALL_COUT: case PK_CONV_SMALL_COUT_BOTH: {
+                const bool dg = P.name.find("#dgrad") != std::string::npos;
+                if (!dg) k_conv_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.shape[0], P.shape[1], 0);
+                else {
+                    // conv_in transposed: src conv_in OIHW [c0][3][3][3]; want [4 (padded cin)][2-ky][2-kx][c0] fp16
+                    const int c0 = P.shape[1];
+                    std::vector<float> hsrc((size_t)c0 * 3 * 9);
+                    MI3D_CHECK(cudaMemcpyAsync(hsrc.data(), src, hsrc.size() * 4, cudaMemcpyDeviceToHost, st));
+                    MI3D_CHECK(cudaStreamSynchronize(st));
+                    std::vector<__half> tmp((size_t)4 * 9 * c0, __float2half(0.f));
+                    for (int o = 0; o < c0; o++) for (int c = 0; c < 3; c++) for (int t = 0; t < 9; t++) tmp[((size_t)c * 9 + (8 - t)) * c0 + o] = __float2half(hsrc[((size_t)o * 3 + c) * 9 + t]);
+                    MI3D_CHECK(cudaMemcpyAsync(P.dst, tmp.data(), tmp.size() * 2, cudaMemcpyHostToDevice, st));
+                    MI3D_CHECK(cudaStreamSynchronize(st));
+                }
+                break;
+            }
+            default: return Builder::load_param(P, src, partner, st);
+        }
+        return (int)cudaGetLastError();
     }
 };
 
@@ -804,143 +868,27 @@ __global__ void k_cfg_sds(const float* __restrict__ unet_out /*[2][pix][4]*/, co
 
 }  // namespace sd
 
-struct mi3d_sd { sd::Engine e; };
-
 extern "C" {
 
-size_t mi3d_sd_workspace_bytes(const mi3d_unet_cfg* u, const mi3d_vae_cfg* v) {
-    sd::Engine e;
-    e.ucfg = u ? *u : mi3d_unet_cfg{}; e.vcfg = v ? *v : mi3d_vae_cfg{};
-    if (v && !u) e.ucfg.groups = v->groups;
-    e.build(true);
-    return e.off + (1 << 20);
-}
+size_t mi3d_sd_workspace_bytes(const mi3d_unet_cfg* u, const mi3d_vae_cfg* v) { return plan::workspace_bytes<sd::Engine>(u, v); }
 
-mi3d_sd_t mi3d_sd_create(const mi3d_unet_cfg* u, const mi3d_vae_cfg* v, void* workspace, size_t workspace_bytes) {
-    if (!workspace) return nullptr;
-    mi3d_sd* h = new mi3d_sd();
-    h->e.ucfg = u ? *u : mi3d_unet_cfg{}; h->e.vcfg = v ? *v : mi3d_vae_cfg{};
-    if (v && !u) h->e.ucfg.groups = v->groups;
-    h->e.base = (uint8_t*)workspace; h->e.cap = workspace_bytes;
-    int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&h->e.num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (h->e.build(false) != 0) { delete h; return nullptr; }
+mi3d_engine_t mi3d_sd_create(const mi3d_unet_cfg* u, const mi3d_vae_cfg* v, void* workspace, size_t workspace_bytes) {
+    sd::Engine* e = plan::create<sd::Engine>(workspace, workspace_bytes, u, v);
+    if (!e) return nullptr;
     cudaFuncSetAttribute(sdk::k_conv_small_cin<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     cudaFuncSetAttribute(sdk::k_conv_small_cin<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
     cudaFuncSetAttribute(sdk::k_conv_small_cout<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
     cudaFuncSetAttribute(sdk::k_conv_small_cout<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-    return h;
+    return e;
 }
 
-void mi3d_sd_destroy(mi3d_sd_t h) { delete h; }
-
-int mi3d_sd_num_params(mi3d_sd_t h) { return h ? (int)h->e.params.size() : 0; }
-const char* mi3d_sd_param_name(mi3d_sd_t h, int i) { return h->e.params[i].name.c_str(); }
-long long mi3d_sd_param_numel(mi3d_sd_t h, int i) { return (long long)h->e.params[i].numel; }
-int mi3d_sd_param_shape(mi3d_sd_t h, int i, int* shape4) {
-    if (!h || i < 0 || i >= (int)h->e.params.size()) return -1;
-    const auto& s = h->e.params[i].shape;
-    for (int k = 0; k < 4; k++) shape4[k] = k < (int)s.size() ? s[k] : 0;
-    return (int)s.size();
-}
-
-// src: fp32 device tensor in the diffusers layout named by mi3d_sd_param_name (names with a '#' suffix are derived copies: pass the base tensor)
-int mi3d_sd_load_param(mi3d_sd_t h, int i, const float* src, const float* partner_src, mi3d_stream_t stream) {
-    if (!h || i < 0 || i >= (int)h->e.params.size() || !src) return MI3D_ERR_ARG;
-    cudaStream_t st = (cudaStream_t)stream;
-    sd::Param& P = h->e.params[i];
-    const int nb = sd::Engine::blocks_for(P.numel);
-    using namespace sdk;
-    switch (P.kind) {
-        case sd::PK_F32: MI3D_CHECK(cudaMemcpyAsync(P.dst, src, P.numel * 4, cudaMemcpyDeviceToDevice, st)); break;
-        case sd::PK_LINEAR: case sd::PK_CONV1: k_f32_to_f16<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.numel); break;
-        case sd::PK_LINEAR_BOTH: case sd::PK_CONV1_BOTH:
-            k_f32_to_f16<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.numel);
-            k_transpose_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst2, P.shape[0], P.shape[1]); break;
-        case sd::PK_LINEAR_T: k_transpose_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.shape[0], P.shape[1]); break;
-        case sd::PK_CONV3: k_conv_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.shape[0], P.shape[1], 0); break;
-        case sd::PK_CONV3_BOTH: {
-            k_conv_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.shape[0], P.shape[1], 0);
-            const bool strided = P.name.find("downsamplers") != std::string::npos;
-            if (strided) {
-                // dgrad of the im2col GEMM needs the plain transpose of the [Cout][9*Cin] matrix: [9*Cin][Cout]
-                // (k_conv_w wrote [O][ky][kx][I]; transpose that fp16 matrix)
-                k_transpose<<<dim3((9 * P.shape[1] + 31) / 32, (P.shape[0] + 31) / 32, 1), dim3(32, 8), 0, st>>>((const __half*)P.dst, (__half*)P.dst2, P.shape[0], 9 * P.shape[1]);
-            } else {
-                k_conv_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst2, P.shape[0], P.shape[1], 1);
-            }
-            break;
-        }
-        case sd::PK_GEGLU_W: {
-            if (!partner_src) return MI3D_ERR_ARG;
-            sd::Param& Bp = h->e.params[h->e.pindex[P.partner]];
-            k_geglu_w<<<nb, 256, 0, st>>>(src, partner_src, (__half*)P.dst, (float*)Bp.dst, P.shape[0] / 2, P.shape[1]);
-            break;
-        }
-        case sd::PK_GEGLU_B: break;     // written together with the weight
-        case sd::PK_CONV_F32_OHWI: {
-            // fp32 direct-conv weights.  Base form: OIHW [O][I][3][3] -> [O][ky][kx][Ipad] with Ipad = 4 (conv_in) ;
-            // "#dgrad_f32" form (conv_out transposed): src is conv_out OIHW [8][ch][3][3] -> [ch][2-ky][2-kx][8]
-            std::vector<float> tmp;   // host staging keeps this one-off path simple
-            const bool dg = P.name.find("#dgrad_f32") != std::string::npos;
-            const int O = dg ? P.shape[1] : P.shape[0], I = dg ? P.shape[0] : P.shape[1];
-            std::vector<float> hsrc((size_t)O * I * 9);
-            MI3D_CHECK(cudaMemcpyAsync(hsrc.data(), src, hsrc.size() * 4, cudaMemcpyDeviceToHost, st));
-            MI3D_CHECK(cudaStreamSynchronize(st));
-            if (!dg) {
-                const int Ip = 4;
-                tmp.assign((size_t)O * 9 * Ip, 0.f);
-                for (int o = 0; o < O; o++) for (int c = 0; c < I; c++) for (int t = 0; t < 9; t++) tmp[((size_t)o * 9 + t) * Ip + c] = hsrc[((size_t)o * I + c) * 9 + t];
-            } else {
-                // hsrc = conv_out [O=8][I=ch][3][3]; want w'[ci=ch][ky'][kx'][co=8] = hsrc[co][ci][2-ky'][2-kx']
-                tmp.assign((size_t)I * 9 * O, 0.f);
-                for (int o = 0; o < O; o++) for (int c = 0; c < I; c++) for (int t = 0; t < 9; t++) tmp[((size_t)c * 9 + (8 - t)) * O + o] = hsrc[((size_t)o * I + c) * 9 + t];
-            }
-            if (tmp.size() * 4 > P.numel * 4 + (dg ? 0 : (size_t)O * 9 * 4 * 4)) {}
-            MI3D_CHECK(cudaMemcpyAsync(P.dst, tmp.data(), std::min(tmp.size(), dg ? P.numel : tmp.size()) * 4, cudaMemcpyHostToDevice, st));
-            MI3D_CHECK(cudaStreamSynchronize(st));
-            break;
-        }
-        case sd::PK_CONV_SMALL_COUT: case sd::PK_CONV_SMALL_COUT_BOTH: {
-            const bool dg = P.name.find("#dgrad") != std::string::npos;
-            if (!dg) k_conv_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.shape[0], P.shape[1], 0);
-            else {
-                // conv_in transposed: src conv_in OIHW [c0][3][3][3]; want [4 (padded cin)][2-ky][2-kx][c0] fp16
-                const int c0 = P.shape[1];
-                std::vector<float> hsrc((size_t)c0 * 3 * 9);
-                MI3D_CHECK(cudaMemcpyAsync(hsrc.data(), src, hsrc.size() * 4, cudaMemcpyDeviceToHost, st));
-                MI3D_CHECK(cudaStreamSynchronize(st));
-                std::vector<__half> tmp((size_t)4 * 9 * c0, __float2half(0.f));
-                for (int o = 0; o < c0; o++) for (int c = 0; c < 3; c++) for (int t = 0; t < 9; t++) tmp[((size_t)c * 9 + (8 - t)) * c0 + o] = __float2half(hsrc[((size_t)o * 3 + c) * 9 + t]);
-                MI3D_CHECK(cudaMemcpyAsync(P.dst, tmp.data(), tmp.size() * 2, cudaMemcpyHostToDevice, st));
-                MI3D_CHECK(cudaStreamSynchronize(st));
-            }
-            break;
-        }
-    }
-    return (int)cudaGetLastError();
-}
-
-// enable != 0: start timing every tensor-core tile launch with CUDA events; enable == 0: stop, synchronise the events and
-// return the accumulated kernel milliseconds and launch count since the last enable
-int mi3d_sd_set_graph_replay(mi3d_sd_t h, int enable) {
-    if (!h) return MI3D_ERR_ARG;
-    h->e.use_graph = enable != 0;
-    return MI3D_OK;
-}
-
-int mi3d_sd_graph_replays(mi3d_sd_t h) {
-    if (!h) return -1;
-    int n = 0;
-    for (auto& kv : h->e.graphs) if (kv.second.exec) n++;
-    return n;
-}
-
-int mi3d_sd_profile(mi3d_sd_t h, int enable, float* gemm_ms, int* launches) { return mi3d_sd_profile_dump(h, enable, gemm_ms, launches, nullptr); }
+int mi3d_sd_profile(mi3d_engine_t h, int enable, float* gemm_ms, int* launches) { return mi3d_sd_profile_dump(h, enable, gemm_ms, launches, nullptr); }
 
 // dump_path_host (nullable): one text line per timed launch "M N K block_n splits conv batch epi ms" (bench.py derives FLOPs from it)
-int mi3d_sd_profile_dump(mi3d_sd_t h, int enable, float* gemm_ms, int* launches, const char* dump) {
-    if (!h) return MI3D_ERR_ARG;
-    sd::Engine& e = h->e;
+int mi3d_sd_profile_dump(mi3d_engine_t h, int enable, float* gemm_ms, int* launches, const char* dump) {
+    sd::Engine* ep = plan::engine_of<sd::Engine>(h);
+    if (!ep) return MI3D_ERR_ARG;
+    sd::Engine& e = *ep;
     if (enable) { e.profile = true; e.prof_used = 0; return MI3D_OK; }
     e.profile = false;
     float total = 0.f; int n_tile = 0;
@@ -958,17 +906,11 @@ int mi3d_sd_profile_dump(mi3d_sd_t h, int enable, float* gemm_ms, int* launches,
     return MI3D_OK;
 }
 
-int mi3d_sd_debug_tensor(mi3d_sd_t h, const char* name, void** ptr, size_t* bytes) {
-    auto it = h->e.named.find(name);
-    if (it == h->e.named.end()) return MI3D_ERR_ARG;
-    *ptr = it->second.first; *bytes = it->second.second;
-    return MI3D_OK;
-}
-
 // nerf/sd.py:124,133,212-220 : pred_rgb [1,3,H,W] fp32 -> bilinear to image_hw -> VAE encode -> posterior sample * 0.18215
-int mi3d_sd_encode(mi3d_sd_t h, const float* pred_rgb, int H, int W, const float* eps_posterior, float* latents, mi3d_stream_t stream) {
-    if (!h || h->e.vcfg.n_levels == 0) return MI3D_ERR_ARG;
-    cudaStream_t st = (cudaStream_t)stream; sd::Engine& e = h->e;
+int mi3d_sd_encode(mi3d_engine_t h, const float* pred_rgb, int H, int W, const float* eps_posterior, float* latents, mi3d_stream_t stream) {
+    sd::Engine* ep = plan::engine_of<sd::Engine>(h);
+    if (!ep || ep->vcfg.n_levels == 0) return MI3D_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream; sd::Engine& e = *ep;
     const int S = e.vcfg.image_hw;
     sd::k_interp_in<<<(S * S + 255) / 256, 256, 0, st>>>(pred_rgb, H, W, e.vae_in.p, S);
     int r = e.run(e.enc_ops, st); if (r) return r;
@@ -979,9 +921,10 @@ int mi3d_sd_encode(mi3d_sd_t h, const float* pred_rgb, int H, int W, const float
 }
 
 // backward of mi3d_sd_encode w.r.t. pred_rgb (weights frozen): grad_pred_rgb [1,3,H,W] fp32 (overwritten)
-int mi3d_sd_encode_backward(mi3d_sd_t h, const float* grad_latents, const float* eps_posterior, int H, int W, float* grad_pred_rgb, mi3d_stream_t stream) {
-    if (!h || h->e.vcfg.n_levels == 0) return MI3D_ERR_ARG;
-    cudaStream_t st = (cudaStream_t)stream; sd::Engine& e = h->e;
+int mi3d_sd_encode_backward(mi3d_engine_t h, const float* grad_latents, const float* eps_posterior, int H, int W, float* grad_pred_rgb, mi3d_stream_t stream) {
+    sd::Engine* ep = plan::engine_of<sd::Engine>(h);
+    if (!ep || ep->vcfg.n_levels == 0) return MI3D_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream; sd::Engine& e = *ep;
     const int pix = (int)e.v_h_last.rows(), S = e.vcfg.image_hw;
     const float* qw = (const float*)e.params[e.pindex["quant_conv.weight"]].dst; const float* qb = (const float*)e.params[e.pindex["quant_conv.bias"]].dst;
     sd::k_sample_latents_bwd<<<(pix + 127) / 128, 128, 0, st>>>(e.vae_moments, qw, qb, eps_posterior, grad_latents, e.vae_gmoments, pix);
@@ -999,9 +942,10 @@ int mi3d_sd_ddim_step(const float* noise_pred, const float* latents_noisy, const
 }
 
 // nerf/sd.py:201-210 decode_latents: imgs = (vae.decode(latents / 0.18215).sample / 2 + 0.5).clamp(0, 1); latents fp32 [1,4,h,w] -> imgs fp32 [1,3,S,S]
-int mi3d_sd_decode(mi3d_sd_t h, const float* latents, float* imgs, mi3d_stream_t stream) {
-    if (!h || h->e.vcfg.n_levels == 0 || !h->e.vcfg.decoder || !latents || !imgs) return MI3D_ERR_ARG;
-    cudaStream_t st = (cudaStream_t)stream; sd::Engine& e = h->e;
+int mi3d_sd_decode(mi3d_engine_t h, const float* latents, float* imgs, mi3d_stream_t stream) {
+    sd::Engine* ep = plan::engine_of<sd::Engine>(h);
+    if (!ep || ep->vcfg.n_levels == 0 || !ep->vcfg.decoder || !latents || !imgs) return MI3D_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream; sd::Engine& e = *ep;
     const int pix = (int)e.dec_in.rows(), S = e.vcfg.image_hw;
     const float* qw = (const float*)e.params[e.pindex["post_quant_conv.weight"]].dst; const float* qb = (const float*)e.params[e.pindex["post_quant_conv.bias"]].dst;
     sd::k_dec_in<<<(pix + 127) / 128, 128, 0, st>>>(latents, qw, qb, e.dec_in.p, pix);
@@ -1011,10 +955,11 @@ int mi3d_sd_decode(mi3d_sd_t h, const float* latents, float* imgs, mi3d_stream_t
 }
 
 // nerf/sd.py:138-171 : add_noise -> U-Net on [uncond, text] -> CFG -> SDS gradient.  t: device int64 scalar; alphas: device [1000] fp32
-int mi3d_sd_unet_sds(mi3d_sd_t h, const float* latents, const float* noise, const long long* t, const float* alphas_cumprod,
+int mi3d_sd_unet_sds(mi3d_engine_t h, const float* latents, const float* noise, const long long* t, const float* alphas_cumprod,
                      const float* text_embeddings, float guidance_scale, float* noise_pred, float* grad, mi3d_stream_t stream) {
-    if (!h || h->e.ucfg.n_levels == 0) return MI3D_ERR_ARG;
-    cudaStream_t st = (cudaStream_t)stream; sd::Engine& e = h->e;
+    sd::Engine* ep = plan::engine_of<sd::Engine>(h);
+    if (!ep || ep->ucfg.n_levels == 0) return MI3D_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream; sd::Engine& e = *ep;
     const int pix = e.ucfg.latent_hw * e.ucfg.latent_hw, B = e.ucfg.batch;
     if (B != 2 || e.ucfg.in_ch != 4) return MI3D_ERR_ARG;
     MI3D_CHECK(cudaMemcpyAsync(e.t_dev, t, sizeof(long long), cudaMemcpyDeviceToDevice, st));

@@ -42,6 +42,7 @@ __global__ void k_layernorm_rows_f32(const __half* __restrict__ x, const float* 
 
 struct Engine : TowerBuilder {
     mi3d_sd_text_cfg cfg;
+    explicit Engine(const mi3d_sd_text_cfg& c) : cfg(c) {}
     Tower t;
     std::vector<BlockW> w;
     std::vector<BlockA> a;
@@ -121,63 +122,20 @@ bool valid_cfg(const mi3d_sd_text_cfg& c) {
 
 }  // namespace sdtext
 
-struct mi3d_sd_text { sdtext::Engine e; };
-
 extern "C" {
 
 size_t mi3d_sd_text_workspace_bytes(const mi3d_sd_text_cfg* cfg) {
-    if (!cfg || !sdtext::valid_cfg(*cfg)) return 0;
-    sdtext::Engine e; e.cfg = *cfg;
-    e.build(true);
-    return e.off + (1 << 20);
+    return cfg && sdtext::valid_cfg(*cfg) ? plan::workspace_bytes<sdtext::Engine>(*cfg) : 0;
 }
 
-mi3d_sd_text_t mi3d_sd_text_create(const mi3d_sd_text_cfg* cfg, void* workspace, size_t workspace_bytes) {
-    if (!cfg || !workspace || !sdtext::valid_cfg(*cfg)) return nullptr;
-    mi3d_sd_text* h = new mi3d_sd_text();
-    h->e.cfg = *cfg; h->e.base = (uint8_t*)workspace; h->e.cap = workspace_bytes;
-    int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&h->e.num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (h->e.build(false) != 0) { delete h; return nullptr; }
-    return h;
+mi3d_engine_t mi3d_sd_text_create(const mi3d_sd_text_cfg* cfg, void* workspace, size_t workspace_bytes) {
+    return cfg && sdtext::valid_cfg(*cfg) ? plan::create<sdtext::Engine>(workspace, workspace_bytes, *cfg) : nullptr;
 }
 
-void mi3d_sd_text_destroy(mi3d_sd_text_t h) { delete h; }
-
-int mi3d_sd_text_num_params(mi3d_sd_text_t h) { return h ? (int)h->e.params.size() : 0; }
-const char* mi3d_sd_text_param_name(mi3d_sd_text_t h, int i) {
-    if (!h || i < 0 || i >= (int)h->e.params.size()) return nullptr;
-    return h->e.params[i].name.c_str();
-}
-int mi3d_sd_text_param_shape(mi3d_sd_text_t h, int i, int* shape4) {
-    if (!h || !shape4 || i < 0 || i >= (int)h->e.params.size()) return -1;
-    const auto& s = h->e.params[i].shape;
-    for (int k = 0; k < 4; k++) shape4[k] = k < (int)s.size() ? s[k] : 0;
-    return (int)s.size();
-}
-
-int mi3d_sd_text_load_param(mi3d_sd_text_t h, int i, const float* src, mi3d_stream_t stream) {
-    if (!h || i < 0 || i >= (int)h->e.params.size() || !src) return MI3D_ERR_ARG;
-    cudaStream_t st = (cudaStream_t)stream;
-    const plan::Param& P = h->e.params[i];
-    switch (P.kind) {
-        case plan::PK_F32: MI3D_CHECK(cudaMemcpyAsync(P.dst, src, P.numel * 4, cudaMemcpyDeviceToDevice, st)); break;
-        case plan::PK_LINEAR: sdk::k_f32_to_f16<<<plan::Builder::blocks_for(P.numel), 256, 0, st>>>(src, (__half*)P.dst, P.numel); break;
-        default: return MI3D_ERR_ARG;
-    }
-    return (int)cudaGetLastError();
-}
-
-int mi3d_sd_text_set_graph_replay(mi3d_sd_text_t h, int enable) {
-    if (!h) return MI3D_ERR_ARG;
-    h->e.use_graph = enable != 0;
-    return MI3D_OK;
-}
-
-int mi3d_sd_text_graph_replays(mi3d_sd_text_t h) { return h ? h->e.graph_replays() : -1; }
-
-int mi3d_sd_text_encode(mi3d_sd_text_t h, const long long* ids, int B, float* out, mi3d_stream_t stream) {
-    if (!h || !ids || !out) return MI3D_ERR_ARG;
-    sdtext::Engine& e = h->e; const mi3d_sd_text_cfg& c = e.cfg;
+int mi3d_sd_text_encode(mi3d_engine_t h, const long long* ids, int B, float* out, mi3d_stream_t stream) {
+    sdtext::Engine* ep = plan::engine_of<sdtext::Engine>(h);
+    if (!ep || !ids || !out) return MI3D_ERR_ARG;
+    sdtext::Engine& e = *ep; const mi3d_sd_text_cfg& c = e.cfg;
     if (B < 1 || B > c.max_batch) return MI3D_ERR_ARG;
     cudaStream_t st = (cudaStream_t)stream;
     MI3D_CHECK(cudaMemcpyAsync(e.tokens, ids, (size_t)B * c.context_len * sizeof(long long), cudaMemcpyDeviceToDevice, st));

@@ -23,8 +23,9 @@ using namespace plan;
 // an NCHW fp32 tensor view: channel c of image n at p + n * ns + c * H * W
 struct V { float* p = nullptr; long long ns = 0; };
 
+// what the registry entry of the same index (Builder::params) is, and where the engine keeps its value and gradient
 enum EKind { E_PARAM = 0, E_RMEAN = 1, E_RVAR = 2, E_COUNT = 3 };
-struct Entry { std::string name; std::vector<int> shape; int kind = E_PARAM; float* slot = nullptr; float* grad = nullptr; size_t numel = 1; };
+struct Entry { int kind = E_PARAM; float* slot = nullptr; float* grad = nullptr; };
 
 struct Gated {            // one gated block's storage
     int cin = 0, c = 0, bn = 0;
@@ -42,6 +43,7 @@ constexpr int kMaxWgradElems = kWgradCtas * unk::WOB * unk::WCB * 9;   // S x Co
 
 struct Engine : Builder {
     mi3d_unet_shape cfg;
+    explicit Engine(const mi3d_unet_shape& c) : cfg(c) {}
     std::vector<Entry> entries;
     Gated gs, gd1, gd2, gu2, gu1;
     Conv cu2, cu1, fin;
@@ -57,8 +59,8 @@ struct Engine : Builder {
     static constexpr int kChanChunks = 64;
 
     void add(const std::string& name, std::vector<int> shape, int kind, float* slot, float* grad) {
-        Entry e; e.name = name; e.shape = shape; e.kind = kind; e.slot = slot; e.grad = grad;
-        for (int s : shape) e.numel *= (size_t)s;
+        param_view(name, shape, PK_F32, slot);
+        Entry e; e.kind = kind; e.slot = slot; e.grad = grad;
         entries.push_back(e);
     }
 
@@ -285,7 +287,7 @@ struct Engine : Builder {
     }
 
     int build(bool dry_run) {
-        dry = dry_run; off = 0; err = 0; entries.clear(); named.clear();
+        dry = dry_run; off = 0; err = 0; params.clear(); pindex.clear(); entries.clear(); named.clear();
         fwd_train.clear(); fwd_eval.clear(); bwd_train.clear(); bwd_eval.clear();
         const int N = cfg.N;
         for (int l = 0; l < 3; l++) { H[l] = cfg.H >> l; Wd[l] = cfg.W >> l; HW[l] = (size_t)H[l] * Wd[l]; }
@@ -328,6 +330,9 @@ struct Engine : Builder {
         tap("out", y, (size_t)N * 3 * HW[0] * 4);
         return err;
     }
+
+    // the parameters are read from the caller's tensors on every call (mi3d_unet_forward's state), never loaded
+    int load_param(const Param&, const float*, const float*, cudaStream_t) override { return MI3D_ERR_ARG; }
 };
 
 bool valid_cfg(const mi3d_unet_shape& c) { return c.N >= 1 && c.N <= 16 && c.H >= 4 && c.W >= 4 && c.H % 4 == 0 && c.W % 4 == 0 && c.H <= 4096 && c.W <= 4096; }
@@ -339,52 +344,21 @@ cudaError_t copy_slice(float* dst, long long dst_ns, const float* src, long long
 
 }  // namespace unet
 
-struct mi3d_unet { unet::Engine e; };
-
 extern "C" {
 
 size_t mi3d_unet_workspace_bytes(const mi3d_unet_shape* cfg) {
-    if (!cfg || !unet::valid_cfg(*cfg)) return 0;
-    unet::Engine e; e.cfg = *cfg;
-    e.build(true);
-    return e.off + (1 << 20);
+    return cfg && unet::valid_cfg(*cfg) ? plan::workspace_bytes<unet::Engine>(*cfg) : 0;
 }
 
-mi3d_unet_t mi3d_unet_create(const mi3d_unet_shape* cfg, void* workspace, size_t workspace_bytes) {
-    if (!cfg || !workspace || !unet::valid_cfg(*cfg)) return nullptr;
-    mi3d_unet* h = new mi3d_unet();
-    h->e.cfg = *cfg; h->e.base = (uint8_t*)workspace; h->e.cap = workspace_bytes;
-    int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&h->e.num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (h->e.build(false) != 0) { delete h; return nullptr; }
-    return h;
+mi3d_engine_t mi3d_unet_create(const mi3d_unet_shape* cfg, void* workspace, size_t workspace_bytes) {
+    return cfg && unet::valid_cfg(*cfg) ? plan::create<unet::Engine>(workspace, workspace_bytes, *cfg) : nullptr;
 }
 
-void mi3d_unet_destroy(mi3d_unet_t h) { delete h; }
-
-int mi3d_unet_num_params(mi3d_unet_t h) { return h ? (int)h->e.entries.size() : 0; }
-const char* mi3d_unet_param_name(mi3d_unet_t h, int i) {
-    if (!h || i < 0 || i >= (int)h->e.entries.size()) return nullptr;
-    return h->e.entries[i].name.c_str();
-}
-int mi3d_unet_param_shape(mi3d_unet_t h, int i, int* shape4) {
-    if (!h || !shape4 || i < 0 || i >= (int)h->e.entries.size()) return -1;
-    const auto& s = h->e.entries[i].shape;
-    for (int k = 0; k < 4; k++) shape4[k] = k < (int)s.size() ? s[k] : 0;
-    return (int)s.size();
-}
-
-int mi3d_unet_set_graph_replay(mi3d_unet_t h, int enable) {
-    if (!h) return MI3D_ERR_ARG;
-    h->e.use_graph = enable != 0;
-    return MI3D_OK;
-}
-
-int mi3d_unet_graph_replays(mi3d_unet_t h) { return h ? h->e.graph_replays() : -1; }
-
-int mi3d_unet_forward(mi3d_unet_t h, const float* x0, const float* x1, const float* x2, void* const* state, int train, int need_grad, float* out,
+int mi3d_unet_forward(mi3d_engine_t h, const float* x0, const float* x1, const float* x2, void* const* state, int train, int need_grad, float* out,
                       mi3d_stream_t stream) {
-    if (!h || !x0 || !x1 || !x2 || !state || !out) return MI3D_ERR_ARG;
-    unet::Engine& e = h->e; const int N = e.cfg.N;
+    unet::Engine* ep = plan::engine_of<unet::Engine>(h);
+    if (!ep || !x0 || !x1 || !x2 || !state || !out) return MI3D_ERR_ARG;
+    unet::Engine& e = *ep; const int N = e.cfg.N;
     // batch statistics need more than one value per channel (H/4 x W/4 is the smallest level), as in torch's BatchNorm
     if (train && (size_t)N * e.HW[2] < 2) return MI3D_ERR_ARG;
     cudaStream_t st = (cudaStream_t)stream;
@@ -396,7 +370,7 @@ int mi3d_unet_forward(mi3d_unet_t h, const float* x0, const float* x1, const flo
         if (en.kind == unet::E_COUNT) continue;
         if (!state[i]) { if (en.kind == unet::E_PARAM || !train) return MI3D_ERR_ARG; continue; }
         if (nt == 48) return MI3D_ERR_ARG;
-        cl.src[nt] = (const float*)state[i]; cl.dst[nt] = en.slot; cl.n[nt] = (int)en.numel; nt++;
+        cl.src[nt] = (const float*)state[i]; cl.dst[nt] = en.slot; cl.n[nt] = (int)e.params[i].numel; nt++;
     }
     cl.count = nt;
     unk::k_copy_list<<<dim3(32, nt), 256, 0, st>>>(cl);
@@ -423,9 +397,10 @@ int mi3d_unet_forward(mi3d_unet_t h, const float* x0, const float* x1, const flo
     return MI3D_OK;
 }
 
-int mi3d_unet_backward(mi3d_unet_t h, const float* dout, float* dx0, float* dx1, float* dx2, float* const* grads, mi3d_stream_t stream) {
-    if (!h || !dout || !dx0 || !dx1 || !dx2 || !grads) return MI3D_ERR_ARG;
-    unet::Engine& e = h->e; const int N = e.cfg.N;
+int mi3d_unet_backward(mi3d_engine_t h, const float* dout, float* dx0, float* dx1, float* dx2, float* const* grads, mi3d_stream_t stream) {
+    unet::Engine* ep = plan::engine_of<unet::Engine>(h);
+    if (!ep || !dout || !dx0 || !dx1 || !dx2 || !grads) return MI3D_ERR_ARG;
+    unet::Engine& e = *ep; const int N = e.cfg.N;
     if (!e.tape) return MI3D_ERR_ARG;
     cudaStream_t st = (cudaStream_t)stream;
     const size_t* HW = e.HW;
@@ -439,19 +414,11 @@ int mi3d_unet_backward(mi3d_unet_t h, const float* dout, float* dx0, float* dx1,
         const unet::Entry& en = e.entries[i];
         if (en.kind != unet::E_PARAM || !grads[i]) continue;
         if (nt == 48) return MI3D_ERR_ARG;
-        cl.src[nt] = en.grad; cl.dst[nt] = grads[i]; cl.n[nt] = (int)en.numel; nt++;
+        cl.src[nt] = en.grad; cl.dst[nt] = grads[i]; cl.n[nt] = (int)e.params[i].numel; nt++;
     }
     cl.count = nt;
     if (nt) unk::k_copy_list<<<dim3(32, nt), 256, 0, st>>>(cl);
     return (int)cudaGetLastError();
-}
-
-int mi3d_unet_debug_tensor(mi3d_unet_t h, const char* name, void** ptr, size_t* bytes) {
-    if (!h || !name || !ptr || !bytes) return MI3D_ERR_ARG;
-    auto it = h->e.named.find(name);
-    if (it == h->e.named.end()) return MI3D_ERR_ARG;
-    *ptr = it->second.first; *bytes = it->second.second;
-    return MI3D_OK;
 }
 
 }  // extern "C"

@@ -12,7 +12,6 @@ weight-streaming GEMM for the decoder, the greedy step on the device); there is 
   transformers returns them, so `processor.batch_decode(out, skip_special_tokens=True)` works unchanged.
 * The image processor and the BPE detokenizer stay the caller's (they need the checkpoint's files).
 """
-import contextlib
 import ctypes as C
 import glob
 import json
@@ -65,35 +64,15 @@ def cfg_from_config_json(conf):
                 bos_token_id=get(t, "bos_token_id", 2), eos_token_id=get(t, "eos_token_id", d["eos_token_id"]))
 
 
-class Blip2ForConditionalGeneration:
+class Blip2ForConditionalGeneration(L.Engine):
     def __init__(self, cfg=None, state_dict=None, device="cuda", graph_replay=True):
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise L.Mi3dError("the BLIP-2 captioner runs on sm_90a only; there is no CPU fallback")
         self.cfg = dict(cfg or blip2_opt_27b_cfg())
-        lib = L.lib()
-        lib.mi3d_blip2_workspace_bytes.restype = C.c_size_t
-        lib.mi3d_blip2_create.restype = C.c_void_p
-        lib.mi3d_blip2_param_name.restype = C.c_char_p
         self.struct = Blip2Cfg(*(int(self.cfg[k]) for k, _ in Blip2Cfg._fields_))
-        nbytes = lib.mi3d_blip2_workspace_bytes(C.byref(self.struct))
-        if nbytes == 0:
-            raise L.Mi3dError(f"unsupported BLIP-2 configuration {self.cfg}")
-        self.workspace_bytes = nbytes
-        self.workspace = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
-        h = lib.mi3d_blip2_create(C.byref(self.struct), L.ptr(self.workspace), C.c_size_t(nbytes))
-        if not h:
-            raise L.Mi3dError("mi3d_blip2_create failed (TMA descriptor encoding error)")
-        self.h = C.c_void_p(h)
-        self.names, self.shapes = [], []
-        shp = (C.c_int * 4)()
-        for i in range(lib.mi3d_blip2_num_params(self.h)):
-            self.names.append(lib.mi3d_blip2_param_name(self.h, C.c_int(i)).decode())
-            r = lib.mi3d_blip2_param_shape(self.h, C.c_int(i), shp)
-            self.shapes.append(tuple(shp[k] for k in range(r)))
-        # as in the other engines: an engine-owned stream so the launch lists can replay as CUDA graphs
-        self.stream = torch.cuda.Stream(self.device) if graph_replay else None
-        L.check(lib.mi3d_blip2_set_graph_replay(self.h, C.c_int(1 if graph_replay else 0)), "blip2_set_graph_replay")
+        super().__init__("blip2", (C.byref(self.struct),), self.device, graph_replay, f"BLIP-2 configuration {self.cfg}")
+        self.workspace_bytes = self.nbytes
         self.load_state_dict(state_dict if state_dict is not None else _default_state(self.names, self.shapes, self.device))
 
     # ------------------------------------------------------------------ loading
@@ -121,43 +100,17 @@ class Blip2ForConditionalGeneration:
     def load_state_dict(self, state_dict):
         tied = "language_model.lm_head.weight"
         emb = "language_model.model.decoder.embed_tokens.weight"
-        missing = [n for n in self.names if n not in state_dict]
-        unexpected = [k for k in state_dict if k not in self.names and k != tied]
-        if missing or unexpected:
-            raise L.Mi3dError(f"BLIP-2 state_dict mismatch: missing {missing[:4]}, unexpected {unexpected[:4]}")
-        if tied in state_dict:
+        if tied in state_dict and emb in state_dict:
             a, b = state_dict[tied], state_dict[emb]
             if a.shape != b.shape or not torch.equal(a.detach().to(b.device, b.dtype), b.detach()):
                 raise L.Mi3dError(f"{tied} must equal {emb} (lm_head is tied to the token embedding)")
-        lib = L.lib()
-        for i, (name, shape) in enumerate(zip(self.names, self.shapes)):
-            t = state_dict[name].detach()
-            if tuple(t.shape) != shape:
-                raise L.Mi3dError(f"{name}: shape {tuple(t.shape)}, expected {shape}")
-            src = t.to(self.device, torch.float32).contiguous()
-            L.check(lib.mi3d_blip2_load_param(self.h, C.c_int(i), L.ptr(src), L.stream()), f"blip2_load_param({name})")
-        torch.cuda.synchronize(self.device)
-        return self
+        return self.load_strict(state_dict, lambda k: k == tied)
 
     def to(self, *args, **kwargs):
         return self
 
     def eval(self):
         return self
-
-    def graph_replays(self):
-        return int(L.lib().mi3d_blip2_graph_replays(self.h))
-
-    @contextlib.contextmanager
-    def on_stream(self):
-        if self.stream is None:
-            yield
-            return
-        cur = torch.cuda.current_stream()
-        self.stream.wait_stream(cur)
-        with torch.cuda.stream(self.stream):
-            yield
-        cur.wait_stream(self.stream)
 
     # ------------------------------------------------------------------ running
     def _pixels(self, pixel_values):
@@ -226,13 +179,6 @@ class Blip2ForConditionalGeneration:
                                                 L.ptr(logits), L.stream()), "blip2_generate")
         out = ids[: int(count.item())][None].clone()
         return (out, logits) if return_logits else out
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                L.lib().mi3d_blip2_destroy(self.h)
-        except Exception:
-            pass
 
 
 def _default_state(names, shapes, device, seed=0):

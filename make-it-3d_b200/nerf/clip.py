@@ -13,7 +13,6 @@ fused memory-bound kernels); there is no CPU or eager-PyTorch fallback.
   backward runs once, for `rgb` only; the reference encodes `rgb` twice, which gives the same values and, by linearity, the same
   gradient.  No gradient flows to `ref_rgb`.  Normalisation, dot products and the mean stay in torch on the `[B,embed_dim]` features.
 """
-import contextlib
 import ctypes as C
 import math
 
@@ -42,56 +41,13 @@ def _cfg_struct(cfg, max_batch):
     return s
 
 
-class ClipEngine:
-    """Owns the device workspace and the planned launch lists (mi3d_clip_create)."""
+class ClipEngine(L.Engine):
+    """The CLIP engine (mi3d_clip_create): image and text towers planned in one workspace."""
 
     def __init__(self, cfg, device, graph_replay=True, max_batch=2):
-        lib = L.lib()
-        lib.mi3d_clip_workspace_bytes.restype = C.c_size_t
-        lib.mi3d_clip_create.restype = C.c_void_p
-        lib.mi3d_clip_param_name.restype = C.c_char_p
         self.cfg = _cfg_struct(cfg, max_batch)
-        nbytes = lib.mi3d_clip_workspace_bytes(C.byref(self.cfg))
-        if nbytes == 0:
-            raise L.Mi3dError(f"unsupported CLIP configuration {cfg}")
-        self.workspace = torch.zeros(nbytes, dtype=torch.uint8, device=device)
-        h = lib.mi3d_clip_create(C.byref(self.cfg), L.ptr(self.workspace), C.c_size_t(nbytes))
-        if not h:
-            raise L.Mi3dError("mi3d_clip_create failed (TMA descriptor encoding error)")
-        self.h = C.c_void_p(h)
-        self.names, self.shapes = [], []
-        shp = (C.c_int * 4)()
-        for i in range(lib.mi3d_clip_num_params(self.h)):
-            self.names.append(lib.mi3d_clip_param_name(self.h, C.c_int(i)).decode())
-            r = lib.mi3d_clip_param_shape(self.h, C.c_int(i), shp)
-            self.shapes.append(tuple(shp[k] for k in range(r)))
-        # like SDEngine: the lists run on an engine-owned stream so that they can replay as CUDA graphs (torch's legacy default
-        # stream cannot be captured); graph_replay=False keeps plain launches on the caller's stream
-        self.stream = torch.cuda.Stream(device) if graph_replay else None
-        L.check(lib.mi3d_clip_set_graph_replay(self.h, C.c_int(1 if graph_replay else 0)), "clip_set_graph_replay")
+        super().__init__("clip", (C.byref(self.cfg),), device, graph_replay, f"CLIP configuration {cfg}")
         self.tape_id = 0          # bumped by every image forward: each one replaces the engine's tape
-
-    def graph_replays(self):
-        return int(L.lib().mi3d_clip_graph_replays(self.h))
-
-    @contextlib.contextmanager
-    def on_stream(self):
-        if self.stream is None:
-            yield
-            return
-        cur = torch.cuda.current_stream()
-        self.stream.wait_stream(cur)
-        with torch.cuda.stream(self.stream):
-            yield
-        cur.wait_stream(self.stream)
-
-    def load(self, tensors):
-        """tensors: name -> fp32 CUDA tensor named and laid out like openai CLIP's state_dict()"""
-        lib = L.lib()
-        for i, name in enumerate(self.names):
-            src = L.f32c(tensors[name.split("#")[0]])
-            L.check(lib.mi3d_clip_load_param(self.h, C.c_int(i), L.ptr(src), L.stream()), f"clip_load_param({name})")
-        torch.cuda.synchronize()
 
     def encode_image(self, img, aug, need_grad):
         img = L.f32c(img)
@@ -124,13 +80,6 @@ class ClipEngine:
             L.check(L.lib().mi3d_clip_encode_text(self.h, L.ptr(tokens), C.c_int(tokens.shape[0]), L.ptr(feats), L.stream()),
                     "clip_encode_text")
         return feats
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                L.lib().mi3d_clip_destroy(self.h)
-        except Exception:
-            pass
 
 
 class _EncodeImage(torch.autograd.Function):

@@ -10,7 +10,6 @@ GEMM, fp16 storage, fp32 accumulation), then the contextual loss in fp32.  `forw
 backward for `x` only (the weights are frozen and `y` must not require a gradient, as the reference's `gt_rgb`).  One engine is planned
 per (N, H, W) on first use and cached.  There is no CPU or eager-PyTorch fallback.
 """
-import contextlib
 import ctypes as C
 import math
 
@@ -44,52 +43,13 @@ class CxCfg(C.Structure):
     _fields_ = [("N", C.c_int), ("H", C.c_int), ("W", C.c_int)]
 
 
-class CxEngine:
-    """Owns the device workspace and the planned launch lists of one (N, H, W) (mi3d_cx_create)."""
+class CxEngine(L.Engine):
+    """The contextual-loss engine of one (N, H, W) (mi3d_cx_create).  Debug tap "relu5_4": fp16 NHWC [2N,H/16,W/16,512]."""
 
     def __init__(self, N, H, W, device, graph_replay=True):
-        lib = L.lib()
-        lib.mi3d_cx_workspace_bytes.restype = C.c_size_t
-        lib.mi3d_cx_create.restype = C.c_void_p
-        lib.mi3d_cx_param_name.restype = C.c_char_p
         self.cfg = CxCfg(N, H, W)
-        nbytes = lib.mi3d_cx_workspace_bytes(C.byref(self.cfg))
-        if nbytes == 0:
-            raise L.Mi3dError(f"unsupported contextual-loss shape N={N} H={H} W={W}")
-        self.workspace = torch.zeros(nbytes, dtype=torch.uint8, device=device)
-        h = lib.mi3d_cx_create(C.byref(self.cfg), L.ptr(self.workspace), C.c_size_t(nbytes))
-        if not h:
-            raise L.Mi3dError("mi3d_cx_create failed (TMA descriptor encoding error)")
-        self.h = C.c_void_p(h)
-        self.names = [lib.mi3d_cx_param_name(self.h, C.c_int(i)).decode() for i in range(lib.mi3d_cx_num_params(self.h))]
-        # as in ClipEngine: an engine-owned stream, so the lists can replay as CUDA graphs (the legacy default stream cannot be captured)
-        self.stream = torch.cuda.Stream(device) if graph_replay else None
-        L.check(lib.mi3d_cx_set_graph_replay(self.h, C.c_int(1 if graph_replay else 0)), "cx_set_graph_replay")
+        super().__init__("cx", (C.byref(self.cfg),), device, graph_replay, f"contextual-loss shape N={N} H={H} W={W}")
         self.tape_id = 0          # bumped by every forward: each one replaces the engine's tape
-
-    def graph_replays(self):
-        return int(L.lib().mi3d_cx_graph_replays(self.h))
-
-    @contextlib.contextmanager
-    def on_stream(self):
-        if self.stream is None:
-            yield
-            return
-        cur = torch.cuda.current_stream()
-        self.stream.wait_stream(cur)
-        with torch.cuda.stream(self.stream):
-            yield
-        cur.wait_stream(self.stream)
-
-    def load(self, tensors):
-        """tensors: package state_dict name -> fp32 CUDA tensor"""
-        lib = L.lib()
-        for i, name in enumerate(self.names):
-            if "#" in name:
-                continue          # derived copies are written with their base tensor
-            src = L.f32c(tensors[name])
-            L.check(lib.mi3d_cx_load_param(self.h, C.c_int(i), L.ptr(src), L.stream()), f"cx_load_param({name})")
-        torch.cuda.synchronize()
 
     def forward(self, x, y, band_width, need_grad):
         loss = torch.empty((), dtype=torch.float32, device=x.device)
@@ -105,20 +65,6 @@ class CxEngine:
         with self.on_stream():
             L.check(L.lib().mi3d_cx_backward(self.h, L.ptr(dloss), L.ptr(dx), L.stream()), "cx_backward")
         return dx
-
-    def debug_tensor(self, name, dtype=torch.float16):
-        """a named intermediate, as a view of the workspace ("relu5_4": fp16 NHWC [2N,H/16,W/16,512])"""
-        p, n = C.c_void_p(), C.c_size_t()
-        L.check(L.lib().mi3d_cx_debug_tensor(self.h, name.encode(), C.byref(p), C.byref(n)), f"cx_debug_tensor({name})")
-        off = p.value - self.workspace.data_ptr()
-        return self.workspace[off:off + n.value].view(dtype)
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                L.lib().mi3d_cx_destroy(self.h)
-        except Exception:
-            pass
 
 
 class _CxLoss(torch.autograd.Function):

@@ -21,7 +21,7 @@ from .. import _lib as L
 IGNORED_PREFIXES = ("pretrained.model.norm.", "pretrained.model.head.", "scratch.refinenet4.resConfUnit1.")
 
 
-class DPTDepthModel:
+class DPTDepthModel(L.Engine):
     def __init__(self, path=None, non_negative=True, backbone="vitb_rn50_384", enable_attention_hooks=False, state_dict=None,
                  device="cuda"):
         if backbone != "vitb_rn50_384":
@@ -33,22 +33,7 @@ class DPTDepthModel:
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise L.Mi3dError("the DPT engine runs on sm_90a only; there is no CPU fallback")
-        lib = L.lib()
-        lib.mi3d_dpt_workspace_bytes.restype = C.c_size_t
-        lib.mi3d_dpt_create.restype = C.c_void_p
-        lib.mi3d_dpt_param_name.restype = C.c_char_p
-        nbytes = lib.mi3d_dpt_workspace_bytes()
-        self.workspace = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)     # zero: padding rows / channels are never written
-        h = lib.mi3d_dpt_create(L.ptr(self.workspace), C.c_size_t(nbytes))
-        if not h:
-            raise L.Mi3dError("mi3d_dpt_create failed (TMA descriptor encoding error)")
-        self.h = C.c_void_p(h)
-        self.names, self.shapes = [], []
-        shp = (C.c_int * 4)()
-        for i in range(lib.mi3d_dpt_num_params(self.h)):
-            self.names.append(lib.mi3d_dpt_param_name(self.h, C.c_int(i)).decode())
-            r = lib.mi3d_dpt_param_shape(self.h, C.c_int(i), shp)
-            self.shapes.append(tuple(shp[k] for k in range(r)))
+        super().__init__("dpt", (), self.device, False, "DPT configuration")       # one eager forward per image: no graph replay
         if path is not None:
             state_dict = torch.load(path, map_location="cpu")
             if "optimizer" in state_dict:
@@ -66,21 +51,7 @@ class DPTDepthModel:
     def load_state_dict(self, state_dict):
         """the reference's DPTDepthModel.state_dict() names: every tensor the forward reads is required; of the others only
         pretrained.model.norm.*, pretrained.model.head.* and scratch.refinenet4.resConfUnit1.* are accepted (and ignored)"""
-        missing = [n for n in self.names if n not in state_dict]
-        known = set(self.names)
-        unexpected = [k for k in state_dict if k not in known and not k.startswith(IGNORED_PREFIXES)]
-        if missing or unexpected:
-            raise L.Mi3dError(f"DPT state_dict mismatch: missing {missing[:4]}, unexpected {unexpected[:4]}")
-        lib = L.lib()
-        for i, (name, shape) in enumerate(zip(self.names, self.shapes)):
-            t = state_dict[name].detach()
-            if tuple(t.shape) != shape:
-                raise L.Mi3dError(f"{name}: shape {tuple(t.shape)}, expected {shape}")
-            src = t.to(self.device, torch.float32).contiguous()
-            # the caching allocator reuses src's memory only after the load kernel queued behind it on this stream
-            L.check(lib.mi3d_dpt_load_param(self.h, C.c_int(i), L.ptr(src), L.stream()), f"dpt_load_param({name})")
-        torch.cuda.synchronize(self.device)
-        return self
+        return self.load_strict(state_dict, lambda k: k.startswith(IGNORED_PREFIXES))
 
     def forward(self, x):
         """x CUDA fp32 [1, 3, 384, 384] -> inverse depth fp32 [1, 384, 384]"""
@@ -105,13 +76,6 @@ class DPTDepthModel:
             L.check(L.lib().mi3d_dpt_tap(self.h, C.c_int(i), L.ptr(t), L.stream()), "dpt_tap")
             out.append(t)
         return out
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                L.lib().mi3d_dpt_destroy(self.h)
-        except Exception:
-            pass
 
 
 def _default_state(names, shapes, seed=0):

@@ -45,7 +45,6 @@ def _check(points, feats, image_size, acc="alphacomposite"):
 
 def _forward(points, feats, k, rt, H, W, S, radius, ppp, want_image, want_extra):
     lib = L.lib()
-    lib.mi3d_points_workspace_bytes.restype = C.c_size_t
     P = points.shape[0]
     Cn = feats.shape[1] if feats is not None else 1
     nbytes = lib.mi3d_points_workspace_bytes(C.c_uint32(P), C.c_uint32(S), C.c_uint32(S), C.c_double(radius))

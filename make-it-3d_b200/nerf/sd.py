@@ -16,7 +16,6 @@ A native `nerf.clip.CLIP` computes them on the CLIP engine (csrc/clip_engine.cu,
 `load_diffusers_state_dict(text_encoder_state=...)`; prompts given as strings go through the `tokenizer` passed to the constructor.
 Without text-encoder weights it returns a deterministic stand-in keyed by the prompt strings.
 """
-import contextlib
 import ctypes as C
 import hashlib
 import math
@@ -78,81 +77,21 @@ def alphas_cumprod(num_train_timesteps=1000, beta_start=0.00085, beta_end=0.012)
     return torch.cumprod(1.0 - betas, dim=0)
 
 
-class SDEngine:
-    """Owns the device workspace and the planned launch lists (mi3d_sd_create)."""
+class SDEngine(L.Engine):
+    """The SD engine (mi3d_sd_create): U-Net and VAE launch lists planned in one workspace."""
 
     def __init__(self, unet_cfg, vae_cfg, device, graph_replay=True):
-        lib = L.lib()
-        lib.mi3d_sd_workspace_bytes.restype = C.c_size_t
-        lib.mi3d_sd_create.restype = C.c_void_p
-        lib.mi3d_sd_param_name.restype = C.c_char_p
-        lib.mi3d_sd_param_numel.restype = C.c_longlong
         self.u = _unet_struct(unet_cfg) if unet_cfg else None
         self.v = _vae_struct(vae_cfg) if vae_cfg else None
-        up = C.byref(self.u) if self.u else None
-        vp = C.byref(self.v) if self.v else None
-        nbytes = lib.mi3d_sd_workspace_bytes(up, vp)
-        self.workspace = torch.empty(nbytes, dtype=torch.uint8, device=device)
-        self.workspace.zero_()
-        self.h = lib.mi3d_sd_create(up, vp, L.ptr(self.workspace), C.c_size_t(nbytes))
-        if not self.h:
-            raise L.Mi3dError("mi3d_sd_create failed (unsupported configuration or TMA descriptor encoding error)")
-        self.h = C.c_void_p(self.h)
-        self.names, self.shapes = [], []
-        shp = (C.c_int * 4)()
-        for i in range(lib.mi3d_sd_num_params(self.h)):
-            self.names.append(lib.mi3d_sd_param_name(self.h, C.c_int(i)).decode())
-            r = lib.mi3d_sd_param_shape(self.h, C.c_int(i), shp)
-            self.shapes.append(tuple(shp[k] for k in range(r)))
-        self.nbytes = nbytes
-        # The launch lists run on the engine's own stream (event-ordered against the caller's, see on_stream) and replay as CUDA
-        # graphs from their third call on: torch's default stream is the legacy stream, which CUDA cannot capture.
-        # graph_replay=False keeps plain launches on the caller's stream (used by the parity tests as the A/B arm).
-        self.stream = torch.cuda.Stream(device) if graph_replay else None
-        L.check(lib.mi3d_sd_set_graph_replay(self.h, C.c_int(1 if graph_replay else 0)), "sd_set_graph_replay")
+        # graph_replay=False keeps plain launches on the caller's stream (used by the parity tests as the A/B arm)
+        super().__init__("sd", (C.byref(self.u) if self.u else None, C.byref(self.v) if self.v else None), device, graph_replay,
+                         f"SD configuration unet={unet_cfg} vae={vae_cfg}")
 
-    def graph_replays(self):
-        """number of launch lists currently instantiated as CUDA graphs (0..3)"""
-        return int(L.lib().mi3d_sd_graph_replays(self.h))
-
-    @contextlib.contextmanager
-    def on_stream(self):
-        """Engine calls inside run on self.stream, ordered after the caller's pending work; the caller's stream then waits for them."""
-        if self.stream is None:
-            yield
-            return
-        cur = torch.cuda.current_stream()
-        self.stream.wait_stream(cur)
-        with torch.cuda.stream(self.stream):
-            yield
-        cur.wait_stream(self.stream)
-
-    def load(self, tensors):
-        """tensors: name -> fp32 CUDA tensor in diffusers layout (VAE names as in AutoencoderKL.state_dict())."""
-        lib = L.lib()
-        for i, name in enumerate(self.names):
-            base = name.split("#")[0]
-            if base not in tensors:
-                raise L.Mi3dError(f"missing SD parameter {base}")
-            src = L.f32c(tensors[base])
-            partner = None
-            if name.endswith("ff.net.0.proj.weight"):
-                partner = L.f32c(tensors[name[:-len("weight")] + "bias"])
-            L.check(lib.mi3d_sd_load_param(self.h, C.c_int(i), L.ptr(src), L.ptr(partner), L.stream()), f"sd_load_param({name})")
-        torch.cuda.synchronize()
-
-    def debug_tensor(self, name, dtype=torch.float16):
-        p, n = C.c_void_p(), C.c_size_t()
-        L.check(L.lib().mi3d_sd_debug_tensor(self.h, name.encode(), C.byref(p), C.byref(n)), "sd_debug_tensor")
-        off = p.value - self.workspace.data_ptr()
-        return self.workspace[off:off + n.value].view(dtype)
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                L.lib().mi3d_sd_destroy(self.h)
-        except Exception:
-            pass
+    def partner(self, name, tensors):
+        """the GEGLU proj weight is written together with its bias"""
+        if not name.endswith("ff.net.0.proj.weight"):
+            return None
+        return tensors[name[:-len("weight")] + "bias"]
 
 
 def _default_init(name, shape, gen):

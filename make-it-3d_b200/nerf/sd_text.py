@@ -12,7 +12,6 @@ fused memory-bound kernels); there is no CPU or eager-PyTorch fallback.
 * `encoder(input_ids)` -> `(last_hidden_state,)`: int64 CUDA ids `[B, 77]` -> fp32 `[B, 77, 1024]`, no gradient (the encoder is frozen),
   so the reference's `self.text_encoder(ids)[0]` works unchanged.
 """
-import contextlib
 import ctypes as C
 
 import torch
@@ -38,72 +37,25 @@ def cfg_from_state_dict(state_dict):
                 context_len=state_dict["text_model.embeddings.position_embedding.weight"].shape[0], vocab=tok.shape[0])
 
 
-class TextEncoder:
+class TextEncoder(L.Engine):
     def __init__(self, device, cfg=None, state_dict=None, graph_replay=True, max_batch=2):
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise L.Mi3dError("the SD-2 text encoder runs on sm_90a only; there is no CPU fallback")
         self.cfg = dict(cfg or sd2_text_cfg())
-        lib = L.lib()
-        lib.mi3d_sd_text_workspace_bytes.restype = C.c_size_t
-        lib.mi3d_sd_text_create.restype = C.c_void_p
-        lib.mi3d_sd_text_param_name.restype = C.c_char_p
         self.struct = SdTextCfg(*(int(self.cfg[k]) for k, _ in SdTextCfg._fields_[:-1]), int(max_batch))
-        nbytes = lib.mi3d_sd_text_workspace_bytes(C.byref(self.struct))
-        if nbytes == 0:
-            raise L.Mi3dError(f"unsupported SD text encoder configuration {self.cfg} with max_batch={max_batch}")
-        self.workspace = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
-        h = lib.mi3d_sd_text_create(C.byref(self.struct), L.ptr(self.workspace), C.c_size_t(nbytes))
-        if not h:
-            raise L.Mi3dError("mi3d_sd_text_create failed (TMA descriptor encoding error)")
-        self.h = C.c_void_p(h)
-        self.names, self.shapes = [], []
-        shp = (C.c_int * 4)()
-        for i in range(lib.mi3d_sd_text_num_params(self.h)):
-            self.names.append(lib.mi3d_sd_text_param_name(self.h, C.c_int(i)).decode())
-            r = lib.mi3d_sd_text_param_shape(self.h, C.c_int(i), shp)
-            self.shapes.append(tuple(shp[k] for k in range(r)))
-        # as in the other engines: the launch list runs on an engine-owned stream so that it can replay as a CUDA graph (torch's legacy
-        # default stream cannot be captured); graph_replay=False keeps plain launches on the caller's stream
-        self.stream = torch.cuda.Stream(self.device) if graph_replay else None
-        L.check(lib.mi3d_sd_text_set_graph_replay(self.h, C.c_int(1 if graph_replay else 0)), "sd_text_set_graph_replay")
+        super().__init__("sd_text", (C.byref(self.struct),), self.device, graph_replay,
+                         f"SD text encoder configuration {self.cfg} with max_batch={max_batch}")
         self.load_state_dict(state_dict if state_dict is not None else _default_state(self.names, self.shapes))
 
     @property
     def max_batch(self):
         return self.struct.max_batch
 
-    def graph_replays(self):
-        return int(L.lib().mi3d_sd_text_graph_replays(self.h))
-
-    @contextlib.contextmanager
-    def on_stream(self):
-        if self.stream is None:
-            yield
-            return
-        cur = torch.cuda.current_stream()
-        self.stream.wait_stream(cur)
-        with torch.cuda.stream(self.stream):
-            yield
-        cur.wait_stream(self.stream)
-
     def load_state_dict(self, state_dict):
         """tensors named like transformers' CLIPTextModel.state_dict() (any float dtype, any device); every entry is required, and no
         other entry but `text_model.embeddings.position_ids` is accepted"""
-        missing = [n for n in self.names if n not in state_dict]
-        unexpected = [k for k in state_dict if k not in self.names and not k.endswith("position_ids")]
-        if missing or unexpected:
-            raise L.Mi3dError(f"SD text encoder state_dict mismatch: missing {missing[:4]}, unexpected {unexpected[:4]}")
-        lib = L.lib()
-        for i, (name, shape) in enumerate(zip(self.names, self.shapes)):
-            t = state_dict[name].detach()
-            if tuple(t.shape) != shape:
-                raise L.Mi3dError(f"{name}: shape {tuple(t.shape)}, expected {shape}")
-            src = t.to(self.device, torch.float32).contiguous()
-            # the caching allocator reuses src's memory only after the load kernel queued behind it on this stream
-            L.check(lib.mi3d_sd_text_load_param(self.h, C.c_int(i), L.ptr(src), L.stream()), f"sd_text_load_param({name})")
-        torch.cuda.synchronize(self.device)
-        return self
+        return self.load_strict(state_dict, lambda k: k.endswith("position_ids"))
 
     def __call__(self, input_ids):
         """input_ids int64 CUDA [B, context_len] -> (last_hidden_state fp32 [B, context_len, width],)"""
@@ -121,13 +73,6 @@ class TextEncoder:
         with self.on_stream():
             L.check(L.lib().mi3d_sd_text_encode(self.h, L.ptr(ids), C.c_int(B), L.ptr(out), L.stream()), "sd_text_encode")
         return (out,)
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                L.lib().mi3d_sd_text_destroy(self.h)
-        except Exception:
-            pass
 
 
 def _default_state(names, shapes, seed=0):

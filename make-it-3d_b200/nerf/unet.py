@@ -11,7 +11,6 @@ call.  `.train()` uses batch statistics and updates the running statistics once 
 The backward may run more than once per forward (`retain_graph=True`).  One engine is planned per (N, H, W) on first use and cached.
 Only the refine configuration is built, and there is no CPU or eager-PyTorch fallback.
 """
-import contextlib
 import ctypes as C
 
 import torch
@@ -24,42 +23,16 @@ class UNetCfg(C.Structure):
     _fields_ = [("N", C.c_int), ("H", C.c_int), ("W", C.c_int)]
 
 
-class UNetEngine:
-    """Owns the device workspace and the planned launch lists of one (N, H, W) (mi3d_unet_create)."""
+class UNetEngine(L.Engine):
+    """The U-Net engine of one (N, H, W) (mi3d_unet_create).  Its registry names the module's state_dict entries; their values are
+    passed to every call, not loaded.  Debug taps are fp32 NCHW."""
+
+    debug_dtype = torch.float32
 
     def __init__(self, N, H, W, device, graph_replay=True):
-        lib = L.lib()
-        lib.mi3d_unet_workspace_bytes.restype = C.c_size_t
-        lib.mi3d_unet_create.restype = C.c_void_p
-        lib.mi3d_unet_param_name.restype = C.c_char_p
         self.cfg = UNetCfg(N, H, W)
-        nbytes = lib.mi3d_unet_workspace_bytes(C.byref(self.cfg))
-        if nbytes == 0:
-            raise L.Mi3dError(f"unsupported U-Net shape N={N} H={H} W={W}")
-        self.workspace = torch.empty(nbytes, dtype=torch.uint8, device=device)
-        h = lib.mi3d_unet_create(C.byref(self.cfg), L.ptr(self.workspace), C.c_size_t(nbytes))
-        if not h:
-            raise L.Mi3dError("mi3d_unet_create failed")
-        self.h = C.c_void_p(h)
-        self.names = [lib.mi3d_unet_param_name(self.h, C.c_int(i)).decode() for i in range(lib.mi3d_unet_num_params(self.h))]
-        # an engine-owned stream, so the lists can replay as CUDA graphs (the legacy default stream cannot be captured)
-        self.stream = torch.cuda.Stream(device) if graph_replay else None
-        L.check(lib.mi3d_unet_set_graph_replay(self.h, C.c_int(1 if graph_replay else 0)), "unet_set_graph_replay")
+        super().__init__("unet", (C.byref(self.cfg),), device, graph_replay, f"U-Net shape N={N} H={H} W={W}")
         self.tape_id = 0          # bumped by every forward: each one replaces the engine's tape
-
-    def graph_replays(self):
-        return int(L.lib().mi3d_unet_graph_replays(self.h))
-
-    @contextlib.contextmanager
-    def on_stream(self):
-        if self.stream is None:
-            yield
-            return
-        cur = torch.cuda.current_stream()
-        self.stream.wait_stream(cur)
-        with torch.cuda.stream(self.stream):
-            yield
-        cur.wait_stream(self.stream)
 
     def forward(self, xs, state, train, need_grad):
         """state: registry name -> CUDA tensor (or None: a running statistic not to update)"""
@@ -82,20 +55,6 @@ class UNetEngine:
             L.check(L.lib().mi3d_unet_backward(self.h, L.ptr(dout), L.ptr(dxs[0]), L.ptr(dxs[1]), L.ptr(dxs[2]), ptrs, L.stream()),
                     "unet_backward")
         return dxs, grads
-
-    def debug_tensor(self, name):
-        """a named fp32 intermediate, as a view of the workspace"""
-        p, n = C.c_void_p(), C.c_size_t()
-        L.check(L.lib().mi3d_unet_debug_tensor(self.h, name.encode(), C.byref(p), C.byref(n)), f"unet_debug_tensor({name})")
-        off = p.value - self.workspace.data_ptr()
-        return self.workspace[off:off + n.value].view(torch.float32)
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                L.lib().mi3d_unet_destroy(self.h)
-        except Exception:
-            pass
 
 
 class _UNetFn(torch.autograd.Function):

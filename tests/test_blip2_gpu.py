@@ -128,16 +128,16 @@ def test_early_stop_at_eos_reduced_config():
     assert out.shape == (1, 33 + k + 1) and int(out[0, -1]) == gen[k]
 
 
-def test_bit_identical_across_calls_and_graph_replay(setup):
+def test_bit_identical_across_calls_and_with_engine_graph_replay_off(setup):
     b2, _, _, model, px, ref, _ = setup
     _, L = _mods()
     runs = [model.generate(pixel_values=px, max_new_tokens=N_NEW, eos_token_id=-1, return_logits=True) for _ in range(3)]
     assert model.graph_replays() >= 1
-    L.check(L.lib().mi3d_blip2_set_graph_replay(model.h, 0), "set_graph_replay")
+    L.check(L.lib().mi3d_engine_set_graph_replay(model.h, 0), "set_graph_replay")
     try:
         runs.append(model.generate(pixel_values=px, max_new_tokens=N_NEW, eos_token_id=-1, return_logits=True))
     finally:
-        L.check(L.lib().mi3d_blip2_set_graph_replay(model.h, 1), "set_graph_replay")
+        L.check(L.lib().mi3d_engine_set_graph_replay(model.h, 1), "set_graph_replay")
     for ids, lg in runs[1:]:
         assert torch.equal(ids, runs[0][0]) and torch.equal(lg, runs[0][1])
 
