@@ -150,13 +150,6 @@ typedef struct { const float *w1, *b1, *w2, *b2, *w3, *b3; } mi3d_mlp;
 typedef struct { float *w1, *b1, *w2, *b2, *w3, *b3; } mi3d_mlp_grad;
 
 enum { MI3D_SHADING_ALBEDO = 0, MI3D_SHADING_LAMBERTIAN = 1, MI3D_SHADING_TEXTURELESS = 2, MI3D_SHADING_NORMAL = 3 };
-/* kernel family of the fused field (the names are historical).  TCGEN05 (default): wgmma split-precision tiles; the backward chain kernel issues the
- * table-gradient REDs itself (LSU-bound RED stream under the latency-bound MMA chain; = _FUSED_SCATTER).  _SPLIT_SCATTER: the
- * round-1 pipeline with a separate full-occupancy scatter kernel (A/B arm).  _SINGLE_E: fused scatter, but the encoding operand of the
- * chain kernel single-buffered (the default alternates consecutive evaluations between the two column halves of its tile; A/B arm).
- * FFMA = the register-tiled fp32 kernels. */
-enum { MI3D_FIELD_IMPL_TCGEN05 = 0, MI3D_FIELD_IMPL_FFMA = 1, MI3D_FIELD_IMPL_TCGEN05_FUSED_SCATTER = 2, MI3D_FIELD_IMPL_TCGEN05_SPLIT_SCATTER = 3,
-       MI3D_FIELD_IMPL_TCGEN05_SINGLE_E = 4 };
 
 typedef struct {
     float bound;          /* opt.bound */
@@ -167,8 +160,6 @@ typedef struct {
     int shading;          /* MI3D_SHADING_* (network_tcnn.py:146-170) */
     float ambient_ratio;
     const float* light_d; /* device [3] (multi-view batches: [n_views][3]), needed unless shading == albedo */
-    int impl;             /* MI3D_FIELD_IMPL_* (explicit: the library reads no environment variables) */
-    float scatter_agg_scale; /* tuning knob of the fused scatter: REDs of hash-grid levels with scale below this are warp-aggregated; 0 = library default (100) */
 } mi3d_field_cfg;
 
 /* Multi-view batches (several camera views' rays in one march: ray-parallel multi-GPU render, or several views per GPU).
@@ -203,7 +194,7 @@ typedef struct {
     uint32_t enc_cache_valid;
     /* multi-view batch: DEVICE table (NULL = one view: counter / m_fixed / align above describe the rows) and its view count.
      * With segs, loss_orient / loss_smooth / grad_loss_* are [n_views] arrays and loss_partials holds
-     * 2 * n_views * mi3d_field_grid_ctas(0) floats.  Tensor-core kernels only. */
+     * 2 * n_views * mi3d_field_grid_ctas(0) floats. */
     const mi3d_view_segs* segs;
     uint32_t n_views;
     uint32_t noise_mode;       /* in-kernel smoothness perturbation keyed by 0: (seed, row)  1: (seed, sample position) */
@@ -226,9 +217,9 @@ int mi3d_field_backward(const mi3d_field_io* io, const float* table, const mi3d_
                         const mi3d_field_cfg* cfg, const float* tape, const float* grad_sigmas, const float* grad_rgbs,
                         const float* grad_normals, const float* grad_loss_orient, const float* grad_loss_smooth,
                         float* grad_table, const mi3d_mlp_grad* grad_mlp, void* workspace, mi3d_stream_t stream);
-/* workspace (nullable): mi3d_field_backward_workspace_bytes() bytes of scratch.  When given, the backward runs per chunk of 1 048 576
- * samples: encodings come from io->enc_cache or from a full-occupancy gather kernel into the scratch, then the tensor-core chain kernel
- * runs and issues the table-gradient REDs itself (cfg->impl = _SPLIT_SCATTER: a separate full-occupancy scatter kernel instead).
+/* workspace (nullable): mi3d_field_backward_workspace_bytes() bytes of scratch (one encoding staging buffer, 1.74 GB).  When given,
+ * the backward runs per chunk of 1 048 576 samples: encodings come from io->enc_cache or from a full-occupancy gather kernel into the
+ * scratch, then the tensor-core chain kernel runs and issues the table-gradient REDs itself.
  * When NULL the chain kernel also gathers in-kernel (slower: its eight gather warps are starved); the Python host always passes scratch. */
 size_t mi3d_field_backward_workspace_bytes(void);
 

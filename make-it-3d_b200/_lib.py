@@ -39,7 +39,7 @@ class Epilogue(C.Structure):
 
 class FieldCfg(C.Structure):
     _fields_ = [("bound", C.c_float), ("blob_density", C.c_float), ("blob_radius", C.c_float), ("n_evals", C.c_int),
-                ("shading", C.c_int), ("ambient_ratio", C.c_float), ("light_d", C.c_void_p), ("impl", C.c_int), ("scatter_agg_scale", C.c_float)]
+                ("shading", C.c_int), ("ambient_ratio", C.c_float), ("light_d", C.c_void_p)]
 
 
 class FieldIO(C.Structure):
@@ -88,7 +88,6 @@ class RenderWs(C.Structure):
 RENDER_PHASE_MARCH, RENDER_PHASE_SHADE, RENDER_PHASE_ALL = 1, 2, 3
 
 SHADING = {"albedo": 0, "lambertian": 1, "textureless": 2, "normal": 3}
-FIELD_IMPL = {"tcgen05": 0, "ffma": 1, "tcgen05_fused_scatter": 2, "tcgen05_split_scatter": 3, "tcgen05_single_e": 4}
 
 # every symbol include/mi3d.h declares (tests/test_abi.py checks the .so exports exactly these)
 SYMBOLS = [

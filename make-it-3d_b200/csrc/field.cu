@@ -4,17 +4,16 @@
 // do with 13 separate encoder/MLP passes in the reference:
 //     multires hash-grid gather (tiny-cuda-nn HashGrid, fp32 table)  ->  32-64-64-4 MLP (fp32, bias, ReLU)
 //     -> trunc_exp / sigmoid -> 6-tap finite-difference normal -> shading -> orientation / smoothness terms
-// without ever materialising encodings or activations in HBM.  The backward kernel recomputes the
-// activations tile-by-tile, back-propagates through the MLP, accumulates the weight gradients in registers
-// across the whole persistent CTA, and scatters the table gradient with vector reductions (RED.ADD.v2.f32).
-//
-// Tiling (both kernels): CTA = 256 threads = one tile of T=128 samples.  Activations live in shared memory
-// k-major ([feature][row], row stride TP=132 floats) so that (a) the 32 lanes of a warp read/write 128
-// consecutive rows -> conflict-free LDS.128/STS.128, (b) weights are warp-broadcast LDS.128, (c) the
-// weight-gradient reduction over rows also vectorises along rows without bank conflicts (TP = 4 mod 32).
-// Each thread owns a 4-row x (N/8)-column register tile of every layer GEMM; this is plain fp32 FFMA on
-// purpose: the finite-difference normals difference two densities 0.02 apart, so the MLP needs full fp32
-// (fp16/bf16/tf32 tensor-core inputs would put ~1e-2 relative error on the normals; see DESIGN.md).
+// without materialising activations in HBM.  The finite-difference normals difference two densities 0.02 apart, so the
+// MLP needs fp32-class products (plain fp16 / bf16 / tf32 inputs would put ~1e-2 relative error on the normals; see
+// DESIGN.md): the layer GEMMs run on wgmma over split-precision operands.
+//   k_field_fwd_tc    forward: 3-term tf32 split, one 128-sample tile per CTA at a time (owner / encoder / MMA warps)
+//   k_field_bwd_tc    backward chain: recomputes the activations tile by tile, back-propagates through the MLP (6-term bf16
+//                     split), keeps the weight gradients in registers across the whole persistent CTA and scatters the
+//                     table gradient with vector reductions (RED.ADD.v2 / v4.f32) under the MMA chain
+//   k_bwd_enc_scatter full-occupancy hash-grid gather that feeds the chain kernel its encodings through HBM
+//   k_field_fwd       density only, fp32 FFMA tiles in shared memory: the density-grid refresh (mi3d_density_grid_update)
+// plus the stand-alone hash-grid encoder (k_hashgrid_fwd / k_hashgrid_bwd) and the density-grid kernels (k_grid_*).
 //
 // Grid: persistent, gridDim = SM count (132 on H100 SXM) x resident CTAs; the number of valid rows is read from device memory
 // (counter[0] written by mi3d_march_rays_train), so there is no host synchronisation between march and field.
@@ -229,13 +228,13 @@ __device__ __forceinline__ void gather16(const float* __restrict__ table, const 
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// tile GEMMs over shared memory.  A: [K][TP] (k-major), W: [K][N] row-major, Out: [N][TP].
-// thread -> rows lane*4..+3, columns warp*NC..+NC-1 with NC = N/8.
-// MASK: multiply by (mask[n][row] > 0) (ReLU backward; mask may alias Out).
+// fp32 FFMA layer of k_field_fwd over shared memory: Out = relu(A W + bias).  A: [K][TP] (k-major), W: [K][N] row-major, Out: [N][TP].
+// thread -> rows lane*4..+3, columns warp*NC..+NC-1 with NC = N/8.  Activations are k-major ([feature][row], row stride TP = 132
+// floats = 4 mod 32) so that the 32 lanes of a warp read / write 128 consecutive rows (conflict-free LDS.128 / STS.128) and the
+// weights are warp-broadcast LDS.128.
 // ---------------------------------------------------------------------------------------------------------
-template <int K, int N, bool RELU, bool MASK>
-__device__ __forceinline__ void tile_gemm(const float* __restrict__ A, const float* __restrict__ W, const float* __restrict__ bias,
-                                          float* Out, const float* mask) {
+template <int K, int N>
+__device__ __forceinline__ void tile_gemm(const float* __restrict__ A, const float* __restrict__ W, const float* __restrict__ bias, float* Out) {
     constexpr int NC = N / 8;
     static_assert(NC == 4 || NC == 8, "column tile");
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -243,7 +242,7 @@ __device__ __forceinline__ void tile_gemm(const float* __restrict__ A, const flo
     float acc[NC][4];
     #pragma unroll
     for (int c = 0; c < NC; c++) {
-        const float b = bias ? bias[c0 + c] : 0.f;
+        const float b = bias[c0 + c];
         acc[c][0] = b; acc[c][1] = b; acc[c][2] = b; acc[c][3] = b;
     }
     #pragma unroll 8
@@ -263,12 +262,7 @@ __device__ __forceinline__ void tile_gemm(const float* __restrict__ A, const flo
     }
     #pragma unroll
     for (int c = 0; c < NC; c++) {
-        float4 o = make_float4(acc[c][0], acc[c][1], acc[c][2], acc[c][3]);
-        if (RELU) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-        if (MASK) {
-            const float4 m = *reinterpret_cast<const float4*>(mask + (c0 + c) * TP + r0);
-            o.x = m.x > 0.f ? o.x : 0.f; o.y = m.y > 0.f ? o.y : 0.f; o.z = m.z > 0.f ? o.z : 0.f; o.w = m.w > 0.f ? o.w : 0.f;
-        }
+        const float4 o = make_float4(fmaxf(acc[c][0], 0.f), fmaxf(acc[c][1], 0.f), fmaxf(acc[c][2], 0.f), fmaxf(acc[c][3], 0.f));
         *reinterpret_cast<float4*>(Out + (c0 + c) * TP + r0) = o;
     }
 }
@@ -287,53 +281,16 @@ __device__ __forceinline__ void out_layer(const float* __restrict__ H2, const fl
     O[(2 * pair) * TP + row] = o0; O[(2 * pair + 1) * TP + row] = o1;
 }
 
-// Weight-gradient tile: dW[j][i] += sum_rows P[j][row] * Q[i][row]; thread owns j in {jt + 16a}, i in {it + IT*b}.
-// J = 64 always (16 j-groups x 4); I = 64 (NI=4) or 32 (NI=2).  Also accumulates db[j] on threads with it == 0.
-template <int NI>
-__device__ __forceinline__ void tile_wgrad(const float* __restrict__ P, const float* __restrict__ Q, float (&acc)[4][NI], float (&db)[4]) {
-    const int jt = threadIdx.x >> 4, it = threadIdx.x & 15;
-    #pragma unroll 2
-    for (int s = 0; s < T; s += 4) {
-        float4 p[4], q[NI];
-        #pragma unroll
-        for (int a = 0; a < 4; a++) p[a] = *reinterpret_cast<const float4*>(P + (jt + 16 * a) * TP + s);
-        #pragma unroll
-        for (int b = 0; b < NI; b++) q[b] = *reinterpret_cast<const float4*>(Q + (it + 16 * b) * TP + s);
-        #pragma unroll
-        for (int a = 0; a < 4; a++) {
-            #pragma unroll
-            for (int b = 0; b < NI; b++) {
-                acc[a][b] = fmaf(p[a].x, q[b].x, acc[a][b]); acc[a][b] = fmaf(p[a].y, q[b].y, acc[a][b]);
-                acc[a][b] = fmaf(p[a].z, q[b].z, acc[a][b]); acc[a][b] = fmaf(p[a].w, q[b].w, acc[a][b]);
-            }
-            if (it == 0) db[a] += (p[a].x + p[a].y) + (p[a].z + p[a].w);
-        }
-    }
-}
-
-// dW3[o][i] (4 x 64 = 256 entries, one per thread) and db3 (threads 0..3).
-__device__ __forceinline__ void tile_wgrad3(const float* __restrict__ dO, const float* __restrict__ H2, float& acc, float& db) {
-    const int o = threadIdx.x >> 6, i = threadIdx.x & 63;
-    #pragma unroll 4
-    for (int s = 0; s < T; s += 4) {
-        const float4 p = *reinterpret_cast<const float4*>(dO + o * TP + s);
-        const float4 q = *reinterpret_cast<const float4*>(H2 + i * TP + s);
-        acc = fmaf(p.x, q.x, acc); acc = fmaf(p.y, q.y, acc); acc = fmaf(p.z, q.z, acc); acc = fmaf(p.w, q.w, acc);
-        if (i == 0) db += (p.x + p.y) + (p.z + p.w);
-    }
-}
-
 // ---------------------------------------------------------------------------------------------------------
-// shared bookkeeping
+// shared memory of k_field_fwd
 // ---------------------------------------------------------------------------------------------------------
 struct Smem {
-    float* wt1; float* b1; float* wt2; float* b2; float* w3t; float* b3;   // forward layouts [in][out]
-    float* w1; float* w2; float* w3;                                        // backward layouts [out][in] (bwd kernel only)
+    float* wt1; float* b1; float* wt2; float* b2; float* w3t; float* b3;   // weights as [in][out]
     LevelSm* lv;
     float* enc; float* h1; float* h2; float* o;
 };
 
-__device__ __forceinline__ Smem carve(float* base, bool bwd) {
+__device__ __forceinline__ Smem carve(float* base) {
     Smem s;
     float* p = base;
     s.enc = p; p += D_IN * TP;
@@ -343,30 +300,17 @@ __device__ __forceinline__ Smem carve(float* base, bool bwd) {
     s.wt1 = p; p += D_IN * D_H; s.b1 = p; p += D_H;
     s.wt2 = p; p += D_H * D_H; s.b2 = p; p += D_H;
     s.w3t = p; p += D_H * D_OUT; s.b3 = p; p += D_OUT;
-    if (bwd) { s.w1 = p; p += D_H * D_IN; s.w2 = p; p += D_H * D_H; s.w3 = p; p += D_OUT * D_H; }
-    else { s.w1 = s.w2 = s.w3 = nullptr; }
     s.lv = reinterpret_cast<LevelSm*>(p);
     return s;
 }
 
-constexpr size_t smem_bytes(bool bwd) {
-    return sizeof(float) * ((D_IN + 2 * D_H + D_OUT) * TP + D_IN * D_H + D_H + D_H * D_H + D_H + D_H * D_OUT + D_OUT
-                            + (bwd ? (D_H * D_IN + D_H * D_H + D_OUT * D_H) : 0)) + 16 * sizeof(LevelSm);
-}
+constexpr size_t kFwdSmem = sizeof(float) * ((D_IN + 2 * D_H + D_OUT) * TP + D_IN * D_H + D_H + D_H * D_H + D_H + D_H * D_OUT + D_OUT)
+                            + 16 * sizeof(LevelSm);
 
-__device__ __forceinline__ void load_weights(const Smem& s, const mi3d_mlp& m, const mi3d_hashgrid& hg, bool bwd) {
-    for (int i = threadIdx.x; i < D_H * D_IN; i += NT) {           // W1 [64][32]
-        const int j = i / D_IN, k = i % D_IN; const float v = m.w1[i];
-        s.wt1[k * D_H + j] = v; if (bwd) s.w1[i] = v;
-    }
-    for (int i = threadIdx.x; i < D_H * D_H; i += NT) {            // W2 [64][64]
-        const int j = i / D_H, k = i % D_H; const float v = m.w2[i];
-        s.wt2[k * D_H + j] = v; if (bwd) s.w2[i] = v;
-    }
-    for (int i = threadIdx.x; i < D_OUT * D_H; i += NT) {          // W3 [4][64]
-        const int j = i / D_H, k = i % D_H; const float v = m.w3[i];
-        s.w3t[k * D_OUT + j] = v; if (bwd) s.w3[i] = v;
-    }
+__device__ __forceinline__ void load_weights(const Smem& s, const mi3d_mlp& m, const mi3d_hashgrid& hg) {
+    for (int i = threadIdx.x; i < D_H * D_IN; i += NT) s.wt1[(i % D_IN) * D_H + i / D_IN] = m.w1[i];      // W1 [64][32]
+    for (int i = threadIdx.x; i < D_H * D_H; i += NT) s.wt2[(i % D_H) * D_H + i / D_H] = m.w2[i];         // W2 [64][64]
+    for (int i = threadIdx.x; i < D_OUT * D_H; i += NT) s.w3t[(i % D_H) * D_OUT + i / D_H] = m.w3[i];     // W3 [4][64]
     for (int i = threadIdx.x; i < D_H; i += NT) { s.b1[i] = m.b1[i]; s.b2[i] = m.b2[i]; }
     if (threadIdx.x < D_OUT) s.b3[threadIdx.x] = m.b3[threadIdx.x];
     if (threadIdx.x < 16) {
@@ -513,118 +457,45 @@ struct FwdArgs {
 };
 
 // ---------------------------------------------------------------------------------------------------------
-// forward
+// density only, plain fp32 FFMA: sigmas[row] = trunc_exp(h0(xyzs[row]) + blob) for rows [0, n).  The density-grid refresh evaluates
+// every grid cell with it (mi3d_density_grid_update).
+// CTA = 256 threads = one tile of T = 128 samples; each thread owns a 4-row x (N/8)-column register tile of a layer GEMM.
 // ---------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(NT, 2) k_field_fwd(const FwdArgs a) {
+__global__ void __launch_bounds__(NT, 2) k_field_fwd(const float* __restrict__ xyzs, uint32_t n, const float* __restrict__ table,
+                                                     const mi3d_hashgrid hg, const mi3d_mlp mlp, float bound, float blob_density,
+                                                     float two_r2, float* __restrict__ sigmas) {
     extern __shared__ __align__(16) float smem_raw[];
-    const Smem s = carve(smem_raw, false);
-    load_weights(s, a.mlp, a.hg, false);
-    const uint32_t M = a.counter ? min((uint32_t)a.counter[0], a.cap) : a.m_fixed;
-    const uint32_t m_pad = padded_rows(M, a.align, a.cap);
+    const Smem s = carve(smem_raw);
+    load_weights(s, mlp, hg);
     const int lrow = threadIdx.x & (T - 1), half = threadIdx.x >> 7;
-    const int nl = (int)a.hg.n_levels, l0 = half * (nl / 2), lcount = half ? nl - nl / 2 : nl / 2;
-    const bool lit = a.shading != MI3D_SHADING_ALBEDO && m_pad < 1000000u;   // network_tcnn.py:159 fallback
-    float light[3] = {0.f, 0.f, 0.f};
-    if (a.light_d) { light[0] = a.light_d[0]; light[1] = a.light_d[1]; light[2] = a.light_d[2]; }
-    float acc_orient = 0.f, acc_smooth = 0.f;
+    const int nl = (int)hg.n_levels, l0 = half * (nl / 2), lcount = half ? nl - nl / 2 : nl / 2;
     __syncthreads();
 
-    for (uint32_t tile = blockIdx.x; (uint64_t)tile * T < m_pad; tile += gridDim.x) {
+    for (uint32_t tile = blockIdx.x; (uint64_t)tile * T < n; tile += gridDim.x) {
         const uint32_t row = tile * T + lrow;
-        const bool in_range = row < m_pad, real = row < M;
-        float x[3] = {0.f, 0.f, 0.f}, d[3] = {0.f, 0.f, 0.f}, xp[3] = {0.f, 0.f, 0.f};
-        if (real) {
-            x[0] = a.xyzs[3 * (size_t)row]; x[1] = a.xyzs[3 * (size_t)row + 1]; x[2] = a.xyzs[3 * (size_t)row + 2];
-            if (a.dirs) { d[0] = a.dirs[3 * (size_t)row]; d[1] = a.dirs[3 * (size_t)row + 1]; d[2] = a.dirs[3 * (size_t)row + 2]; }
-        }
-        if (a.n_evals > 7 && in_range) {
-            float z[3];
-            if (a.smooth_noise) { z[0] = a.smooth_noise[3 * (size_t)row]; z[1] = a.smooth_noise[3 * (size_t)row + 1]; z[2] = a.smooth_noise[3 * (size_t)row + 2]; }
-            else gauss_pair(a.seed, row, 1u, z);
-            #pragma unroll
-            for (int c = 0; c < 3; c++) xp[c] = x[c] + z[c] * kSmoothStd;
-        }
-        float sigma0 = 0.f, alb[3] = {0.f, 0.f, 0.f}, tapv[12];
-        #pragma unroll
-        for (int i = 0; i < 12; i++) tapv[i] = 0.f;
-
-        for (int e = 0; e < a.n_evals; e++) {
-            float p[3];
-            eval_pos(e, x, xp, a.bound, p);
-            const float inv2b = 2.f * a.bound;
-            encode_levels(a.table, s.lv, l0, lcount, (p[0] + a.bound) / inv2b, (p[1] + a.bound) / inv2b, (p[2] + a.bound) / inv2b,
-                          s.enc, TP, lrow);
-            __syncthreads();
-            tile_gemm<D_IN, D_H, true, false>(s.enc, s.wt1, s.b1, s.h1, nullptr);
-            __syncthreads();
-            tile_gemm<D_H, D_H, true, false>(s.h1, s.wt2, s.b2, s.h2, nullptr);
-            __syncthreads();
-            out_layer(s.h2, s.w3t, s.b3, s.o);
-            __syncthreads();
-            if (half == 0) {
-                const float sg = expf(s.o[lrow] + blob(p, a.blob_density, a.two_r2));
-                if (e == 0) {
-                    sigma0 = sg;
-                    #pragma unroll
-                    for (int c = 0; c < 3; c++) alb[c] = 1.f / (1.f + expf(-s.o[(1 + c) * TP + lrow]));
-                } else {
-                    #pragma unroll
-                    for (int i = 0; i < 12; i++) if (i == e - 1) tapv[i] = sg;
-                }
-            }
-        }
-        if (half == 0 && in_range) {
-            float col[3] = {alb[0], alb[1], alb[2]};
-            Normal nm, np;
-            if (a.n_evals >= 7) {
-                const float sp[3] = {tapv[0], tapv[2], tapv[4]}, sn[3] = {tapv[1], tapv[3], tapv[5]};
-                nm = make_normal(sp, sn);
-                if (lit) {
-                    const float ndl = (nm.n[0] * light[0] + nm.n[1] * light[1]) + nm.n[2] * light[2];
-                    const float lam = a.ratio + (1 - a.ratio) * fmaxf(ndl, 0.1f);
-                    if (a.shading == MI3D_SHADING_TEXTURELESS) { col[0] = col[1] = col[2] = lam; }
-                    else if (a.shading == MI3D_SHADING_NORMAL) { col[0] = (nm.n[0] + 1) / 2; col[1] = (nm.n[1] + 1) / 2; col[2] = (nm.n[2] + 1) / 2; }
-                    else { col[0] = alb[0] * lam; col[1] = alb[1] * lam; col[2] = alb[2] * lam; }
-                }
-                const float wgt = 1.f - expf(-sigma0);
-                const float ndd = fmaxf((nm.n[0] * d[0] + nm.n[1] * d[1]) + nm.n[2] * d[2], 0.f);
-                acc_orient += wgt * (ndd * ndd);
-                if (a.n_evals > 7) {
-                    const float sp2[3] = {tapv[6], tapv[8], tapv[10]}, sn2[3] = {tapv[7], tapv[9], tapv[11]};
-                    np = make_normal(sp2, sn2);
-                    acc_smooth += (fabsf(nm.n[0] - np.n[0]) + fabsf(nm.n[1] - np.n[1])) + fabsf(nm.n[2] - np.n[2]);
-                }
-                if (a.normals) { a.normals[3 * (size_t)row] = nm.n[0]; a.normals[3 * (size_t)row + 1] = nm.n[1]; a.normals[3 * (size_t)row + 2] = nm.n[2]; }
-            }
-            a.sigmas[row] = sigma0;
-            if (a.rgbs) { a.rgbs[3 * (size_t)row] = col[0]; a.rgbs[3 * (size_t)row + 1] = col[1]; a.rgbs[3 * (size_t)row + 2] = col[2]; }
-            if (a.tape) {
-                float4* tp = reinterpret_cast<float4*>(a.tape + 16 * (size_t)row);
-                tp[0] = make_float4(sigma0, alb[0], alb[1], alb[2]);
-                tp[1] = make_float4(tapv[0], tapv[1], tapv[2], tapv[3]);
-                tp[2] = make_float4(tapv[4], tapv[5], tapv[6], tapv[7]);
-                tp[3] = make_float4(tapv[8], tapv[9], tapv[10], tapv[11]);
-            }
-        }
-    }
-    if (a.loss_partials) {
-        // deterministic block reduction (fixed order), one slot per CTA
-        __shared__ float red[2][NT / 32];
-        float v0 = acc_orient, v1 = acc_smooth;
-        #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) { v0 += __shfl_xor_sync(0xffffffffu, v0, o); v1 += __shfl_xor_sync(0xffffffffu, v1, o); }
-        if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = v0; red[1][threadIdx.x >> 5] = v1; }
+        const bool in_range = row < n;
+        float p[3] = {0.f, 0.f, 0.f};
+        if (in_range) { p[0] = xyzs[3 * (size_t)row]; p[1] = xyzs[3 * (size_t)row + 1]; p[2] = xyzs[3 * (size_t)row + 2]; }
+        const float inv2b = 2.f * bound;
+        encode_levels(table, s.lv, l0, lcount, (p[0] + bound) / inv2b, (p[1] + bound) / inv2b, (p[2] + bound) / inv2b, s.enc, TP, lrow);
         __syncthreads();
-        if (threadIdx.x == 0) {
-            float t0 = 0.f, t1 = 0.f;
-            for (int w = 0; w < NT / 32; w++) { t0 += red[0][w]; t1 += red[1][w]; }
-            a.loss_partials[2 * blockIdx.x] = t0; a.loss_partials[2 * blockIdx.x + 1] = t1;
+        tile_gemm<D_IN, D_H>(s.enc, s.wt1, s.b1, s.h1);
+        __syncthreads();
+        tile_gemm<D_H, D_H>(s.h1, s.wt2, s.b2, s.h2);
+        __syncthreads();
+        out_layer(s.h2, s.w3t, s.b3, s.o);
+        __syncthreads();
+        if (half == 0 && in_range) {
+            // trunc_exp(h0 + blob(p)) with the fused multiply-adds spelled out: the compiler may contract blob()'s sum of squares either
+            // way, and the grid (hence the bitfield that every rank of a multi-GPU step must agree on) should not depend on its choice
+            const float d2 = fmaf(p[2], p[2], fmaf(p[0], p[0], p[1] * p[1]));
+            sigmas[row] = expf(fmaf(blob_density, expf(-d2 / two_r2), s.o[lrow]));
         }
     }
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// forward, tensor-core variant: the three layer GEMMs run on wgmma (tf32) with a 3-term split
+// forward: the three layer GEMMs run on wgmma (tf32) with a 3-term split
 //   x = hi + lo (hi = tf32-rounded x):  A.B ~= A_hi.B_hi + A_lo.B_hi + A_hi.B_lo     (error ~2^-21, fp32-class)
 // so the finite-difference normals keep their accuracy while the MLP leaves the FFMA pipe.
 // CTA = 512 threads, one 128-sample tile at a time (persistent):
@@ -984,11 +855,10 @@ struct BwdArgs {
     const float* tape;
     const float* g_sigmas; const float* g_rgbs; const float* g_normals; const float* g_loss_orient; const float* g_loss_smooth;
     float* g_table; mi3d_mlp_grad g_mlp;
-    // split pipeline (encode kernel -> tensor-core chain kernel -> scatter kernel) over tiles [tile0, tile1): see k_bwd_encode
-    float* enc_buf; float* denc_buf; uint32_t tile0, tile1;
+    // tiles [tile0, tile1) of this launch; enc_buf: their encodings [tile - tile0][13][128][32] (see k_bwd_enc_scatter), NULL = the
+    // chain kernel gathers them itself
+    float* enc_buf; uint32_t tile0, tile1;
     const mi3d_view_segs* segs; uint32_t noise_mode;   // multi-view: g_loss_orient / g_loss_smooth are [n_views] arrays
-    float agg_scale_max;                               // fused scatter: warp-aggregate the REDs of levels with scale below this
-    int e_pingpong;                                    // chain kernel: encodings of consecutive evaluations alternate between the two column halves of the E tile
 };
 
 // d(loss)/d(h) of the 13 evaluations of one sample from the upstream gradients and the forward tape (sigma0, albedo, tap sigmas):
@@ -1062,114 +932,6 @@ __device__ __forceinline__ void sample_out_grads(const BwdArgs& a, uint32_t row,
             for (int c = 0; c < 3; c++) dh[1 + c] = dalb[c] * alb[c] * (1.f - alb[c]);
 }
 
-__global__ void __launch_bounds__(NT, 1) k_field_bwd(const BwdArgs a) {
-    extern __shared__ __align__(16) float smem_raw[];
-    const Smem s = carve(smem_raw, true);
-    load_weights(s, a.mlp, a.hg, true);
-    const uint32_t M = a.counter ? min((uint32_t)a.counter[0], a.cap) : a.m_fixed;
-    const uint32_t m_pad = padded_rows(M, a.align, a.cap);
-    const int lrow = threadIdx.x & (T - 1), half = threadIdx.x >> 7;
-    const int nl = (int)a.hg.n_levels, l0 = half * (nl / 2), lcount = half ? nl - nl / 2 : nl / 2;
-    const bool lit = a.shading != MI3D_SHADING_ALBEDO && m_pad < 1000000u;
-    float light[3] = {0.f, 0.f, 0.f};
-    if (a.light_d) { light[0] = a.light_d[0]; light[1] = a.light_d[1]; light[2] = a.light_d[2]; }
-    const float Go = (a.g_loss_orient && a.n_evals >= 7) ? *a.g_loss_orient / (float)m_pad : 0.f;
-    const float Gs = (a.g_loss_smooth && a.n_evals > 7) ? *a.g_loss_smooth / (3.f * (float)m_pad) : 0.f;
-    // which evaluations can receive a non-zero gradient (CTA-uniform)
-    const bool need_ptaps = Gs != 0.f;
-    const bool need_taps = a.n_evals >= 7 && (need_ptaps || Go != 0.f || lit || a.g_normals != nullptr);
-    const int e_end = !need_taps ? 1 : (need_ptaps ? 13 : 7);
-
-    float aw2[4][4], aw1[4][2], aw3 = 0.f, ab2[4], ab1[4], ab3 = 0.f;
-    #pragma unroll
-    for (int i = 0; i < 4; i++) {
-        ab2[i] = 0.f; ab1[i] = 0.f;
-        #pragma unroll
-        for (int j = 0; j < 4; j++) aw2[i][j] = 0.f;
-        aw1[i][0] = 0.f; aw1[i][1] = 0.f;
-    }
-    __syncthreads();
-
-    for (uint32_t tile = blockIdx.x; (uint64_t)tile * T < m_pad; tile += gridDim.x) {
-        const uint32_t row = tile * T + lrow;
-        const bool in_range = row < m_pad, real = row < M;
-        float x[3] = {0.f, 0.f, 0.f}, d[3] = {0.f, 0.f, 0.f}, xp[3] = {0.f, 0.f, 0.f};
-        if (real) {
-            x[0] = a.xyzs[3 * (size_t)row]; x[1] = a.xyzs[3 * (size_t)row + 1]; x[2] = a.xyzs[3 * (size_t)row + 2];
-            if (a.dirs) { d[0] = a.dirs[3 * (size_t)row]; d[1] = a.dirs[3 * (size_t)row + 1]; d[2] = a.dirs[3 * (size_t)row + 2]; }
-        }
-        if (a.n_evals > 7 && in_range) {
-            float z[3];
-            if (a.smooth_noise) { z[0] = a.smooth_noise[3 * (size_t)row]; z[1] = a.smooth_noise[3 * (size_t)row + 1]; z[2] = a.smooth_noise[3 * (size_t)row + 2]; }
-            else gauss_pair(a.seed, row, 1u, z);
-            #pragma unroll
-            for (int c = 0; c < 3; c++) xp[c] = x[c] + z[c] * kSmoothStd;
-        }
-        // ---- per-sample output gradients (threads of half 0 own a sample) ----
-        float dh[4] = {0.f, 0.f, 0.f, 0.f};     // d/d(h0..h3) of the centre evaluation
-        float dtap[12];                          // d/d(h0) of the 12 tap evaluations
-        #pragma unroll
-        for (int i = 0; i < 12; i++) dtap[i] = 0.f;
-        if (half == 0 && in_range) sample_out_grads(a, row, real, d, lit, light, Go, Gs, need_ptaps, dh, dtap);
-
-        for (int e = 0; e < e_end; e++) {
-            float p[3];
-            eval_pos(e, x, xp, a.bound, p);
-            const float inv2b = 2.f * a.bound;
-            const float u0 = (p[0] + a.bound) / inv2b, u1 = (p[1] + a.bound) / inv2b, u2 = (p[2] + a.bound) / inv2b;
-            encode_levels(a.table, s.lv, l0, lcount, u0, u1, u2, s.enc, TP, lrow);
-            if (half == 0) {
-                float g0 = 0.f;
-                if (e == 0) { g0 = dh[0]; s.o[1 * TP + lrow] = dh[1]; s.o[2 * TP + lrow] = dh[2]; s.o[3 * TP + lrow] = dh[3]; }
-                else {
-                    #pragma unroll
-                    for (int i = 0; i < 12; i++) if (i == e - 1) g0 = dtap[i];
-                    s.o[1 * TP + lrow] = 0.f; s.o[2 * TP + lrow] = 0.f; s.o[3 * TP + lrow] = 0.f;
-                }
-                s.o[lrow] = g0;
-            }
-            __syncthreads();
-            tile_gemm<D_IN, D_H, true, false>(s.enc, s.wt1, s.b1, s.h1, nullptr);
-            __syncthreads();
-            tile_gemm<D_H, D_H, true, false>(s.h1, s.wt2, s.b2, s.h2, nullptr);
-            __syncthreads();
-            // layer 3: dW3 += dO^T H2 ; dH2 = relu'(H2) * (dO W3)
-            tile_wgrad3(s.o, s.h2, aw3, ab3);
-            __syncthreads();
-            tile_gemm<D_OUT, D_H, false, true>(s.o, s.w3, nullptr, s.h2, s.h2);
-            __syncthreads();
-            // layer 2
-            tile_wgrad<4>(s.h2, s.h1, aw2, ab2);
-            __syncthreads();
-            tile_gemm<D_H, D_H, false, true>(s.h2, s.w2, nullptr, s.h1, s.h1);
-            __syncthreads();
-            // layer 1
-            tile_wgrad<2>(s.h1, s.enc, aw1, ab1);
-            __syncthreads();
-            tile_gemm<D_H, D_IN, false, false>(s.h1, s.w1, nullptr, s.enc, nullptr);
-            __syncthreads();
-            if (in_range) scatter_levels(a.g_table, s.lv, l0, lcount, u0, u1, u2, s.enc, TP, lrow);
-            __syncthreads();
-        }
-    }
-    // flush the register-resident weight gradients (one RED per element per CTA)
-    {
-        const int jt = threadIdx.x >> 4, it = threadIdx.x & 15;
-        #pragma unroll
-        for (int p = 0; p < 4; p++) {
-            const int j = jt + 16 * p;
-            #pragma unroll
-            for (int q = 0; q < 4; q++) atomicAdd(a.g_mlp.w2 + j * D_H + it + 16 * q, aw2[p][q]);
-            #pragma unroll
-            for (int q = 0; q < 2; q++) atomicAdd(a.g_mlp.w1 + j * D_IN + it + 16 * q, aw1[p][q]);
-            if (it == 0) { atomicAdd(a.g_mlp.b2 + j, ab2[p]); atomicAdd(a.g_mlp.b1 + j, ab1[p]); }
-        }
-        const int o = threadIdx.x >> 6, i = threadIdx.x & 63;
-        atomicAdd(a.g_mlp.w3 + o * D_H + i, aw3);
-        if (i == 0) atomicAdd(a.g_mlp.b3 + o, ab3);
-    }
-}
-
 // the 16 encoding columns of one (row, half): four 16-byte chunks, 8 floats apart (see half_level)
 __device__ __forceinline__ void load16(const float* __restrict__ src, float (&f)[16]) {
     #pragma unroll
@@ -1180,16 +942,14 @@ __device__ __forceinline__ void load16(const float* __restrict__ src, float (&f)
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Split backward pipeline.  The single-kernel tensor-core backward can afford only 8 gather / scatter warps next to ~200 KB of operand
-// tiles.  The hash-grid gather and
-// the RED scatter are embarrassingly parallel over (sample, level), so they run as their own full-occupancy kernels around the
-// chain kernel and exchange encodings / encoding-gradients through a per-chunk HBM buffer (128 B per evaluation each way:
-// ~1.4 GB per backward at 128x128).
-//   k_bwd_encode : block = (tile, evaluation), thread = (row, group of 4 levels)  -> enc_buf[tile][e][row][32]
-//   k_field_bwd_tc (ext mode): loads enc, runs the MMA chain, stores d(enc) -> denc_buf
-//   k_bwd_scatter: same mapping as encode, warp-aggregated REDs (lanes = consecutive samples of a ray)
+// Gather kernel of the backward.  The chain kernel (k_field_bwd_tc) can afford only 8 gather / scatter warps next to ~200 KB of
+// operand tiles, and the scatter keeps them busy.  The hash-grid gather is embarrassingly parallel over (sample, level), so it runs
+// as a full-occupancy kernel ahead of the chain kernel and hands it the encodings through a per-chunk HBM buffer (128 B per
+// evaluation):
+//   k_bwd_enc_scatter: work item = (tile, evaluation), thread = (row, group of 4 levels)  -> enc_buf[tile - tile0][e][row][32]
+//   k_field_bwd_tc   : loads them, runs the MMA chain and scatters d(enc) itself
 // ---------------------------------------------------------------------------------------------------------
-// which evaluations can receive a non-zero gradient (uniform over the launch; identical in the gather / chain / scatter kernels)
+// which evaluations can receive a non-zero gradient (uniform over the launch; identical in the gather and chain kernels)
 struct BwdPlan { int e_end; bool need_ptaps; };
 __device__ __forceinline__ BwdPlan bwd_plan(const BwdArgs& a, const Rows& R) {
     const int nv = R.segs ? (int)R.segs->n_views : 1;
@@ -1207,7 +967,6 @@ __device__ __forceinline__ BwdPlan bwd_plan(const BwdArgs& a, const Rows& R) {
     return p;
 }
 
-template <bool SCATTER>
 __global__ void __launch_bounds__(512, 2) k_bwd_enc_scatter(const BwdArgs a) {
     __shared__ LevelSm lv[16];
     __shared__ mi3d_view_segs segs_sm;
@@ -1225,7 +984,7 @@ __global__ void __launch_bounds__(512, 2) k_bwd_enc_scatter(const BwdArgs a) {
     const Rows R = rows_make(a.counter, a.m_fixed, a.align, a.cap, a.segs ? &segs_sm : nullptr);
     const uint32_t m_pad = R.m_pad;
     const int e_end = bwd_plan(a, R).e_end;
-    const int r = threadIdx.x & (T - 1), lg = threadIdx.x >> 7, lane = threadIdx.x & 31;   // levels 4 lg .. 4 lg + 3
+    const int r = threadIdx.x & (T - 1), lg = threadIdx.x >> 7;   // levels 4 lg .. 4 lg + 3
     const float inv2b = 2.f * a.bound;
     // persistent grid-stride loop over (tile, evaluation) work items of this chunk
     for (uint32_t w = blockIdx.x;; w += gridDim.x) {
@@ -1247,25 +1006,15 @@ __global__ void __launch_bounds__(512, 2) k_bwd_enc_scatter(const BwdArgs a) {
         eval_pos(e, x, xp, a.bound, p);
         const float u0 = (p[0] + a.bound) / inv2b, u1 = (p[1] + a.bound) / inv2b, u2 = (p[2] + a.bound) / inv2b;
         const size_t base = ((size_t)(tile - a.tile0) * 13 + e) * (T * 32) + (size_t)r * 32 + 8 * lg;
-        if (!SCATTER) {
-            float f[16];
-            gather16(a.table, lv, 4 * lg, 4, u0, u1, u2, f);
-            float4* dst = reinterpret_cast<float4*>(a.enc_buf + base);
-            dst[0] = make_float4(f[0], f[1], f[2], f[3]); dst[1] = make_float4(f[4], f[5], f[6], f[7]);
-        } else {
-            const float4 g0 = __ldg(reinterpret_cast<const float4*>(a.denc_buf + base)), g1 = __ldg(reinterpret_cast<const float4*>(a.denc_buf + base) + 1);
-            const float g[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-            #pragma unroll
-            for (int i = 0; i < 4; i++) {
-                const LevelSm L = lv[4 * lg + i];
-                scatter_level_agg(a.g_table, L, u0, u1, u2, g[2 * i], g[2 * i + 1], in_range, L.scale < 200.f, lane);
-            }
-        }
+        float f[16];
+        gather16(a.table, lv, 4 * lg, 4, u0, u1, u2, f);
+        float4* dst = reinterpret_cast<float4*>(a.enc_buf + base);
+        dst[0] = make_float4(f[0], f[1], f[2], f[3]); dst[1] = make_float4(f[4], f[5], f[6], f[7]);
     }
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// backward, tensor-core variant.  Same roles as k_field_fwd_tc; per evaluation the MMA warpgroup runs
+// backward chain kernel.  Same roles as k_field_fwd_tc; per evaluation the MMA warpgroup runs
 //   F1: D1 = Enc W1^T          F2: D2 = H1 W2^T                               (recompute, K-major operands)
 //   G2: dH1 = dZ2 W2           WG2: dW2 += dZ2^T H1   (A3/A2/W2 tiles re-read MN-major: no transposed copies)
 //   G1: dEnc = dZ1 W1          WG1: dW1 += dZ1^T Enc
@@ -1290,6 +1039,11 @@ constexpr int oStg = oW2 + 3 * 8192;                               // staging [1
 constexpr int kStgLd = 36;
 constexpr int oMisc = oStg + 128 * kStgLd * 4;
 constexpr size_t kSmem = 1024 + oMisc + 3072;
+// Which levels' table-gradient REDs are warp-aggregated (scatter_level_agg): those with scale below this, i.e. where a cell spans
+// several march steps (2 / scale  >  ~1.5 dt_min): levels 0..7 of the reference grid.  The scans cost issue slots next to the owner
+// warps; the REDs they remove are the ones that serialise in L2 (the benchmark scene concentrates every sample in a sphere of radius
+// 0.2: ~2 k occupied cells at level 5).
+constexpr float kAggScaleMax = 100.f;
 
 // column-wise sum over the 32 lanes of a warp of v[0..31]; lane j returns the total of column j (recursive halving, 31 shuffles)
 __device__ __forceinline__ float warp_colsum32(float (&v)[32], int lane) {
@@ -1514,7 +1268,7 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
         asm volatile("setmaxnreg.dec.sync.aligned.u32 96;");
         const int et = tid - 128, r = et & (T - 1), half = et >> 7;
         const float* denc = reinterpret_cast<const float*>(sm + oZ);
-        const bool ext = a.enc_buf != nullptr, ext_out = a.denc_buf != nullptr, pp = a.e_pingpong != 0;
+        const bool ext = a.enc_buf != nullptr;
         for (uint32_t tile = a.tile0 + blockIdx.x; tile < a.tile1 && (uint64_t)tile * T < m_pad; tile += gridDim.x) {
             const uint32_t row = tile * T + r;
             const RowInfo ri = row_info(R, row);
@@ -1527,16 +1281,13 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                 #pragma unroll
                 for (int c = 0; c < 3; c++) xp[c] = x[c] + z[c] * kSmoothStd;
             }
-            // Software pipeline over the evaluations of this tile.
-            //   single-buffered E (pp == false): write E(e+1) as soon as chain(e) has retired (d4) and BEFORE scattering dEnc(e), so that the
-            //     MMA / epilogue chain of e+1 overlaps the scatter of e and the gather of e+2.  The hand-off (d4 -> dEnc load -> split -> store ->
-            //     a1) sits on the chain's critical path.
-            //   ping-pong E (pp == true): the encoding uses 32 of the tile's 64 columns, so evaluation `it` lives in columns 32 (it & 1) .. + 31
-            //     (operand start address + 64 B).  E(it+2) is written at the END of iteration `it` (its half was last read by chain(it), retired
-            //     at d4(it)); chain(it+1) then starts the moment chain(it) retires -- the MMA warp has already seen a1(it+1).
+            // Software pipeline over the evaluations of this tile: ping-pong E.  The encoding uses 32 of the tile's 64 columns, so evaluation
+            // `it` lives in columns 32 (it & 1) .. + 31 (operand start address + 64 B).  E(it+2) is written at the END of iteration `it` (its
+            // half was last read by chain(it), retired at d4(it)), after the scatter of dEnc(it) under which its gather loads were in flight;
+            // chain(it+1) then starts the moment chain(it) retires -- the MMA warp has already seen a1(it+1).
             float f[16];
             auto write_E = [&](const float (&ff)[16], const uint32_t itw) {
-                const int ecol = pp ? 32 * (int)(itw & 1u) : 0;
+                const int ecol = 32 * (int)(itw & 1u);
                 #pragma unroll
                 for (int i = 0; i < 8; i++) {
                     const int k = 2 * half_level(i, half) + ecol;
@@ -1557,8 +1308,8 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                 gather16s(a.table, lv, half, (p[0] + a.bound) / inv2b, (p[1] + a.bound) / inv2b, (p[2] + a.bound) / inv2b, ff);
             };
             fetch(0, f);
-            write_E(f, it);            // E (pp: this half) is free: this thread waited for d4 of the evaluations that read it
-            if (pp && e_end > 1) {
+            write_E(f, it);            // this half of E is free: this thread waited for d4 of the evaluations that read it
+            if (e_end > 1) {
                 fetch(1, f);
                 // a1 may run at most one phase ahead of its waiter: F1(it) issued (d1) => the MMA warp has consumed a1 phase `it`
                 tc::mbar_wait(d1_full, it & 1);
@@ -1569,9 +1320,7 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                 float p[3];
                 eval_pos(e, x, xp, a.bound, p);
                 const float u0 = (p[0] + a.bound) / inv2b, u1 = (p[1] + a.bound) / inv2b, u2 = (p[2] + a.bound) / inv2b;
-                const int en = pp ? e + 2 : e + 1;              // the evaluation whose encodings this iteration hands over
-                // single-buffered: prefetch the next evaluation's gather while the MMA / epilogue chain of this one runs
-                if (!pp && en < e_end) fetch(en, f);
+                const int en = e + 2;                           // the evaluation whose encodings this iteration hands over
                 // dEnc (this thread's 16 columns of its row: 8j + 4 half .. + 3, j = 0..3) into registers
                 tc::mbar_wait(d4_full, par);
                 uint32_t g[16];
@@ -1581,24 +1330,16 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                     g[4 * j] = __float_as_uint(t.x); g[4 * j + 1] = __float_as_uint(t.y); g[4 * j + 2] = __float_as_uint(t.z); g[4 * j + 3] = __float_as_uint(t.w);
                 }
                 mbar_arrive(denc_free);
-                // chain(e) has retired: E is free -> hand the next evaluation to the MMA warp before scattering this one
-                if (!pp && en < e_end) write_E(f, it + 1);
-                if (pp && en < e_end) fetch(en, f);            // ping-pong: loads in flight under the scatter
-                if (ext_out) {
-                    float4* dst = reinterpret_cast<float4*>(a.denc_buf + ((size_t)(tile - a.tile0) * 13 + e) * (T * 32) + (size_t)r * 32 + 4 * half);
-                    #pragma unroll
-                    for (int q = 0; q < 4; q++) dst[2 * q] = make_float4(__uint_as_float(g[4 * q]), __uint_as_float(g[4 * q + 1]), __uint_as_float(g[4 * q + 2]), __uint_as_float(g[4 * q + 3]));
-                } else
+                if (en < e_end) fetch(en, f);                   // loads in flight under the scatter
                 #pragma unroll 1
                 for (int i = 0; i < 8; i++) {
                     float g0 = 0.f, g1 = 0.f;
                     #pragma unroll
                     for (int q = 0; q < 8; q++) if (q == i) { g0 = __uint_as_float(g[2 * q]); g1 = __uint_as_float(g[2 * q + 1]); }
                     const LevelSm L = lv[half_level(i, half)];
-                    // aggregate where a cell spans several march steps (2 / scale  >  ~1.5 dt_min): levels 0..7 of the reference grid
-                    scatter_level_agg(a.g_table, L, u0, u1, u2, g0, g1, in_range, L.scale < a.agg_scale_max, lane);
+                    scatter_level_agg(a.g_table, L, u0, u1, u2, g0, g1, in_range, L.scale < kAggScaleMax, lane);
                 }
-                if (pp && en < e_end) write_E(f, it + 2);
+                if (en < e_end) write_E(f, it + 2);
             }
         }
     } else {
@@ -1608,7 +1349,6 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
         float* stg_w = reinterpret_cast<float*>(sm + oStg);
         float* denc_w = reinterpret_cast<float*>(sm + oZ);
         const int wl = warp & 3;
-        const bool pp = a.e_pingpong != 0;
         // dW2 [64 x 64], dW1 [64 x 32] over every sample of this CTA: each evaluation's product starts a fresh accumulator and is added
         // here in fp32 (round to nearest) -- a chain of thousands of accumulating MMAs drifts further from the fp32 sum
         float dw2[32], dw1[16];
@@ -1630,12 +1370,12 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
         for (uint32_t tile = a.tile0 + blockIdx.x; tile < a.tile1 && (uint64_t)tile * T < m_pad; tile += gridDim.x) {
             for (int e = 0; e < e_end; e++, it++) {
                 const uint32_t par = it & 1;
-                const uint32_t eoff = pp ? 64u * (it & 1u) : 0u;            // ping-pong E: columns 32 (it & 1) .. + 31 of the tile
+                const uint32_t eoff = 64u * (it & 1u);                      // ping-pong E: columns 32 (it & 1) .. + 31 of the tile
                 const Operand E{sbase + oE + eoff, (uint32_t)kTile, (uint32_t)kTile}, H{sbase + oH, (uint32_t)kTile, (uint32_t)kTile};
                 const Operand Z{sbase + oZ, (uint32_t)kTile, (uint32_t)kTile};
                 const Operand W1{sbase + oW1, 8192u, 8192u}, W2{sbase + oW2, 8192u, 8192u};
                 float d[2][32];
-                if (!(pp && e > 0)) tc::mbar_wait(a1_full, par);     // ping-pong: consumed before d4 of the previous evaluation
+                if (e == 0) tc::mbar_wait(a1_full, par);             // e > 0: consumed before d4 of the previous evaluation
                 mbar_arrive(d1_full);
                 wg::fence();
                 #pragma unroll
@@ -1669,9 +1409,9 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                 #pragma unroll
                 for (int i = 0; i < 16; i++) dw1[i] += t1[i];
                 stage_frag<16>(g1, denc_w, 32, 0, 32, wl, lane);                                       // over the dZ tiles, now free
-                // ping-pong: E(it+1) is already there (other half).  Consuming its a1 phase BEFORE releasing d4(it) keeps the encoders,
+                // E(it+1) is already there (other half).  Consuming its a1 phase BEFORE releasing d4(it) keeps the encoders,
                 // who arrive for it+2 only after d4(it), from lapping this waiter.
-                if (pp && e + 1 < e_end) tc::mbar_wait(a1_full, par ^ 1u);
+                if (e + 1 < e_end) tc::mbar_wait(a1_full, par ^ 1u);
                 mbar_arrive(d4_full);
             }
         }
@@ -1805,8 +1545,7 @@ int num_sms() {
 bool g_attr_set = false;
 int ensure_attrs() {
     if (!g_attr_set) {
-        MI3D_CHECK(cudaFuncSetAttribute(k_field_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes(false)));
-        MI3D_CHECK(cudaFuncSetAttribute(k_field_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes(true)));
+        MI3D_CHECK(cudaFuncSetAttribute(k_field_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFwdSmem));
         MI3D_CHECK(cudaFuncSetAttribute(k_field_fwd_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwdtc::kSmem));
         MI3D_CHECK(cudaFuncSetAttribute(k_field_bwd_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwdtc::kSmem));
         g_attr_set = true;
@@ -1852,11 +1591,9 @@ int mi3d_hashgrid_backward(const float* x, uint32_t E, const float* grad_out, co
     MI3D_RETURN_LAUNCH();
 }
 
-// cfg->impl selects the kernels explicitly (no environment switches inside the library): MI3D_FIELD_IMPL_TCGEN05 (default) or
-// MI3D_FIELD_IMPL_FFMA (the round-1a register-tiled kernels; they also serve the density-grid refresh).  Both are parity-tested.
-constexpr uint32_t kBwdChunkTiles = 8192;     // 1 048 576 samples per chunk: 2 x 1.74 GB of encoding / gradient staging
+constexpr uint32_t kBwdChunkTiles = 8192;     // 1 048 576 samples per chunk: 1.74 GB of encoding staging
 
-size_t mi3d_field_backward_workspace_bytes(void) { return (size_t)2 * kBwdChunkTiles * 13 * T * 32 * sizeof(float); }
+size_t mi3d_field_backward_workspace_bytes(void) { return (size_t)kBwdChunkTiles * 13 * T * 32 * sizeof(float); }
 
 int mi3d_field_grid_ctas(int backward) { return num_sms() * (backward ? 1 : 2); }
 
@@ -1875,14 +1612,11 @@ int mi3d_field_forward(const mi3d_field_io* io, const float* table, const mi3d_h
     a.n_evals = cfg->n_evals; a.shading = cfg->shading; a.ratio = cfg->ambient_ratio; a.light_d = cfg->light_d;
     a.smooth_noise = io->smooth_noise; a.seed = io->seed;
     a.sigmas = sigmas; a.rgbs = rgbs; a.normals = normals; a.tape = tape; a.loss_partials = loss_partials;
-    const bool use_tc = cfg->impl != MI3D_FIELD_IMPL_FFMA;
-    a.enc_cache = (use_tc && hg->n_levels == 16) ? io->enc_cache : nullptr; a.enc_cache_tiles = io->enc_cache_tiles;
+    a.enc_cache = io->enc_cache; a.enc_cache_tiles = io->enc_cache_tiles;
     a.segs = io->segs; a.noise_mode = io->noise_mode;
-    if ((io->segs || io->noise_mode) && !use_tc) return MI3D_ERR_ARG;
     if (io->segs && (io->n_views == 0 || io->n_views > MI3D_MAX_VIEWS)) return MI3D_ERR_ARG;
-    int grid = mi3d_field_grid_ctas(0);
-    if (use_tc) { grid = num_sms(); k_field_fwd_tc<<<grid, fwdtc::kThreads, fwdtc::kSmem, (cudaStream_t)stream>>>(a); }
-    else k_field_fwd<<<grid, NT, smem_bytes(false), (cudaStream_t)stream>>>(a);
+    const int grid = num_sms();
+    k_field_fwd_tc<<<grid, fwdtc::kThreads, fwdtc::kSmem, (cudaStream_t)stream>>>(a);
     if (loss_orient || loss_smooth)
         k_loss_finalize<<<1, 32, 0, (cudaStream_t)stream>>>(loss_partials, grid, io->counter, io->m_fixed, io->align, io->cap, loss_orient, loss_smooth,
                                                              io->segs ? (int)io->n_views : 0);
@@ -1906,48 +1640,27 @@ int mi3d_field_backward(const mi3d_field_io* io, const float* table, const mi3d_
     a.tape = tape; a.g_sigmas = grad_sigmas; a.g_rgbs = grad_rgbs; a.g_normals = grad_normals;
     a.g_loss_orient = grad_loss_orient; a.g_loss_smooth = grad_loss_smooth;
     a.g_table = grad_table; a.g_mlp = *grad_mlp;
-    a.enc_buf = nullptr; a.denc_buf = nullptr; a.tile0 = 0; a.tile1 = 0xFFFFFFFFu; a.agg_scale_max = 100.f;
-    a.e_pingpong = cfg->impl != MI3D_FIELD_IMPL_TCGEN05_SINGLE_E && cfg->impl != MI3D_FIELD_IMPL_TCGEN05_SPLIT_SCATTER;
+    a.enc_buf = nullptr; a.tile0 = 0; a.tile1 = 0xFFFFFFFFu;
     a.segs = io->segs; a.noise_mode = io->noise_mode;
-    if ((io->segs || io->noise_mode) && cfg->impl == MI3D_FIELD_IMPL_FFMA) return MI3D_ERR_ARG;
     if (io->segs && (io->n_views == 0 || io->n_views > MI3D_MAX_VIEWS)) return MI3D_ERR_ARG;
-    if (cfg->impl != MI3D_FIELD_IMPL_FFMA) {
-        if (workspace && hg->n_levels == 16) {
-            // split pipeline, chunk by chunk (the sample count lives on the device: chunks past it return immediately)
-            float* enc_tmp = (float*)workspace;
-            a.denc_buf = enc_tmp + (size_t)kBwdChunkTiles * 13 * T * 32;
-            const bool cached = io->enc_cache && io->enc_cache_valid;
-            const uint32_t total_tiles = (io->cap + T - 1) / T;
-            for (uint32_t t0 = 0; t0 < total_tiles; t0 += kBwdChunkTiles) {
-                a.tile0 = t0; a.tile1 = t0 + kBwdChunkTiles;
-                if (cached && (t0 + kBwdChunkTiles < total_tiles ? t0 + kBwdChunkTiles : total_tiles) <= io->enc_cache_tiles)
-                    a.enc_buf = io->enc_cache + (size_t)t0 * 13 * T * 32;   // saved by the forward
-                else { a.enc_buf = enc_tmp; k_bwd_enc_scatter<false><<<num_sms() * 4, 512, 0, (cudaStream_t)stream>>>(a); }
-                // Where the table-gradient REDs are issued: the RED stream is bound by the load / store unit, the MMA / epilogue chain by
-                // its serial hand-offs, so by default they overlap in one kernel (impl = TCGEN05_SPLIT_SCATTER runs the scatter as a kernel
-                // of its own; tools/prof_render.py --impl times both arms).
-                const bool fuse = cfg->impl != MI3D_FIELD_IMPL_TCGEN05_SPLIT_SCATTER;
-                // Which levels' REDs are warp-aggregated inside the chain kernel.  The scans cost issue slots next to the owner warps, the REDs
-                // they remove are the ones that serialise in L2 (the benchmark scene concentrates every sample in a sphere of radius 0.2:
-                // ~2 k occupied cells at level 5).  The threshold is cfg->scatter_agg_scale (default 100); tools/prof_render.py --agg times it.
-                a.agg_scale_max = cfg->scatter_agg_scale > 0.f ? cfg->scatter_agg_scale : 100.f;
-                if (fuse) {
-                    // the chain kernel's encoder warps scatter d(enc) themselves, from shared memory: the RED stream (LSU-bound) runs
-                    // under the MMA / epilogue chain (latency-bound) of the next evaluation instead of in a kernel of its own
-                    float* const denc = a.denc_buf;
-                    a.denc_buf = nullptr;
-                    k_field_bwd_tc<<<num_sms(), bwdtc::kThreads, bwdtc::kSmem, (cudaStream_t)stream>>>(a);
-                    a.denc_buf = denc;
-                } else {
-                    k_field_bwd_tc<<<num_sms(), bwdtc::kThreads, bwdtc::kSmem, (cudaStream_t)stream>>>(a);
-                    k_bwd_enc_scatter<true><<<num_sms() * 4, 512, 0, (cudaStream_t)stream>>>(a);
-                }
-                if (!io->counter && (uint64_t)(t0 + kBwdChunkTiles) * T >= io->m_fixed) break;
-            }
-        } else {
+    if (workspace) {
+        // chunk by chunk (the sample count lives on the device: chunks past it return immediately): gather kernel, then the chain
+        // kernel, whose encoder warps scatter d(enc) themselves from shared memory -- the RED stream is bound by the load / store unit,
+        // the MMA / epilogue chain by its serial hand-offs, so they overlap in one kernel
+        float* enc_tmp = (float*)workspace;
+        const bool cached = io->enc_cache && io->enc_cache_valid;
+        const uint32_t total_tiles = (io->cap + T - 1) / T;
+        for (uint32_t t0 = 0; t0 < total_tiles; t0 += kBwdChunkTiles) {
+            a.tile0 = t0; a.tile1 = t0 + kBwdChunkTiles;
+            if (cached && (t0 + kBwdChunkTiles < total_tiles ? t0 + kBwdChunkTiles : total_tiles) <= io->enc_cache_tiles)
+                a.enc_buf = io->enc_cache + (size_t)t0 * 13 * T * 32;   // saved by the forward
+            else { a.enc_buf = enc_tmp; k_bwd_enc_scatter<<<num_sms() * 4, 512, 0, (cudaStream_t)stream>>>(a); }
             k_field_bwd_tc<<<num_sms(), bwdtc::kThreads, bwdtc::kSmem, (cudaStream_t)stream>>>(a);
+            if (!io->counter && (uint64_t)(t0 + kBwdChunkTiles) * T >= io->m_fixed) break;
         }
-    } else k_field_bwd<<<mi3d_field_grid_ctas(1), NT, smem_bytes(true), (cudaStream_t)stream>>>(a);
+    } else {
+        k_field_bwd_tc<<<num_sms(), bwdtc::kThreads, bwdtc::kSmem, (cudaStream_t)stream>>>(a);
+    }
     MI3D_RETURN_LAUNCH();
 }
 
@@ -1978,14 +1691,8 @@ int mi3d_density_grid_update(float* density_grid, uint8_t* bitfield, uint32_t C,
     for (uint32_t cas = 0; cas < C; cas++) {
         const float cas_bound = fminf((float)(1u << cas), bound);                 // renderer.py:612
         k_grid_positions<<<nparts, 256, 0, st>>>(H, cas_bound, jitter ? jitter + (size_t)cas * n * 3 : nullptr, seed, cas, xyz);
-        FwdArgs a{};
-        a.xyzs = xyz; a.dirs = nullptr; a.counter = nullptr; a.m_fixed = n; a.align = 0; a.cap = n;
-        a.table = table; a.hg = *hg; a.mlp = *mlp;
-        a.bound = cfg->bound; a.blob_density = cfg->blob_density; a.two_r2 = (float)(2.0 * (double)cfg->blob_radius * (double)cfg->blob_radius);
-        a.n_evals = 1; a.shading = MI3D_SHADING_ALBEDO; a.ratio = 1.f; a.light_d = nullptr;
-        a.smooth_noise = nullptr; a.seed = 0;
-        a.sigmas = sig; a.rgbs = nullptr; a.normals = nullptr; a.tape = nullptr; a.loss_partials = nullptr;
-        k_field_fwd<<<mi3d_field_grid_ctas(0), NT, smem_bytes(false), st>>>(a);
+        k_field_fwd<<<mi3d_field_grid_ctas(0), NT, kFwdSmem, st>>>(xyz, n, table, *hg, *mlp, cfg->bound, cfg->blob_density,
+                                                                   (float)(2.0 * (double)cfg->blob_radius * (double)cfg->blob_radius), sig);
         k_grid_ema<<<nparts, 256, 0, st>>>(density_grid + (size_t)cas * n, sig, n, decay, psum + (size_t)cas * nparts, pcnt + (size_t)cas * nparts);
     }
     k_grid_mean<<<1, 256, 0, st>>>(psum, pcnt, nparts * C, mean_density_out);

@@ -61,8 +61,6 @@ def _cfg_struct(cfg, light_d):
     c.bound = cfg["bound"]; c.blob_density = cfg["blob_density"]; c.blob_radius = cfg["blob_radius"]
     c.n_evals = cfg["n_evals"]; c.shading = L.SHADING[cfg["shading"]]; c.ambient_ratio = cfg["ambient_ratio"]
     c.light_d = light_d.data_ptr() if light_d is not None else None
-    c.impl = L.FIELD_IMPL[cfg.get("impl", "tcgen05")]
-    c.scatter_agg_scale = float(cfg.get("scatter_agg_scale", 0.0))
     return c
 
 

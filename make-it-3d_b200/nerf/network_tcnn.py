@@ -108,8 +108,7 @@ class NeRFNetwork(NeRFRenderer):
         net = self.sigma_net.net
         mlp_params = (net[0].weight, net[0].bias, net[1].weight, net[1].bias, net[2].weight, net[2].bias)
         cfg = dict(bound=float(self.bound), blob_density=float(self.opt.blob_density), blob_radius=float(self.opt.blob_radius),
-                   n_evals=7, shading='albedo', ambient_ratio=1.0, impl=getattr(self.opt, "field_impl", "tcgen05"),
-                   scatter_agg_scale=float(getattr(self.opt, "scatter_agg_scale", 0.0)))
+                   n_evals=7, shading='albedo', ambient_ratio=1.0)
         return self.encoder.params, mlp_params, self.encoder.hg, cfg
 
     def _eval(self, x, d, l, n_evals, shading, ratio):

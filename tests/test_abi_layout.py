@@ -43,7 +43,5 @@ def test_enum_values_match_the_header():
     hdr = open(os.path.join(ROOT, "include", "mi3d.h")).read()
     import re
     vals = {k: int(v) for k, v in re.findall(r"(MI3D_[A-Z0-9_]+)\s*=\s*(\d+)", hdr)}
-    for name, v in L.FIELD_IMPL.items():
-        assert vals["MI3D_FIELD_IMPL_" + name.upper()] == v
     for name, v in L.SHADING.items():
         assert vals["MI3D_SHADING_" + name.upper()] == v

@@ -108,14 +108,12 @@ def test_density_matches_oracle_and_k1_backward():
     assert max_abs(net.sigma_net.net[1].weight.grad.cpu(), q) / float(q.abs().max()) < 1e-3
 
 
-@pytest.mark.parametrize("impl", ["tcgen05", "ffma", "tcgen05_fused_scatter", "tcgen05_split_scatter", "tcgen05_single_e"])
 @pytest.mark.parametrize("case", ["albedo", "lambertian", "textureless"])
-def test_fused_render_step_matches_reference_golden(case, impl):
+def test_fused_render_step_matches_reference_golden(case):
     """The drop-in call Trainer.train_step makes (model.render(...), nerf/utils.py:496) on the fused CUDA path vs the
-    golden vectors recorded from the reference's Python: image / depth / weights_sum / losses and parameter gradients.
-    Both kernel families (mi3d_field_cfg.impl: tensor-core split-precision tiles, fp32 FFMA tiles) are held to the same bounds."""
+    golden vectors recorded from the reference's Python: image / depth / weights_sum / losses and parameter gradients."""
     g = load_golden(f"render_{case}.npz")
-    net = _net_from_golden(g, field_impl=impl)
+    net = _net_from_golden(g)
     net.train()
     net.density_bitfield = _cu(sphere_bitfield(float(g["radius"])))
     out = net.render(_cu(g["rays_o"])[None], _cu(g["rays_d"])[None], depth_scale=_cu(g["depth_scale"])[None], bg_color=_cu(g["bg_color"]),

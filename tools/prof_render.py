@@ -20,12 +20,10 @@ def main():
     ap.add_argument("--radius", type=float, default=0.2)
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--shading", default="albedo")
-    ap.add_argument("--impl", default="tcgen05")
-    ap.add_argument("--agg", type=float, default=0.0, help="mi3d_field_cfg.scatter_agg_scale (0 = library default)")
     args = ap.parse_args()
     nt = importlib.import_module("make-it-3d_b200.nerf.network_tcnn")
     opt = argparse.Namespace(bound=1, min_near=0.1, density_thresh=10, bg_radius=-1, blob_density=5, blob_radius=0.1,
-                             lambda_smooth=1, max_depth=10.0, field_impl=args.impl, scatter_agg_scale=args.agg)
+                             lambda_smooth=1, max_depth=10.0)
     torch.manual_seed(0)
     net = nt.NeRFNetwork(opt).cuda().train()
     with torch.no_grad():
