@@ -410,6 +410,38 @@ int mi3d_gemm_f16_bt(const void* a, const void* bt, void* out, int M, int N, int
 int mi3d_conv3x3_f16(const void* x, const void* w, void* y, int Nimg, int H, int W, int Cin, int Cout, int block_n,
                      const float* bias, const void* residual, mi3d_stream_t stream);
 
+/* Test path: one op of the engines' shared op layer (plan::Builder / plan::TowerBuilder), recorded through the same builder method
+ * the engines call (block-N choice, split-K planning, m_valid and tensor-map encoding included) and run eagerly on `stream`.
+ * plan (nullable, int[2]): receives the tile kernel's block-N and split count the builder planned.
+ * splitk_ws / splitk_bytes: the fp32 split-K scratch the builder may plan into (NULL / 0: no split-K). */
+typedef struct {
+    const void* a; long long lda, a_rows; int K; int a_z1; long long a_sz1; int a_z2; long long a_sz2;   /* Builder::Mat of A */
+    const void* b; long long ldb, b_rows; int b_z1; long long b_sz1; int b_z2; long long b_sz2;          /* Builder::Mat of B */
+    int N, batch, b_batched;
+    void* out16; void* out32; long long ldc; int out_z1; long long out_s_lo, out_s_hi;                   /* Builder::Out */
+    const float* bias; const float* row_bias; int rows_per_group; const void* residual; long long ld_res;   /* Builder::Epi */
+    int mode; float alpha; void* aux;
+} mi3d_op_gemm_args;
+int mi3d_op_gemm(const mi3d_op_gemm_args* g, void* splitk_ws, size_t splitk_bytes, int* plan, mi3d_stream_t stream);
+/* Builder::conv3: x [Nimg,H,W,Cin], w [Cout][3][3][Cin], y [Nimg,H,W,Cout]; row_bias [Nimg][Cout] (one row per image) */
+int mi3d_op_conv3(const void* x, const void* w, void* y, int Nimg, int H, int W, int Cin, int Cout, const float* bias, const float* row_bias,
+                  const void* residual, void* splitk_ws, size_t splitk_bytes, int* plan, mi3d_stream_t stream);
+/* Builder::conv3_block (any H x W): mode 0 plain (+ residual), 5 ReLU, 6 ReLU input gradient masked by aux > 0 */
+int mi3d_op_conv3_block(const void* x, const void* w, void* y, int Nimg, int H, int W, int Cin, int Cout, const float* bias, int mode,
+                        const void* aux, const void* residual, int* plan, mi3d_stream_t stream);
+/* TowerBuilder attention on the packed qkv [B*Tpad][3C] of a block (C = 64 heads): mode 0 the fused attention as block_fwd calls it,
+ * 1 attention_materialised, 2 attention_materialised causal.  Writes o [B*Tpad][C]; modes 1, 2 also need qkvT [B][3C][Tpad] and
+ * S [B*heads][Tpad][Tpad] (left holding P). */
+int mi3d_op_attention(const void* qkv, void* qkvT, void* S, void* o, int B, int T, int Tpad, int heads, int mode, mi3d_stream_t stream);
+/* row kernels with the engines' launch geometry: Builder::layernorm, clipk::k_layernorm_bwd (add nullable), Builder::softmax
+ * (causal_tq > 0: clipk::k_softmax_causal over [rows / tq][tq][cols]), sdk::k_softmax_bwd, Builder::transpose ([Z][R][C] -> [Z][C][R]) */
+int mi3d_op_layernorm(const void* x, void* y, const float* gamma, const float* beta, int rows, int C, float eps, mi3d_stream_t stream);
+int mi3d_op_layernorm_bwd(const void* x, const void* dy, const float* gamma, const void* add, void* dx, int rows, int C, float eps,
+                          mi3d_stream_t stream);
+int mi3d_op_softmax(void* s, size_t rows, int cols, int valid, int causal_tq, float scale, mi3d_stream_t stream);
+int mi3d_op_softmax_bwd(const void* p, void* dp, size_t rows, int cols, float scale, mi3d_stream_t stream);
+int mi3d_op_transpose(const void* in, void* out, int Z, int R, int C, mi3d_stream_t stream);
+
 /* Stable-Diffusion engine: a statically planned launch list over the tile kernel above + memory-bound kernels.
  * Configuration mirrors diffusers' UNet2DConditionModel / AutoencoderKL config.json fields that nerf/sd.py:41,53 load. */
 typedef struct {

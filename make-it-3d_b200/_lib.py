@@ -85,6 +85,19 @@ class RenderWs(C.Structure):
                                           "segs", "enc_cache")] + [("enc_cache_tiles", C.c_uint32), ("bytes", C.c_size_t)]
 
 
+class OpGemmArgs(C.Structure):
+    """mi3d_op_gemm_args: one plan::Builder::gemm (test path)"""
+    _fields_ = [("a", C.c_void_p), ("lda", C.c_longlong), ("a_rows", C.c_longlong), ("K", C.c_int), ("a_z1", C.c_int), ("a_sz1", C.c_longlong),
+                ("a_z2", C.c_int), ("a_sz2", C.c_longlong),
+                ("b", C.c_void_p), ("ldb", C.c_longlong), ("b_rows", C.c_longlong), ("b_z1", C.c_int), ("b_sz1", C.c_longlong),
+                ("b_z2", C.c_int), ("b_sz2", C.c_longlong),
+                ("N", C.c_int), ("batch", C.c_int), ("b_batched", C.c_int),
+                ("out16", C.c_void_p), ("out32", C.c_void_p), ("ldc", C.c_longlong), ("out_z1", C.c_int), ("out_s_lo", C.c_longlong),
+                ("out_s_hi", C.c_longlong),
+                ("bias", C.c_void_p), ("row_bias", C.c_void_p), ("rows_per_group", C.c_int), ("residual", C.c_void_p), ("ld_res", C.c_longlong),
+                ("mode", C.c_int), ("alpha", C.c_float), ("aux", C.c_void_p)]
+
+
 RENDER_PHASE_MARCH, RENDER_PHASE_SHADE, RENDER_PHASE_ALL = 1, 2, 3
 
 SHADING = {"albedo": 0, "lambertian": 1, "textureless": 2, "normal": 3}
@@ -102,6 +115,8 @@ SYMBOLS = [
     "mi3d_density_grid_workspace_bytes", "mi3d_density_grid_update", "mi3d_version",
     "mi3d_sumsq_workspace_bytes", "mi3d_sumsq", "mi3d_adan_step",
     "mi3d_gemm_f16", "mi3d_gemm_f16_splitk", "mi3d_flash_attn_f16", "mi3d_conv3x3_f16", "mi3d_tf32_tile_test", "mi3d_gemm_f16_bt",
+    "mi3d_op_gemm", "mi3d_op_conv3", "mi3d_op_conv3_block", "mi3d_op_attention", "mi3d_op_layernorm", "mi3d_op_layernorm_bwd",
+    "mi3d_op_softmax", "mi3d_op_softmax_bwd", "mi3d_op_transpose",
     "mi3d_engine_destroy", "mi3d_engine_num_params", "mi3d_engine_param_name", "mi3d_engine_param_shape", "mi3d_engine_load_param",
     "mi3d_engine_set_graph_replay", "mi3d_engine_graph_replays", "mi3d_engine_debug_tensor",
     "mi3d_sd_workspace_bytes", "mi3d_sd_create", "mi3d_sd_encode", "mi3d_sd_encode_backward", "mi3d_sd_unet_sds", "mi3d_sd_profile",

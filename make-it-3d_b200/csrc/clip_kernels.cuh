@@ -178,15 +178,8 @@ __global__ void k_layernorm_bwd(const __half* __restrict__ x, const __half* __re
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (row >= rows) return;
     const __half* xr = x + (size_t)row * C; const __half* dr = dy + (size_t)row * C;
-    float s = 0.f, ss = 0.f;
-    for (int c = lane * 8; c < C; c += 256) {
-        const uint4 raw = *reinterpret_cast<const uint4*>(xr + c);
-        const __half* h = reinterpret_cast<const __half*>(&raw);
-        #pragma unroll
-        for (int k = 0; k < 8; k++) { const float v = __half2float(h[k]); s += v; ss += v * v; }
-    }
-    s = sdk::warp_sum(s); ss = sdk::warp_sum(ss);
-    const float mean = s / C, var = fmaxf(ss / C - mean * mean, 0.f), rstd = rsqrtf(var + eps);
+    float mean, rstd;
+    sdk::row_stats(xr, C, eps, lane, mean, rstd);
     float g1 = 0.f, g2 = 0.f;
     for (int c = lane * 8; c < C; c += 256) {
         const uint4 rx = *reinterpret_cast<const uint4*>(xr + c), rd = *reinterpret_cast<const uint4*>(dr + c);

@@ -150,7 +150,7 @@ struct Builder : mi3d_engine {
     void gemm(const Mat& a, const Mat& b, int N, const Out& o, const Epi& e, int batch = 1, bool b_batched = false) {
         if (dry) return;
         const long long mt = (a.rows + 127) / 128;
-        int bn = tc::pick_block_n(N, mt * batch, num_sms);
+        int bn = tc::pick_block_n(N, mt * batch, num_sms, tc::has_block_n_160(e.mode, 0));
         if (bn == 0 || a.K % 64) { err = MI3D_ERR_ARG; return; }
         int splits = 1;
         if (batch == 1 && e.mode == tc::EPI_PLAIN && o.p16 && a.rows % 128 == 0 && (size_t)a.rows * N <= splitk_elems) {
@@ -227,7 +227,7 @@ struct Builder : mi3d_engine {
             if (best < 0 || area < best) { best = area; bw = cw; bh = 128 / cw; }
         }
         const long long tiles = (long long)x.n * ((x.w + bw - 1) / bw) * ((x.h + bh - 1) / bh);
-        const int bn = tc::pick_block_n(Cout, tiles, num_sms);
+        const int bn = tc::pick_block_n(Cout, tiles, num_sms, tc::has_block_n_160(mode, 2));
         if (!bn) { err = MI3D_ERR_ARG; return; }
         CUtensorMap ma, mb;
         int r = tc::make_map_nhwc(&ma, x.p, x.c, x.w, x.h, x.n, bw, bh, 1);

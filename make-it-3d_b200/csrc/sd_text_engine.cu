@@ -19,15 +19,8 @@ __global__ void k_layernorm_rows_f32(const __half* __restrict__ x, const float* 
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (row >= B * T) return;
     const __half* xr = x + ((size_t)(row / T) * Tpad + row % T) * C;
-    float s = 0.f, ss = 0.f;
-    for (int c = lane * 8; c < C; c += 256) {
-        const uint4 raw = *reinterpret_cast<const uint4*>(xr + c);
-        const __half* h = reinterpret_cast<const __half*>(&raw);
-        #pragma unroll
-        for (int k = 0; k < 8; k++) { const float v = __half2float(h[k]); s += v; ss += v * v; }
-    }
-    s = sdk::warp_sum(s); ss = sdk::warp_sum(ss);
-    const float mean = s / C, var = fmaxf(ss / C - mean * mean, 0.f), rstd = rsqrtf(var + eps);
+    float mean, rstd;
+    sdk::row_stats(xr, C, eps, lane, mean, rstd);
     float* yr = out + (size_t)row * C;
     for (int c = lane * 8; c < C; c += 256) {
         const uint4 raw = *reinterpret_cast<const uint4*>(xr + c);

@@ -53,11 +53,14 @@ inline int make_map_nhwc(CUtensorMap* map, const __half* base, int C, int W, int
     return make_map_f16(map, base, dims, str, box);
 }
 
-inline int pick_block_n(int N, long long m_tiles_times_batch, int num_sms) {
+// Only the plain kernel has a 160-wide instantiation (launch() below): epilogues PLAIN, GEGLU, TRANSPOSED, conv 0 or 1.
+inline bool has_block_n_160(int epi_mode, int conv) { return conv != 2 && (epi_mode == EPI_PLAIN || epi_mode == EPI_GEGLU || epi_mode == EPI_TRANSPOSED); }
+
+inline int pick_block_n(int N, long long m_tiles_times_batch, int num_sms, bool allow_160 = true) {
     // largest tile that divides N; prefer 256 only when the grid still fills the machine
     if (N % 256 == 0 && m_tiles_times_batch * (N / 256) >= num_sms) return 256;
     if (N % 128 == 0 && m_tiles_times_batch * (N / 128) >= num_sms) return 128;
-    if (N % 160 == 0 && N % 128 != 0 && m_tiles_times_batch * (N / 160) >= num_sms / 2) return 160;   // N = 320: 2.5x the MACs per operand byte of BN = 64
+    if (allow_160 && N % 160 == 0 && N % 128 != 0 && m_tiles_times_batch * (N / 160) >= num_sms / 2) return 160;   // N = 320: 2.5x the MACs per operand byte of BN = 64
     if (N % 64 == 0) return 64;
     return 0;
 }

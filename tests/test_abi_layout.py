@@ -13,7 +13,7 @@ sys.path.insert(0, ROOT)
 PAIRS = [("mi3d_hashgrid", "_lib", "HashGrid"), ("mi3d_raygen", "_lib", "RayGen"), ("mi3d_mlp", "_lib", "Mlp"), ("mi3d_epilogue", "_lib", "Epilogue"),
          ("mi3d_field_cfg", "_lib", "FieldCfg"), ("mi3d_field_io", "_lib", "FieldIO"), ("mi3d_view_segs", "_lib", "ViewSegs"),
          ("mi3d_adan_cfg", "_lib", "AdanCfg"), ("mi3d_render_args", "_lib", "RenderArgs"), ("mi3d_render_eval_args", "_lib", "RenderEvalArgs"),
-         ("mi3d_render_ws", "_lib", "RenderWs"), ("mi3d_unet_cfg", "nerf.sd", "UNetCfg"), ("mi3d_vae_cfg", "nerf.sd", "VaeCfg")]
+         ("mi3d_render_ws", "_lib", "RenderWs"), ("mi3d_op_gemm_args", "_lib", "OpGemmArgs"), ("mi3d_unet_cfg", "nerf.sd", "UNetCfg"), ("mi3d_vae_cfg", "nerf.sd", "VaeCfg")]
 
 
 def test_ctypes_mirrors_match_the_header_layout(tmp_path):
