@@ -396,7 +396,7 @@ int mi3d_gemm_f16_splitk(const void* a, const void* b, void* out, int M, int N, 
                          const float* bias, const void* residual, void* ws, mi3d_stream_t stream);
 
 /* Fused multi-head attention, head_dim 64 (stands in for diffusers' attention processor inside BasicTransformerBlock.attn1 /
- * .attn2, nerf/sd.py:146): o = softmax(q k^T / 8) v per (batch, head), scores kept in registers.
+ * .attn2, nerf/sd.py:146): o = softmax(q k^T / 8) v per (batch, head), scores kept in registers.  Other head dims: mi3d_op_attention_core.
  * q [B*T, ldq], k and v [B*Tk, ldk / ldv], o [B*T, ldo], fp16, head h at columns [64h, 64h+64); only the first Tk_valid keys of
  * every batch take part (77 of the 128 padded text rows for cross attention).  All ld % 8 == 0. */
 int mi3d_flash_attn_f16(const void* q, const void* k, const void* v, void* o, int B, int T, int Tk, int Tk_valid, int heads,
@@ -433,6 +433,12 @@ int mi3d_op_conv3_block(const void* x, const void* w, void* y, int Nimg, int H, 
  * 1 attention_materialised, 2 attention_materialised causal.  Writes o [B*Tpad][C]; modes 1, 2 also need qkvT [B][3C][Tpad] and
  * S [B*heads][Tpad][Tpad] (left holding P). */
 int mi3d_op_attention(const void* qkv, void* qkvT, void* S, void* o, int B, int T, int Tpad, int heads, int mode, mi3d_stream_t stream);
+/* Builder::attention_core as the SD engine calls it: the fused attention for head_dim 40, 64, 80 or 160 (SD-2.x: 64 at every level;
+ * SD-1.x: 40, 80, 160), o = softmax(q k^T / sqrt(head_dim)) v.  q [B*T, ldq], k / v [B*Tk, ldk / ldv], o [B*T, ldo], fp16, head h
+ * at columns [h*head_dim, (h+1)*head_dim); only the first Tk_valid keys of every batch take part.  All ld % 8 == 0.  Any other
+ * head_dim returns MI3D_ERR_ARG. */
+int mi3d_op_attention_core(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* o, long long ldo,
+                           int B, int T, int Tk, int Tk_valid, int heads, int head_dim, mi3d_stream_t stream);
 /* row kernels with the engines' launch geometry: Builder::layernorm, clipk::k_layernorm_bwd (add nullable), Builder::softmax
  * (causal_tq > 0: clipk::k_softmax_causal over [rows / tq][tq][cols]), sdk::k_softmax_bwd, Builder::transpose ([Z][R][C] -> [Z][C][R]) */
 int mi3d_op_layernorm(const void* x, void* y, const float* gamma, const float* beta, int rows, int C, float eps, mi3d_stream_t stream);
@@ -449,12 +455,14 @@ typedef struct {
     int n_levels;             /* len(block_out_channels): 4 for SD-2.0-base; 0 = no U-Net in this engine */
     int block_out[4];         /* 320, 640, 1280, 1280 */
     int layers_per_block;     /* 2 */
-    int heads[4];             /* 5, 10, 20, 20 (head_dim 64) */
-    int cross_dim;            /* 1024 */
+    int heads[4];             /* SD-2.x: 5, 10, 20, 20 (head_dim 64); SD-1.x: 8, 8, 8, 8 (head_dim 40, 80, 160); head_dim 40 / 64 / 80 / 160 */
+    int cross_dim;            /* 1024 (SD-1.x: 768) */
     int ctx_len;              /* 77 text tokens */
     int groups;               /* 32 */
     int latent_hw;            /* 64 (nerf/sd.py:124 always feeds 512x512 -> 64x64 latents) */
     int batch;                /* 2 = [uncond, text] (nerf/sd.py:143) */
+    int proj_conv;            /* transformer proj_in / proj_out: 0 = Linear [C, C] (SD-2.x, use_linear_projection), 1 = 1x1 Conv2d
+                                 [C, C, 1, 1] (SD-1.x); the same GEMM either way, only the registered parameter shape differs */
 } mi3d_unet_cfg;
 
 typedef struct {
@@ -498,17 +506,22 @@ int mi3d_sd_profile(mi3d_engine_t h, int enable, float* gemm_ms_host, int* launc
 int mi3d_sd_profile_dump(mi3d_engine_t h, int enable, float* gemm_ms_host, int* launches_host, const char* dump_path_host);
 
 /* ------------------------------------------------------------------------------------------------------
- * B3': Stable Diffusion 2 text encoder  (replaces transformers' CLIPTextModel behind get_text_embeds, nerf/sd.py:68-85: OpenCLIP
- * ViT-H/14's text tower truncated to 23 layers, as every SD-2.x checkpoint ships it)
+ * B3': Stable Diffusion text encoder  (replaces transformers' CLIPTextModel behind get_text_embeds, nerf/sd.py:68-85: OpenCLIP
+ * ViT-H/14's text tower truncated to 23 layers, as every SD-2.x checkpoint ships it, or OpenAI CLIP ViT-L/14's, as SD-1.x ships it)
  * ------------------------------------------------------------------------------------------------------ */
 typedef struct {
-    int width, layers, heads;  /* 1024, 23, 16 (head_dim 64; MLP width 4 x width, exact-erf GELU) */
+    int width, layers, heads;  /* 1024, 23, 16 (SD-1.x: 768, 12, 12); head_dim 64; MLP width 4 x width */
     int context_len, vocab;    /* 77, 49408 */
     int max_batch;             /* prompts per call (1..8); 2 encodes [negative, positive] in one pass */
 } mi3d_sd_text_cfg;
 
+/* The MLP activation is exact-erf GELU (SD-2.x, OpenCLIP ViT-H/14) */
 size_t mi3d_sd_text_workspace_bytes(const mi3d_sd_text_cfg* cfg);
 mi3d_engine_t mi3d_sd_text_create(const mi3d_sd_text_cfg* cfg, void* workspace, size_t workspace_bytes);
+/* The same engine with the MLP activation chosen by act: 0 = exact-erf GELU (SD-2.x; the two calls above), 1 = quick-GELU
+ * x * sigmoid(1.702 x) (SD-1.x, OpenAI CLIP ViT-L/14's text tower); any other value is invalid (0 bytes / NULL). */
+size_t mi3d_sd_text_act_workspace_bytes(const mi3d_sd_text_cfg* cfg, int act);
+mi3d_engine_t mi3d_sd_text_act_create(const mi3d_sd_text_cfg* cfg, int act, void* workspace, size_t workspace_bytes);
 /* Parameters are enumerated by transformers' CLIPTextModel state_dict names, in its order ("text_model.embeddings.token_embedding.weight"
  * .. "text_model.final_layer_norm.bias"; no position_ids).  The separate q / k / v projections are stored as row slices of one packed
  * weight. */

@@ -115,13 +115,14 @@ SYMBOLS = [
     "mi3d_density_grid_workspace_bytes", "mi3d_density_grid_update", "mi3d_version",
     "mi3d_sumsq_workspace_bytes", "mi3d_sumsq", "mi3d_adan_step",
     "mi3d_gemm_f16", "mi3d_gemm_f16_splitk", "mi3d_flash_attn_f16", "mi3d_conv3x3_f16", "mi3d_tf32_tile_test", "mi3d_gemm_f16_bt",
-    "mi3d_op_gemm", "mi3d_op_conv3", "mi3d_op_conv3_block", "mi3d_op_attention", "mi3d_op_layernorm", "mi3d_op_layernorm_bwd",
+    "mi3d_op_gemm", "mi3d_op_conv3", "mi3d_op_conv3_block", "mi3d_op_attention", "mi3d_op_attention_core", "mi3d_op_layernorm", "mi3d_op_layernorm_bwd",
     "mi3d_op_softmax", "mi3d_op_softmax_bwd", "mi3d_op_transpose",
     "mi3d_engine_destroy", "mi3d_engine_num_params", "mi3d_engine_param_name", "mi3d_engine_param_shape", "mi3d_engine_load_param",
     "mi3d_engine_set_graph_replay", "mi3d_engine_graph_replays", "mi3d_engine_debug_tensor",
     "mi3d_sd_workspace_bytes", "mi3d_sd_create", "mi3d_sd_encode", "mi3d_sd_encode_backward", "mi3d_sd_unet_sds", "mi3d_sd_profile",
     "mi3d_sd_profile_dump", "mi3d_sd_ddim_step", "mi3d_sd_decode",
-    "mi3d_sd_text_workspace_bytes", "mi3d_sd_text_create", "mi3d_sd_text_encode",
+    "mi3d_sd_text_workspace_bytes", "mi3d_sd_text_create", "mi3d_sd_text_act_workspace_bytes", "mi3d_sd_text_act_create",
+    "mi3d_sd_text_encode",
     "mi3d_clip_workspace_bytes", "mi3d_clip_create", "mi3d_clip_encode_image", "mi3d_clip_encode_image_backward", "mi3d_clip_encode_text",
     "mi3d_points_workspace_bytes", "mi3d_points_render_forward", "mi3d_points_render_backward", "mi3d_points_zbuffer_visible",
     "mi3d_cx_workspace_bytes", "mi3d_cx_create", "mi3d_cx_forward", "mi3d_cx_backward",

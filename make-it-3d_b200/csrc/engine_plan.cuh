@@ -269,20 +269,20 @@ struct Builder : mi3d_engine {
     int small_cout_grid(size_t pixels, int cin) const { const int ppw = cin <= 128 ? 2 : 1; return (int)std::min<size_t>((pixels / ppw + 7) / 8 + 1, (size_t)num_sms * 8); }
     static int blocks_for(size_t n) { return (int)std::min<size_t>((n + 255) / 256, 132 * 16); }
 
-    // multi-head attention core on token matrices (attn.cuh).  q: [B*T, ldq] (head h at column h*64), k / v likewise
-    // [B*Tk, ld]; only the first Tk_valid keys of each batch take part.  Writes o [B*T, C].
+    // multi-head attention core on token matrices (attn.cuh).  q: [B*T, ldq] (head h at column h*d), k / v likewise
+    // [B*Tk, ld]; only the first Tk_valid keys of each batch take part.  Writes o [B*T, C].  d: 40, 64, 80 or 160.
     void attention_core(const __half* q, long long ldq, const __half* k, long long ldk, const __half* v, long long ldv, int B, int T, int Tk,
                         int Tk_valid, int heads, int d, __half* o, int C) {
-        if (d != 64) { err = MI3D_ERR_ARG; return; }
+        if (!attn::supported(d)) { err = MI3D_ERR_ARG; return; }
         if (dry) return;
         attn::Maps m;
-        if (int r = attn::make_maps(&m, q, ldq, k, ldk, v, ldv, B, T, Tk, heads)) { err = r; return; }
+        if (int r = attn::make_maps(&m, q, ldq, k, ldk, v, ldv, B, T, Tk, heads, d)) { err = r; return; }
         push([=](cudaStream_t st) {
             if (!profile) return attn::launch(m, o, C, B, T, Tk_valid, heads, st);
             // profiling: same event bracket as the tile kernel; recorded with conv = 2 (M = queries, N = keys, K = head_dim, batch = B * heads)
             if (prof_used == prof_events.size()) { cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b); prof_events.push_back({a, b}); }
             if (prof_shapes.size() < prof_events.size()) prof_shapes.resize(prof_events.size());
-            prof_shapes[prof_used] = {T, Tk_valid, 64, 0, 1, 2, B * heads, 0};
+            prof_shapes[prof_used] = {T, Tk_valid, d, 0, 1, 2, B * heads, 0};
             auto& ev = prof_events[prof_used++];
             cudaEventRecord(ev.first, st);
             const int r = attn::launch(m, o, C, B, T, Tk_valid, heads, st);

@@ -129,7 +129,10 @@ struct Engine : Builder {
         T4 n = act(x.n, x.h, x.w, C);
         groupnorm(x, pre + ".norm", 1e-6f, 0, n);
         __half* h = alloc16(M * C);
-        linear(n.p, M, C, (const __half*)param(pre + ".proj_in.weight", {C, C}, PK_LINEAR).dst, C, h, pf(pre + ".proj_in.bias", {C}));
+        // proj_in / proj_out: Linear [C, C] (SD-2.x) or 1x1 Conv2d [C, C, 1, 1] (SD-1.x), the same [C][C] fp16 matrix either way
+        const std::vector<int> pshape = ucfg.proj_conv ? std::vector<int>{C, C, 1, 1} : std::vector<int>{C, C};
+        const PKind pkind = ucfg.proj_conv ? PK_CONV1 : PK_LINEAR;
+        linear(n.p, M, C, (const __half*)param(pre + ".proj_in.weight", pshape, pkind).dst, C, h, pf(pre + ".proj_in.bias", {C}));
         const std::string tb = pre + ".transformer_blocks.0";
         // ---- self attention ----
         __half* ln = alloc16(M * C);
@@ -181,7 +184,7 @@ struct Engine : Builder {
         __half* h4 = alloc16(M * C);
         linear(f1, M, 4 * C, (const __half*)param(tb + ".ff.net.2.weight", {C, 4 * C}, PK_LINEAR).dst, C, h4, pf(tb + ".ff.net.2.bias", {C}), h3);
         T4 out = act(x.n, x.h, x.w, C);
-        linear(h4, M, C, (const __half*)param(pre + ".proj_out.weight", {C, C}, PK_LINEAR).dst, C, out.p, pf(pre + ".proj_out.bias", {C}), x.p);
+        linear(h4, M, C, (const __half*)param(pre + ".proj_out.weight", pshape, pkind).dst, C, out.p, pf(pre + ".proj_out.bias", {C}), x.p);
         return out;
     }
 

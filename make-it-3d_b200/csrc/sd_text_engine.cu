@@ -1,10 +1,11 @@
-// sd_text_engine.cu -- the Stable Diffusion 2 text encoder (C ABI: include/mi3d.h, section B3').
+// sd_text_engine.cu -- the Stable Diffusion text encoder (C ABI: include/mi3d.h, section B3').
 //
 // What `CLIPTextModel(input_ids)[0]` computes for SD-2.x (nerf/sd.py:68-85): OpenCLIP ViT-H/14's text tower truncated to 23 layers
 // (width 1024, 16 heads of 64, MLP 4096 with exact GELU, causal attention, no padding mask), then final_layer_norm over every one of
-// the 77 positions (last_hidden_state; no EOT pooling, no projection).  A statically planned list of launches: the token embedding
-// (clipk::k_text_embed), the pre-LN blocks of transformer_plan.cuh with the tile GEMM's EPI_GELU epilogue, and a final LayerNorm that
-// writes fp32.  Activations fp16, statistics and accumulation fp32, weights fp16 (the embeddings and LayerNorms fp32).  Forward only
+// the 77 positions (last_hidden_state; no EOT pooling, no projection).  SD-1.x ships OpenAI CLIP ViT-L/14's text tower instead (12
+// layers, width 768, 12 heads of 64, quick-GELU; act = 1), otherwise the same computation.  A statically planned list of
+// launches: the token embedding (clipk::k_text_embed), the pre-LN blocks of transformer_plan.cuh with the tile GEMM's EPI_GELU or
+// EPI_QUICKGELU epilogue, and a final LayerNorm that writes fp32.  Activations fp16, statistics and accumulation fp32, weights fp16 (the embeddings and LayerNorms fp32).  Forward only
 // (the encoder is frozen), so all blocks share one set of activation buffers.  No split-K and no atomics: results are bit-identical
 // run to run, under graph replay, and for a sequence whether it is encoded alone or in a batch.
 #include "transformer_plan.cuh"
@@ -35,7 +36,8 @@ __global__ void k_layernorm_rows_f32(const __half* __restrict__ x, const float* 
 
 struct Engine : TowerBuilder {
     mi3d_sd_text_cfg cfg;
-    explicit Engine(const mi3d_sd_text_cfg& c) : cfg(c) {}
+    int act;                                  // 0: exact GELU, 1: quick-GELU (the MLP epilogue)
+    Engine(const mi3d_sd_text_cfg& c, int a) : cfg(c), act(a) {}
     Tower t;
     std::vector<BlockW> w;
     std::vector<BlockA> a;
@@ -97,7 +99,7 @@ struct Engine : TowerBuilder {
                 clipk::k_text_embed<<<blocks_for((size_t)B * Tp * C / 8), 256, 0, st>>>(tk, tok, pos, x0, B, T, Tp, C, V);
                 return (int)cudaGetLastError();
             });
-            for (int i = 0; i < t.L; i++) block_fwd(t, w[i], a[i], B, 2, tc::EPI_GELU);
+            for (int i = 0; i < t.L; i++) block_fwd(t, w[i], a[i], B, 2, act ? tc::EPI_QUICKGELU : tc::EPI_GELU);
             push([=](cudaStream_t st) {
                 k_layernorm_rows_f32<<<(unsigned)((B * T + 7) / 8), 256, 0, st>>>(r_last, lnf, lnf_b, o, B, T, Tp, C, 1e-5f);
                 return (int)cudaGetLastError();
@@ -117,12 +119,19 @@ bool valid_cfg(const mi3d_sd_text_cfg& c) {
 
 extern "C" {
 
-size_t mi3d_sd_text_workspace_bytes(const mi3d_sd_text_cfg* cfg) {
-    return cfg && sdtext::valid_cfg(*cfg) ? plan::workspace_bytes<sdtext::Engine>(*cfg) : 0;
+size_t mi3d_sd_text_act_workspace_bytes(const mi3d_sd_text_cfg* cfg, int act) {
+    return cfg && sdtext::valid_cfg(*cfg) && (act == 0 || act == 1) ? plan::workspace_bytes<sdtext::Engine>(*cfg, act) : 0;
 }
 
+mi3d_engine_t mi3d_sd_text_act_create(const mi3d_sd_text_cfg* cfg, int act, void* workspace, size_t workspace_bytes) {
+    return cfg && sdtext::valid_cfg(*cfg) && (act == 0 || act == 1) ? plan::create<sdtext::Engine>(workspace, workspace_bytes, *cfg, act)
+                                                                      : nullptr;
+}
+
+size_t mi3d_sd_text_workspace_bytes(const mi3d_sd_text_cfg* cfg) { return mi3d_sd_text_act_workspace_bytes(cfg, 0); }
+
 mi3d_engine_t mi3d_sd_text_create(const mi3d_sd_text_cfg* cfg, void* workspace, size_t workspace_bytes) {
-    return cfg && sdtext::valid_cfg(*cfg) ? plan::create<sdtext::Engine>(workspace, workspace_bytes, *cfg) : nullptr;
+    return mi3d_sd_text_act_create(cfg, 0, workspace, workspace_bytes);
 }
 
 int mi3d_sd_text_encode(mi3d_engine_t h, const long long* ids, int B, float* out, mi3d_stream_t stream) {

@@ -80,7 +80,7 @@ int mi3d_flash_attn_f16(const void* q, const void* k, const void* v, void* o, in
                         int ldq, int ldk, int ldv, int ldo, mi3d_stream_t stream) {
     if (B < 1 || T < 1 || Tk < 1 || Tk_valid < 1 || Tk_valid > Tk || heads < 1 || (ldq | ldk | ldv | ldo) % 8) return MI3D_ERR_ARG;
     attn::Maps m;
-    int r = attn::make_maps(&m, (const __half*)q, ldq, (const __half*)k, ldk, (const __half*)v, ldv, B, T, Tk, heads);
+    int r = attn::make_maps(&m, (const __half*)q, ldq, (const __half*)k, ldk, (const __half*)v, ldv, B, T, Tk, heads, 64);
     if (r) return r;
     return attn::launch(m, (__half*)o, ldo, B, T, Tk_valid, heads, (cudaStream_t)stream);
 }
@@ -135,6 +135,14 @@ int mi3d_op_conv3_block(const void* x, const void* w, void* y, int Nimg, int H, 
     op.b.conv3_block(t4(x, Nimg, H, W, Cin), (const __half*)w, Cout, t4(y, Nimg, H, W, Cout), bias, mode, (const __half*)aux,
                      (const __half*)residual);
     return op.run(stream, plan);
+}
+
+int mi3d_op_attention_core(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* o, long long ldo,
+                           int B, int T, int Tk, int Tk_valid, int heads, int head_dim, mi3d_stream_t stream) {
+    if (B < 1 || T < 1 || Tk < 1 || Tk_valid < 1 || Tk_valid > Tk || heads < 1 || (ldq | ldk | ldv | ldo) % 8) return MI3D_ERR_ARG;
+    OneOp op;
+    op.b.attention_core((const __half*)q, ldq, (const __half*)k, ldk, (const __half*)v, ldv, B, T, Tk, Tk_valid, heads, head_dim, (__half*)o, (int)ldo);
+    return op.run(stream);
 }
 
 int mi3d_op_attention(const void* qkv, void* qkvT, void* S, void* o, int B, int T, int Tpad, int heads, int mode, mi3d_stream_t stream) {

@@ -6,13 +6,17 @@ guidance_scale=10) -> (loss, imgs)` performs the SDS backward itself into pred_r
 engine of csrc/sd_engine.cu (wgmma tile kernel + fused memory-bound kernels); there is no diffusers / cuDNN / cuBLAS
 call and no CPU fallback.
 
-Weights: parameters are enumerated by diffusers' state_dict names; real SD-2.0-base checkpoints load through
+Weights: parameters are enumerated by diffusers' state_dict names; real SD-2.x checkpoints load through
 `load_diffusers_state_dict(unet_state, vae_state)` (which also pushes them into the engine); offline (no network, no weights on disk) they are seeded random tensors with PyTorch's default
 initialisers -- which is what the benchmark and the parity tests use (`data: synthetic`).
+SD-1.x (`sd_version='1.5'`, or `hf_key` of any SD-1.x checkpoint) runs on the same engine with its own topology (`sd15_unet_cfg`: 8 heads
+of 40 / 80 / 160, cross dim 768, 1x1-conv proj_in / proj_out) and needs its checkpoint: pass `unet_state` / `vae_state` (diffusers'
+`UNet2DConditionModel` / `AutoencoderKL` state_dict()s); there is no seeded SD-1.5 stand-in.  Its text encoder (OpenAI CLIP ViT-L/14,
+quick-GELU) is created by `load_diffusers_state_dict(text_encoder_state=...)`.
 The "denoise" side branch (nerf/sd.py:153-159: DDIM step t -> t-1, VAE decode, CLIP losses) is built on the same engine (`mi3d_sd_ddim_step`,
 `mi3d_sd_decode`); the CLIP losses run on the caller-provided clip_model (the reference passes it in too) and are skipped without one.
 A native `nerf.clip.CLIP` computes them on the CLIP engine (csrc/clip_engine.cu, aug included); any other model is called as before.
-`get_text_embeds` runs the SD-2 text encoder (nerf/sd_text.py, csrc/sd_text_engine.cu) once its weights are loaded with
+`get_text_embeds` runs the SD text encoder (nerf/sd_text.py, csrc/sd_text_engine.cu) once its weights are loaded with
 `load_diffusers_state_dict(text_encoder_state=...)`; prompts given as strings go through the `tokenizer` passed to the constructor.
 Without text-encoder weights it returns a deterministic stand-in keyed by the prompt strings.
 """
@@ -32,7 +36,7 @@ from .sd_text import TextEncoder, cfg_from_state_dict
 class UNetCfg(C.Structure):
     _fields_ = [("in_ch", C.c_int), ("out_ch", C.c_int), ("n_levels", C.c_int), ("block_out", C.c_int * 4), ("layers_per_block", C.c_int),
                 ("heads", C.c_int * 4), ("cross_dim", C.c_int), ("ctx_len", C.c_int), ("groups", C.c_int), ("latent_hw", C.c_int),
-                ("batch", C.c_int)]
+                ("batch", C.c_int), ("proj_conv", C.c_int)]
 
 
 class VaeCfg(C.Structure):
@@ -43,6 +47,18 @@ class VaeCfg(C.Structure):
 def sd20_unet_cfg(latent_hw=64):
     return dict(in_channels=4, out_channels=4, block_out=(320, 640, 1280, 1280), layers_per_block=2, heads=(5, 10, 20, 20),
                 cross_dim=1024, groups=32, ctx_len=77, latent_hw=latent_hw)
+
+
+def sd15_unet_cfg(latent_hw=64):
+    """SD-1.x (stable-diffusion-v1-5 unet/config.json): 8 heads at every level (head_dim 40 / 80 / 160), cross dim 768 (OpenAI CLIP
+    ViT-L/14 text features), 1x1-conv proj_in / proj_out (use_linear_projection false)"""
+    return dict(sd20_unet_cfg(latent_hw), heads=(8, 8, 8, 8), cross_dim=768, proj_conv=True)
+
+
+def is_sd1_unet_state(state):
+    """an SD-1.x U-Net state_dict: its transformer projections are 1x1 convs [C, C, 1, 1]"""
+    w = state.get("down_blocks.0.attentions.0.proj_in.weight") if state is not None else None
+    return w is not None and w.dim() == 4
 
 
 def sd_vae_cfg(image_hw=512):
@@ -58,6 +74,7 @@ def _unet_struct(cfg):
         u.heads[i] = v
     u.layers_per_block, u.cross_dim, u.ctx_len, u.groups = cfg["layers_per_block"], cfg["cross_dim"], cfg["ctx_len"], cfg["groups"]
     u.latent_hw, u.batch = cfg["latent_hw"], 2
+    u.proj_conv = 1 if cfg.get("proj_conv", False) else 0
     return u
 
 
@@ -156,15 +173,22 @@ class StableDiffusion(nn.Module):
         self.defer_backward = bool(defer_backward)
         self.device = torch.device(device)
         self.sd_version = sd_version
-        # nerf/sd.py:29-37: '2.1' / '2.0' select stable-diffusion-2-1-base / 2-base, hf_key any other checkpoint (BASELINE config 4 names
-        # SD-2.1-768).  All SD-2.x U-Nets share ONE topology (block_out 320/640/1280/1280, head_dim 64, cross dim 1024, linear
-        # projections) and nerf/sd.py:124 always feeds 512x512 -> 64x64 latents, so they all run on the same engine plan; the 768
-        # checkpoint's v-prediction output is consumed as if it were epsilon, exactly like the reference does (it never reads
-        # prediction_type, nerf/sd.py:146-151).  SD-1.5 (cross dim 768, conv projections, 8 heads) is not built.
-        if sd_version not in ('2.0', '2.1') and hf_key is None and unet_cfg is None:
-            raise ValueError(f'Stable-diffusion version {sd_version} not built (2.0 / 2.1 / hf_key of an SD-2.x checkpoint; reference default 2.0, nerf/sd.py:33-34)')
+        # nerf/sd.py:29-37: '2.1' / '2.0' select stable-diffusion-2-1-base / 2-base, '1.5' stable-diffusion-v1-5, hf_key any other
+        # checkpoint (BASELINE config 4 names SD-2.1-768).  All SD-2.x U-Nets share ONE topology (block_out 320/640/1280/1280, head_dim
+        # 64, cross dim 1024, linear projections) and all SD-1.x U-Nets another (the same channels, 8 heads of 40 / 80 / 160, cross dim
+        # 768, 1x1-conv projections); nerf/sd.py:124 always feeds 512x512 -> 64x64 latents, so each family runs on one engine plan.  An
+        # hf_key checkpoint is SD-1.x when its unet_state has conv projections.  The 768 checkpoint's v-prediction output is consumed
+        # as if it were epsilon, exactly like the reference does (it never reads prediction_type, nerf/sd.py:146-151).  SD-1.x needs its
+        # checkpoint: the seeded stand-in exists for SD-2.0 only (the benchmark's synthetic workload), so a missing SD-1.5 unet_state
+        # is an error rather than silently random weights.
+        sd1 = unet_cfg is None and (sd_version == '1.5' or is_sd1_unet_state(unet_state))
+        if sd1 and unet_state is None:
+            raise ValueError('Stable-diffusion 1.5 needs its checkpoint: pass the U-Net / VAE state dicts (unet_state=, vae_state=: '
+                             'diffusers UNet2DConditionModel / AutoencoderKL state_dict()s); there is no synthetic SD-1.5')
+        if sd_version not in ('1.5', '2.0', '2.1') and hf_key is None and unet_cfg is None:
+            raise ValueError(f'Stable-diffusion version {sd_version} not built (1.5 / 2.0 / 2.1 / hf_key of an SD-1.x or SD-2.x checkpoint; reference default 2.0, nerf/sd.py:33-34)')
         self.hf_key = hf_key
-        self.unet_cfg = unet_cfg or sd20_unet_cfg()
+        self.unet_cfg = unet_cfg or (sd15_unet_cfg() if sd1 else sd20_unet_cfg())
         self.vae_cfg = vae_cfg or sd_vae_cfg()
         self.engine = SDEngine(self.unet_cfg, self.vae_cfg, self.device, graph_replay=graph_replay)
         gen = torch.Generator().manual_seed(seed)
@@ -191,11 +215,13 @@ class StableDiffusion(nn.Module):
 
     def load_diffusers_state_dict(self, unet_state=None, vae_state=None, text_encoder_state=None):
         """copy tensors named like diffusers' UNet2DConditionModel / AutoencoderKL state_dict()s and push them to the engine;
-        text_encoder_state (transformers' CLIPTextModel.state_dict()) goes into the SD-2 text encoder, created on first use."""
+        text_encoder_state (transformers' CLIPTextModel.state_dict()) goes into the SD text encoder, created on first use (quick-GELU
+        when the U-Net is SD-1.x, exact GELU for SD-2.x)."""
         if text_encoder_state is not None:
             if self.text_encoder is None:
-                self.text_encoder = TextEncoder(self.device, cfg=cfg_from_state_dict(text_encoder_state), state_dict=text_encoder_state,
-                                                graph_replay=self.graph_replay)
+                act = "quick_gelu" if self.unet_cfg.get("proj_conv", False) else "gelu"
+                self.text_encoder = TextEncoder(self.device, cfg=cfg_from_state_dict(text_encoder_state, hidden_act=act),
+                                                state_dict=text_encoder_state, graph_replay=self.graph_replay)
             else:
                 self.text_encoder.load_state_dict(text_encoder_state)
             if unet_state is None and vae_state is None:
@@ -215,7 +241,7 @@ class StableDiffusion(nn.Module):
 
     def get_text_embeds(self, prompt, negative_prompt):
         """nerf/sd.py:68-85: [uncond, cond] text embeddings [2,77,D].  prompt / negative_prompt: a string, a list of one string, or
-        int64 token ids [1,77] / [77].  With text-encoder weights loaded both run through the SD-2 text encoder in one batch of 2;
+        int64 token ids [1,77] / [77].  With text-encoder weights loaded both run through the SD text encoder in one batch of 2;
         strings need the tokenizer (the prompt is truncated to 77 tokens, the negative prompt is not, as in the reference).
         Without them a deterministic stand-in keyed by the prompt strings keeps the call surface."""
         if self.text_encoder is None:

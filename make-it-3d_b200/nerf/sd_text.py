@@ -1,9 +1,11 @@
-"""B3' seam: the Stable Diffusion 2 text encoder (`CLIPTextModel.from_pretrained(model_key, subfolder="text_encoder")`, nerf/sd.py:42)
+"""B3' seam: the Stable Diffusion text encoder (`CLIPTextModel.from_pretrained(model_key, subfolder="text_encoder")`, nerf/sd.py:42)
 on libmi3d.so.
 
 `TextEncoder(device, cfg=None, state_dict=None, graph_replay=True, max_batch=2)` runs OpenCLIP ViT-H/14's text tower as SD-2.x ships it
-(23 layers, width 1024) in the engine of csrc/sd_text_engine.cu (tile GEMM with an exact-GELU epilogue, materialised causal attention,
-fused memory-bound kernels); there is no CPU or eager-PyTorch fallback.
+(23 layers, width 1024, exact GELU; `sd2_text_cfg()`) or OpenAI CLIP ViT-L/14's text tower as SD-1.x ships it (12 layers, width 768,
+quick-GELU; `sd15_text_cfg()`) in the engine of csrc/sd_text_engine.cu (tile GEMM with the activation in its epilogue, materialised
+causal attention, fused memory-bound kernels); there is no CPU or eager-PyTorch fallback.  `cfg["hidden_act"]` takes transformers'
+names, "gelu" (the default) or "quick_gelu"; a state dict does not record it, so `cfg_from_state_dict` takes it as an argument.
 
 * Weights are named like transformers' `CLIPTextModel.state_dict()`, so `load_state_dict(text_encoder.state_dict())` of a diffusers SD-2
   checkpoint loads directly (`text_model.embeddings.position_ids` is ignored when present).  Each tensor passes through the device on
@@ -24,27 +26,43 @@ class SdTextCfg(C.Structure):
                 ("max_batch", C.c_int)]
 
 
+ACTS = {"gelu": 0, "quick_gelu": 1}     # transformers' hidden_act -> the act argument of mi3d_sd_text_act_create
+
+
 def sd2_text_cfg():
     """SD-2.0-base / 2.1-base / 2.1 text_encoder/config.json"""
-    return dict(width=1024, layers=23, heads=16, context_len=77, vocab=49408)
+    return dict(width=1024, layers=23, heads=16, context_len=77, vocab=49408, hidden_act="gelu")
 
 
-def cfg_from_state_dict(state_dict):
-    """the encoder's shape read off a CLIPTextModel state_dict (head_dim 64, as in every SD-2.x checkpoint)"""
+def sd15_text_cfg():
+    """SD-1.5 (and every SD-1.x) text_encoder/config.json: OpenAI CLIP ViT-L/14's text tower"""
+    return dict(width=768, layers=12, heads=12, context_len=77, vocab=49408, hidden_act="quick_gelu")
+
+
+def cfg_from_state_dict(state_dict, hidden_act="gelu"):
+    """the encoder's shape read off a CLIPTextModel state_dict (head_dim 64, as in every SD-1.x / SD-2.x checkpoint); the activation
+    is not in the state dict: "gelu" for SD-2.x, "quick_gelu" for SD-1.x"""
+    if hidden_act not in ACTS:
+        raise L.Mi3dError(f"hidden_act must be one of {sorted(ACTS)}; got {hidden_act!r}")
     tok = state_dict["text_model.embeddings.token_embedding.weight"]
     layers = {k.split(".")[3] for k in state_dict if k.startswith("text_model.encoder.layers.")}
     return dict(width=tok.shape[1], layers=len(layers), heads=tok.shape[1] // 64,
-                context_len=state_dict["text_model.embeddings.position_embedding.weight"].shape[0], vocab=tok.shape[0])
+                context_len=state_dict["text_model.embeddings.position_embedding.weight"].shape[0], vocab=tok.shape[0],
+                hidden_act=hidden_act)
 
 
 class TextEncoder(L.Engine):
     def __init__(self, device, cfg=None, state_dict=None, graph_replay=True, max_batch=2):
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise L.Mi3dError("the SD-2 text encoder runs on sm_90a only; there is no CPU fallback")
+            raise L.Mi3dError("the SD text encoder runs on sm_90a only; there is no CPU fallback")
         self.cfg = dict(cfg or sd2_text_cfg())
+        act = self.cfg.setdefault("hidden_act", "gelu")
+        if act not in ACTS:
+            raise L.Mi3dError(f"hidden_act must be one of {sorted(ACTS)}; got {act!r}")
         self.struct = SdTextCfg(*(int(self.cfg[k]) for k, _ in SdTextCfg._fields_[:-1]), int(max_batch))
-        super().__init__("sd_text", (C.byref(self.struct),), self.device, graph_replay,
+        self.act = ACTS[act]
+        super().__init__("sd_text_act", (C.byref(self.struct), C.c_int(self.act)), self.device, graph_replay,
                          f"SD text encoder configuration {self.cfg} with max_batch={max_batch}")
         self.load_state_dict(state_dict if state_dict is not None else _default_state(self.names, self.shapes))
 
