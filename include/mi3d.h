@@ -741,6 +741,44 @@ int mi3d_mc_emit(const float* volume, uint32_t nx, uint32_t ny, uint32_t nz, flo
 int mi3d_mesh_atlas_texels(const float* vertices, const int* faces, uint32_t F, uint32_t T, uint32_t c, uint32_t n, float bound,
                            float* points, int* owner, float* vt, mi3d_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------
+ * B11: refine loop glue  (the per-iteration losses and the optimiser step of Trainer.refine, nerf/utils.py:865-894; csrc/refine.cu,
+ * oracle/refine_ref.py)
+ * ------------------------------------------------------------------------------------------------------ */
+/* Image losses of one S x S iteration.  weights fp32 [S,S,ppp]: the scale-0 composite weights mi3d_points_render_forward writes;
+ * coverage (nullable) fp32 [S,S] = sum over the ppp slots in slot order, bit-identical to the unit-colour render; dilated fp32 [S,S] =
+ * its 5x5 max (MaxPool2d(5, 1, 2)); pred, gt fp32 [1,3,S,S], gt_mask fp32 [1,1,S,S] (gt and gt_mask may be NULL when front == 0).
+ * losses fp32 [2] (DEVICE) = (1e-3 * sum(1 - pred (1 - dilated)), front ? 1000 * mean|pred m - gt m| : 0), each summed in fp64 in a
+ * fixed order (run-to-run identical).  workspace: mi3d_refine_image_losses_workspace_bytes(S) bytes. */
+size_t mi3d_refine_image_losses_workspace_bytes(uint32_t S);
+int mi3d_refine_image_losses(const float* weights, uint32_t S, uint32_t ppp, const float* pred, const float* gt, const float* gt_mask,
+                             int front, float* coverage, float* dilated, float* losses, void* workspace, size_t workspace_bytes,
+                             mi3d_stream_t stream);
+/* grad_pred fp32 [1,3,S,S] (overwritten) = d(g0 losses[0] + g1 losses[1]) / d pred with grad_losses = (g0, g1) (DEVICE fp32 [2]) and
+ * the dilated mask of the forward, in the operation order of torch's autograd for the same expressions. */
+int mi3d_refine_image_losses_backward(const float* pred, const float* gt, const float* gt_mask, const float* dilated, uint32_t S, int front,
+                                      const float* grad_losses, float* grad_pred, mi3d_stream_t stream);
+/* One parameter tensor of mi3d_refine_adam: n fp32 elements of param / grad / exp_avg / exp_avg_sq (DEVICE), at element `offset` of the
+ * concatenation of all segments (offsets ascending, segment 0 at 0, no gaps). */
+typedef struct {
+    float* param;
+    const float* grad;
+    float* exp_avg;
+    float* exp_avg_sq;
+    unsigned long long offset, n;
+} mi3d_adam_segment;
+/* One torch.optim.Adam step (amsgrad off, no weight decay; `step` counts from 1) over every segment of the DEVICE table segs [n_segs]
+ * (1..256, total elements in all), in torch's operation order: exp_avg.lerp_(g, 1 - beta1), exp_avg_sq.mul_(beta2).addcmul_(g, g,
+ * 1 - beta2), param.addcdiv_(exp_avg, sqrt(exp_avg_sq) / (1 - beta2^step)^0.5 + eps, -lr / (1 - beta1^step)).
+ * origin (nullable) fp32 [p_cano + p_novel, 3]: segment 0 is then the refine cloud's [p_cano + p_novel, 19] buffer (cano rows first)
+ * and its colour columns 0..2 take the gradient of w_cano MSE(colour_cano, origin_cano) + w_novel MSE(colour_novel, origin_novel)
+ * on top of grad; reg (DEVICE fp32 [1]) gets that value for the parameters before the step (an empty region contributes 0).
+ * workspace: mi3d_refine_adam_workspace_bytes(total) bytes, needed with origin only. */
+size_t mi3d_refine_adam_workspace_bytes(unsigned long long total);
+int mi3d_refine_adam(const mi3d_adam_segment* segs, int n_segs, unsigned long long total, double lr, double beta1, double beta2, double eps,
+                     int step, const float* origin, uint32_t p_cano, uint32_t p_novel, double w_cano, double w_novel, float* reg,
+                     void* workspace, size_t workspace_bytes, mi3d_stream_t stream);
+
 /* unit-test entry for the hand-written wgmma tf32 tiles of the field forward (3-term split, K-major operands):
  * mode 0 (the only one): d[128,N] = a[128,K] . b[N,K]^T, N in {16, 32, 64}, K in {32, 64, 96, 128}.  fp32 in/out. */
 int mi3d_tf32_tile_test(const float* a, const float* b, float* d, int N, int K, int mode, mi3d_stream_t stream);

@@ -98,6 +98,12 @@ class OpGemmArgs(C.Structure):
                 ("mode", C.c_int), ("alpha", C.c_float), ("aux", C.c_void_p)]
 
 
+class AdamSegment(C.Structure):
+    """mi3d_adam_segment: one parameter tensor of mi3d_refine_adam"""
+    _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p),
+                ("offset", C.c_ulonglong), ("n", C.c_ulonglong)]
+
+
 RENDER_PHASE_MARCH, RENDER_PHASE_SHADE, RENDER_PHASE_ALL = 1, 2, 3
 
 SHADING = {"albedo": 0, "lambertian": 1, "textureless": 2, "normal": 3}
@@ -132,6 +138,8 @@ SYMBOLS = [
     "mi3d_stream_gemm_workspace_bytes", "mi3d_stream_gemm_f16",
     "mi3d_mc_workspace_bytes", "mi3d_mc_count", "mi3d_mc_emit", "mi3d_mesh_atlas_texels",
     "mi3d_views_workspace_bytes", "mi3d_views_mask", "mi3d_views_cover_mask", "mi3d_views_backproject", "mi3d_views_compact_colour",
+    "mi3d_refine_image_losses_workspace_bytes", "mi3d_refine_image_losses", "mi3d_refine_image_losses_backward",
+    "mi3d_refine_adam_workspace_bytes", "mi3d_refine_adam",
 ]
 
 

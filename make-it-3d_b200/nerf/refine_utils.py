@@ -5,6 +5,8 @@
   Returns `[1, C, h, w]` with a gradient for `points_color` only (the reference never asks for one on the points; `bg_feat` is
   accepted and ignored, as there).  Projection, rasterisation and compositing are fused in csrc/points.cu; the host never
   synchronises.
+* `render_point_weights(...)`: `render_point` with the same arguments that also returns the composite weights `[h, w, ppp]` it
+  saved for its backward (the refine loop derives its coverage mask from them instead of rasterising the cloud again).
 * `rasterize_points(points_xyz_org, H, W, K, world2cam, image_size, radius, ppp)`: pytorch3d's `(idx [1,h,w,K] int32, zbuf, dists)`
   for the same projected cloud, for hosts that composite themselves.
 * `z_buffer(vertices, world2cam_pose_cano, H, W, K)`: numpy in, numpy bool mask out, as the reference; runs in fp64 on the GPU.
@@ -92,6 +94,31 @@ def render_point(points_xyz_org, points_color, H, W, K, world2cam, image_size, r
     pts = L.f32c(points_xyz_org)
     feats = points_color if points_color.dtype == torch.float32 else points_color.float()
     return _RenderPoint.apply(pts, feats.contiguous(), k, rt, float(H), float(W), S, float(radius), int(ppp))
+
+
+class _RenderPointWeights(_RenderPoint):
+    """_RenderPoint that also returns its composite weights (no gradient through them)"""
+
+    @staticmethod
+    def forward(ctx, points, feats, k, rt, H, W, S, radius, ppp):
+        image, idx, wts, _, _ = _forward(points, feats, k, rt, H, W, S, radius, ppp, True, False)
+        ctx.save_for_backward(points, k, rt, idx, wts)
+        ctx.args = (H, W, S, radius, ppp, feats.shape[1])
+        ctx.mark_non_differentiable(wts)
+        return image, wts
+
+    @staticmethod
+    def backward(ctx, grad_image, grad_wts):
+        return _RenderPoint.backward(ctx, grad_image)
+
+
+def render_point_weights(points_xyz_org, points_color, H, W, K, world2cam, image_size, radius, ppp):
+    """(render_point(...) with the same arguments, its composite weights fp32 [h, w, ppp]); summing a pixel's weights in slot order
+    gives, bit for bit, the image render_point makes with unit colours"""
+    S = _check(points_xyz_org, points_color, image_size)
+    k, rt = _cam32(K, world2cam)
+    feats = points_color if points_color.dtype == torch.float32 else points_color.float()
+    return _RenderPointWeights.apply(L.f32c(points_xyz_org), feats.contiguous(), k, rt, float(H), float(W), S, float(radius), int(ppp))
 
 
 def rasterize_points(points_xyz_org, H, W, K, world2cam, image_size, radius, ppp):
