@@ -779,6 +779,36 @@ int mi3d_refine_adam(const mi3d_adam_segment* segs, int n_segs, unsigned long lo
                      int step, const float* origin, uint32_t p_cano, uint32_t p_novel, double w_cano, double w_novel, float* reg,
                      void* workspace, size_t workspace_bytes, mi3d_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------
+ * B12: coarse loop glue  (the per-iteration losses of Trainer.train_step, nerf/utils.py:491-493, :519-533, :551-556;
+ * csrc/coarse.cu, oracle/coarse_ref.py)
+ * ------------------------------------------------------------------------------------------------------ */
+/* Losses of one h x w training render (h, w >= 2).  image fp32 [h*w,3] (ray-major, as the renderer returns it), depth fp32 [h*w]
+ * (may be NULL when front == 0), weights_sum fp32 [h*w]; ref_rgba fp32 [1,4,512,512]; bg_color fp32 [3] (DEVICE); depth_prior fp64
+ * [512,512] and depth_mask uint8 [512,512] (nonzero = pixel used by the depth term; both may be NULL when front == 0).
+ * up = bilinear upsample to 512 x 512 with align_corners=True and torch's fp32 source-index arithmetic.
+ * Writes pred512 = up(image) and gt512 = ref[:3] alpha + bg (1 - alpha), fp32 [1,3,512,512], and terms fp32 [4] (DEVICE):
+ *   terms[0] = mean(ws^2); terms[1] = mean(-a log2 a - (1-a) log2(1-a)), a = clamp(ws, 1e-5, 1-1e-5);
+ *   terms[2] = front ? mean|pred512 - gt512| over 3 * 512^2 : 0;
+ *   terms[3] = front ? clamp(cov(x, y) / sqrt(var x var y), -1, 1) : 0 over the masked pixels, x = nan_to_num(up(depth)), y = the
+ *              prior (two-pass fp64; fewer than 2 masked pixels give NaN).
+ * Every sum is fp64 with per-CTA partials folded in a fixed order (run-to-run identical).  workspace:
+ * mi3d_coarse_losses_workspace_bytes(h, w) bytes (0: invalid size); it also carries what the backward reads, so it must stay
+ * untouched between a forward and its backward. */
+size_t mi3d_coarse_losses_workspace_bytes(uint32_t h, uint32_t w);
+int mi3d_coarse_losses(const float* image, const float* depth, const float* weights_sum, uint32_t h, uint32_t w, const float* ref_rgba,
+                       const float* bg_color, const double* depth_prior, const uint8_t* depth_mask, int front, float* pred512, float* gt512,
+                       float* terms, void* workspace, size_t workspace_bytes, mi3d_stream_t stream);
+/* Gradients of g . terms + <grad_pred512, pred512> with grad_terms = g (DEVICE fp32 [4]) and grad_pred512 fp32 [1,3,512,512]
+ * (nullable), given the forward's pred512, gt512, prior, mask and workspace: grad_image [h*w,3], grad_depth [h*w] and
+ * grad_weights_sum [h*w] (overwritten).  The upsample's adjoint is a gather in a fixed order (no atomics: bitwise repeatable);
+ * nan_to_num passes no gradient where up(depth) was not finite, the clamps pass it at their bounds inclusive (and nowhere for a NaN
+ * coefficient). */
+int mi3d_coarse_losses_backward(const float* weights_sum, uint32_t h, uint32_t w, const float* pred512, const float* gt512,
+                                const double* depth_prior, const uint8_t* depth_mask, int front, const float* grad_terms,
+                                const float* grad_pred512, const void* workspace, size_t workspace_bytes, float* grad_image,
+                                float* grad_depth, float* grad_weights_sum, mi3d_stream_t stream);
+
 /* unit-test entry for the hand-written wgmma tf32 tiles of the field forward (3-term split, K-major operands):
  * mode 0 (the only one): d[128,N] = a[128,K] . b[N,K]^T, N in {16, 32, 64}, K in {32, 64, 96, 128}.  fp32 in/out. */
 int mi3d_tf32_tile_test(const float* a, const float* b, float* d, int N, int K, int mode, mi3d_stream_t stream);

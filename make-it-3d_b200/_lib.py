@@ -140,6 +140,7 @@ SYMBOLS = [
     "mi3d_views_workspace_bytes", "mi3d_views_mask", "mi3d_views_cover_mask", "mi3d_views_backproject", "mi3d_views_compact_colour",
     "mi3d_refine_image_losses_workspace_bytes", "mi3d_refine_image_losses", "mi3d_refine_image_losses_backward",
     "mi3d_refine_adam_workspace_bytes", "mi3d_refine_adam",
+    "mi3d_coarse_losses_workspace_bytes", "mi3d_coarse_losses", "mi3d_coarse_losses_backward",
 ]
 
 

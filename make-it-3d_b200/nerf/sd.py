@@ -342,9 +342,11 @@ class StableDiffusion(nn.Module):
         return noise_pred, grad
 
     def train_step(self, text_embeddings, pred_rgb, ref_rgb=None, noise=None, islarge=False, ref_text=None, clip_model=None,
-                   guidance_scale=10, t=None, eps_posterior=None):
+                   guidance_scale=10, t=None, eps_posterior=None, defer=None):
         """nerf/sd.py:117-174.  `noise` is accepted and ignored like the reference (:140) unless `t` is also injected
-        (additive test hook: t, eps_posterior, noise make the step deterministic)."""
+        (additive test hook: t, eps_posterior, noise make the step deterministic).  `defer` overrides the constructor's
+        defer_backward for this call (None keeps it)."""
+        defer = self.defer_backward if defer is None else bool(defer)
         loss, imgs = 0, None
         if t is None:
             t_host = int(torch.randint(self.min_step, self.max_step + 1, [1]).item())     # CPU generator: no device sync
@@ -352,7 +354,7 @@ class StableDiffusion(nn.Module):
         else:
             t_host = int(t)
         self._t.fill_(t_host)
-        if self.defer_backward and not (not islarge and (t_host / self.num_train_timesteps) <= 0.4):
+        if defer and not (not islarge and (t_host / self.num_train_timesteps) <= 0.4):
             with torch.no_grad():
                 hw = self.vae_cfg["image_hw"] // 8
                 eps = L.f32c(eps_posterior) if eps_posterior is not None else torch.randn(1, 4, hw, hw, device=self.device)
