@@ -1045,20 +1045,51 @@ constexpr size_t kSmem = 1024 + oMisc + 3072;
 // 0.2: ~2 k occupied cells at level 5).
 constexpr float kAggScaleMax = 100.f;
 
-// column-wise sum over the 32 lanes of a warp of v[0..31]; lane j returns the total of column j (recursive halving, 31 shuffles)
-__device__ __forceinline__ float warp_colsum32(float (&v)[32], int lane) {
+// one halving step of warp_colsum32: columns i and i + N of lanes L and L ^ N fold into column i
+template <int N>
+__device__ __forceinline__ void colsum_step(float (&v)[32], int lane) {
+    const bool up = (lane & N) != 0;
     #pragma unroll
-    for (int n = 16; n >= 1; n >>= 1) {
-        const bool up = (lane & n) != 0;
-        #pragma unroll
-        for (int i = 0; i < n; i++) {
-            const float keep = up ? v[i + n] : v[i], send = up ? v[i] : v[i + n];
-            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, n);
-        }
+    for (int i = 0; i < N; i++) {
+        const float keep = up ? v[i + N] : v[i], send = up ? v[i] : v[i + N];
+        v[i] = keep + __shfl_xor_sync(0xffffffffu, send, N);
     }
+}
+
+// column-wise sum over the 32 lanes of a warp of v[0..31]; lane j returns the total of column j (recursive halving, 31 shuffles).
+// The steps are spelled out: a `for (n = 16; n >= 1; n >>= 1)` loop is not unrolled, and its variable inner trip count puts v
+// in local memory.
+__device__ __forceinline__ float warp_colsum32(float (&v)[32], int lane) {
+    colsum_step<16>(v, lane); colsum_step<8>(v, lane); colsum_step<4>(v, lane); colsum_step<2>(v, lane); colsum_step<1>(v, lane);
     return v[0];
 }
+
+// The owners' column loops below run twice (`#pragma unroll 1`, c0 = 0, 32).  State kept per 32-column half is a register pair that
+// each pass updates at [0] and then rotates, so after both passes [0] / [1] hold the halves c0 = 0 / 32: indexing it by c0 instead
+// would place it in local memory.
+template <typename V>
+__device__ __forceinline__ void rot2(V (&v)[2]) { const V t = v[0]; v[0] = v[1]; v[1] = t; }
 }  // namespace bwdtc
+
+// Per-role cycle breakdown of k_field_bwd_tc (tools/prof_field_bwd.py builds a separate library with -DMI3D_FIELD_BWD_CLOCKS).
+// Each thread sums clock64() intervals in registers; lane 0 of every warp adds its totals to g_field_bwd_clocks[slot] at the end:
+//   0 owners: total   1 owners: waiting on stg_full
+//   2 MMA: total      3 MMA: waiting on a1..a4_full
+//   4 encoders: total 5 encoders: waiting on d4_full   6 encoders: scattering
+//   7 evaluations run (one add per CTA)
+// Without the switch the macros expand to nothing.
+#ifdef MI3D_FIELD_BWD_CLOCKS
+__device__ unsigned long long g_field_bwd_clocks[8];
+#define BWD_CLK_VAR(v) long long v = 0
+#define BWD_CLK_T(t) const long long t = clock64()
+#define BWD_CLK_ACC(v, t) v += clock64() - t
+#define BWD_CLK_FLUSH(slot, v) do { if (lane == 0) atomicAdd(&g_field_bwd_clocks[slot], (unsigned long long)(v)); } while (0)
+#else
+#define BWD_CLK_VAR(v)
+#define BWD_CLK_T(t)
+#define BWD_CLK_ACC(v, t)
+#define BWD_CLK_FLUSH(slot, v)
+#endif
 
 __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdArgs a) {
     using namespace bwdtc;
@@ -1124,8 +1155,11 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
         const int r = tid;
         const float* stg = reinterpret_cast<const float*>(sm + oStg);
         uint32_t su = 0;                     // staging hand-offs taken so far (mbarrier phase)
+        BWD_CLK_T(clk_role); BWD_CLK_VAR(clk_wait);
         auto stg_take = [&](uint32_t (&v)[32]) {
+            BWD_CLK_T(t0);
             tc::mbar_wait(stg_full, su & 1u);
+            BWD_CLK_ACC(clk_wait, t0);
             stg_row32(stg + r * kStgLd, v);
             mbar_arrive(stg_empty);
             su++;
@@ -1158,8 +1192,10 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                 float dO[4] = {0.f, 0.f, 0.f, 0.f};
                 if (e == 0) { dO[0] = dh[0]; dO[1] = dh[1]; dO[2] = dh[2]; dO[3] = dh[3]; }
                 else {
+                    // dtap[e - 1], taken from the front: a select on e would be compiled to an indexed load from local memory
+                    dO[0] = dtap[0];
                     #pragma unroll
-                    for (int i = 0; i < 12; i++) if (i == e - 1) dO[0] = dtap[i];
+                    for (int i = 0; i < 11; i++) dtap[i] = dtap[i + 1];
                 }
                 uint32_t m1[2] = {0u, 0u};
                 // ---- epilogue 1: H1 = relu(D1 + b1) -> A2 ; remember the ReLU mask ----
@@ -1178,7 +1214,7 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                         const uint32_t o = oH + sw_off16(r, c0 + 8 * q);
                         *reinterpret_cast<uint4*>(sm + o) = ph; *reinterpret_cast<uint4*>(sm + o + kTile) = pm; *reinterpret_cast<uint4*>(sm + o + 2 * kTile) = pl;
                     }
-                    m1[c0 >> 5] = mk;
+                    m1[0] = mk; rot2(m1);
                 }
                 tc::fence_proxy_async();
                 mbar_arrive(a2_full);
@@ -1207,21 +1243,23 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                         const uint32_t o = oZ + sw_off16(r, c0 + 8 * q);
                         *reinterpret_cast<uint4*>(sm + o) = ph; *reinterpret_cast<uint4*>(sm + o + kTile) = pm; *reinterpret_cast<uint4*>(sm + o + 2 * kTile) = pl;
                     }
-                    ab2[c0 >> 5] += warp_colsum32(tv, lane);          // db2 (tv is dead after the stores above)
+                    ab2[0] += warp_colsum32(tv, lane); rot2(ab2);      // db2 (tv is dead after the stores above)
                     // dW3[o][c0 + lane] += sum over this warp's rows of dO[o] * H2[.][c0 + lane]
                     {
                         float t[32];
                         #pragma unroll
                         for (int j = 0; j < 32; j++) t[j] = dO[0] * h2[j];
-                        aw3[0][c0 >> 5] += warp_colsum32(t, lane);
+                        aw3[0][0] += warp_colsum32(t, lane);
                         if (e == 0) {
                             #pragma unroll
                             for (int o = 1; o < 4; o++) {
                                 #pragma unroll
                                 for (int j = 0; j < 32; j++) t[j] = dO[o] * h2[j];
-                                aw3[o][c0 >> 5] += warp_colsum32(t, lane);
+                                aw3[o][0] += warp_colsum32(t, lane);
                             }
                         }
+                        #pragma unroll
+                        for (int o = 0; o < 4; o++) rot2(aw3[o]);
                     }
                 }
                 tc::fence_proxy_async();
@@ -1240,7 +1278,7 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                 for (int c0 = 0; c0 < D_H; c0 += 32) {
                     uint32_t v[32];
                     stg_take(v);
-                    const uint32_t mk = m1[c0 >> 5];
+                    const uint32_t mk = m1[0]; rot2(m1);
                     float tv[32];
                     #pragma unroll
                     for (int j = 0; j < 32; j++) tv[j] = (mk >> j) & 1u ? __uint_as_float(v[j]) : 0.f;
@@ -1251,7 +1289,7 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                         const uint32_t o = oZ + sw_off16(r, c0 + 8 * q);
                         *reinterpret_cast<uint4*>(sm + o) = ph; *reinterpret_cast<uint4*>(sm + o + kTile) = pm; *reinterpret_cast<uint4*>(sm + o + 2 * kTile) = pl;
                     }
-                    ab1[c0 >> 5] += warp_colsum32(tv, lane);          // db1
+                    ab1[0] += warp_colsum32(tv, lane); rot2(ab1);      // db1
                 }
                 tc::fence_proxy_async();
                 mbar_arrive(a4_full);
@@ -1263,85 +1301,111 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
         if (lane < 4) atomicAdd(a.g_mlp.b3 + lane, ab3);
         atomicAdd(a.g_mlp.b2 + lane, ab2[0]); atomicAdd(a.g_mlp.b2 + 32 + lane, ab2[1]);
         atomicAdd(a.g_mlp.b1 + lane, ab1[0]); atomicAdd(a.g_mlp.b1 + 32 + lane, ab1[1]);
+        BWD_CLK_FLUSH(0, clock64() - clk_role); BWD_CLK_FLUSH(1, clk_wait);
     } else if (warp < 12) {
         // ================================ encoders / scatterers ================================
         asm volatile("setmaxnreg.dec.sync.aligned.u32 96;");
         const int et = tid - 128, r = et & (T - 1), half = et >> 7;
         const float* denc = reinterpret_cast<const float*>(sm + oZ);
         const bool ext = a.enc_buf != nullptr;
-        for (uint32_t tile = a.tile0 + blockIdx.x; tile < a.tile1 && (uint64_t)tile * T < m_pad; tile += gridDim.x) {
-            const uint32_t row = tile * T + r;
-            const RowInfo ri = row_info(R, row);
-            const bool in_range = ri.in_range, real = ri.real;
-            float x[3] = {0.f, 0.f, 0.f}, xp[3] = {0.f, 0.f, 0.f};
-            if (real) { x[0] = a.xyzs[3 * (size_t)row]; x[1] = a.xyzs[3 * (size_t)row + 1]; x[2] = a.xyzs[3 * (size_t)row + 2]; }
-            if (a.n_evals > 7 && in_range) {
-                float z[3];
-                smooth_z(a.smooth_noise, a.seed, a.noise_mode, row, ri, x, z);
-                #pragma unroll
-                for (int c = 0; c < 3; c++) xp[c] = x[c] + z[c] * kSmoothStd;
+        // One stream of evaluations over this CTA's tiles, (tile, e) in order, counted by `it` like the owners and the MMA warpgroup.
+        // Software pipeline with ping-pong E: the encoding uses 32 of the tile's 64 columns, so evaluation `it` lives in columns
+        // 32 (it & 1) .. + 31 (operand start address + 64 B).  E(it+2) is written at the END of iteration `it` (its half was last read
+        // by chain(it), retired at d4(it)), after the scatter of dEnc(it) under which its gather loads were in flight; chain(it+1) then
+        // starts the moment chain(it) retires -- the MMA warp has already seen a1(it+1).  The fetch cursor runs two evaluations ahead
+        // of the scatter across tile boundaries, so a tile's first chains run under the previous tile's last scatters (with e_end = 1,
+        // every evaluation is a tile of its own).
+        uint32_t ftile = a.tile0 + blockIdx.x;   // fetch cursor: (ftile, fe), with the row state of ftile
+        int fe = 0;
+        float x[3], xp[3];
+        bool f_in_range = false;
+        // scatter positions and row masks of evaluations it, it+1, it+2 (slot 2 is filled by the fetch of iteration it)
+        float u[3][3];
+        bool inr[3];
+        auto write_E = [&](const float (&ff)[16], const uint32_t itw) {
+            const int ecol = 32 * (int)(itw & 1u);
+            #pragma unroll
+            for (int i = 0; i < 8; i++) {
+                const int k = 2 * half_level(i, half) + ecol;
+                uint32_t h2, m2, l2;
+                split3x2(ff[2 * i], ff[2 * i + 1], h2, m2, l2);
+                const uint32_t o = oE + sw_off16(r, k);
+                *reinterpret_cast<uint32_t*>(sm + o) = h2;
+                *reinterpret_cast<uint32_t*>(sm + o + kTile) = m2;
+                *reinterpret_cast<uint32_t*>(sm + o + 2 * kTile) = l2;
             }
-            // Software pipeline over the evaluations of this tile: ping-pong E.  The encoding uses 32 of the tile's 64 columns, so evaluation
-            // `it` lives in columns 32 (it & 1) .. + 31 (operand start address + 64 B).  E(it+2) is written at the END of iteration `it` (its
-            // half was last read by chain(it), retired at d4(it)), after the scatter of dEnc(it) under which its gather loads were in flight;
-            // chain(it+1) then starts the moment chain(it) retires -- the MMA warp has already seen a1(it+1).
-            float f[16];
-            auto write_E = [&](const float (&ff)[16], const uint32_t itw) {
-                const int ecol = 32 * (int)(itw & 1u);
+            tc::fence_proxy_async();
+            mbar_arrive(a1_full);
+        };
+        // encodings of the next evaluation of the stream into ff, its scatter position into uu and row mask into ir; false past the end
+        auto fetch = [&](float (&ff)[16], float (&uu)[3], bool& ir) -> bool {
+            if (ftile >= a.tile1 || (uint64_t)ftile * T >= m_pad) return false;
+            if (fe == 0) {
+                const uint32_t row = ftile * T + r;
+                const RowInfo ri = row_info(R, row);
+                f_in_range = ri.in_range;
                 #pragma unroll
-                for (int i = 0; i < 8; i++) {
-                    const int k = 2 * half_level(i, half) + ecol;
-                    uint32_t h2, m2, l2;
-                    split3x2(ff[2 * i], ff[2 * i + 1], h2, m2, l2);
-                    const uint32_t o = oE + sw_off16(r, k);
-                    *reinterpret_cast<uint32_t*>(sm + o) = h2;
-                    *reinterpret_cast<uint32_t*>(sm + o + kTile) = m2;
-                    *reinterpret_cast<uint32_t*>(sm + o + 2 * kTile) = l2;
-                }
-                tc::fence_proxy_async();
-                mbar_arrive(a1_full);
-            };
-            auto fetch = [&](const int e, float (&ff)[16]) {
-                if (ext) { load16(a.enc_buf + ((size_t)(tile - a.tile0) * 13 + e) * (T * 32) + (size_t)r * 32 + 4 * half, ff); return; }
-                float p[3];
-                eval_pos(e, x, xp, a.bound, p);
-                gather16s(a.table, lv, half, (p[0] + a.bound) / inv2b, (p[1] + a.bound) / inv2b, (p[2] + a.bound) / inv2b, ff);
-            };
-            fetch(0, f);
-            write_E(f, it);            // this half of E is free: this thread waited for d4 of the evaluations that read it
-            if (e_end > 1) {
-                fetch(1, f);
-                // a1 may run at most one phase ahead of its waiter: F1(it) issued (d1) => the MMA warp has consumed a1 phase `it`
-                tc::mbar_wait(d1_full, it & 1);
-                write_E(f, it + 1);
-            }
-            for (int e = 0; e < e_end; e++, it++) {
-                const uint32_t par = it & 1;
-                float p[3];
-                eval_pos(e, x, xp, a.bound, p);
-                const float u0 = (p[0] + a.bound) / inv2b, u1 = (p[1] + a.bound) / inv2b, u2 = (p[2] + a.bound) / inv2b;
-                const int en = e + 2;                           // the evaluation whose encodings this iteration hands over
-                // dEnc (this thread's 16 columns of its row: 8j + 4 half .. + 3, j = 0..3) into registers
-                tc::mbar_wait(d4_full, par);
-                uint32_t g[16];
-                #pragma unroll
-                for (int j = 0; j < 4; j++) {
-                    const float4 t = *reinterpret_cast<const float4*>(denc + r * 32 + 8 * j + 4 * half);
-                    g[4 * j] = __float_as_uint(t.x); g[4 * j + 1] = __float_as_uint(t.y); g[4 * j + 2] = __float_as_uint(t.z); g[4 * j + 3] = __float_as_uint(t.w);
-                }
-                mbar_arrive(denc_free);
-                if (en < e_end) fetch(en, f);                   // loads in flight under the scatter
-                #pragma unroll 1
-                for (int i = 0; i < 8; i++) {
-                    float g0 = 0.f, g1 = 0.f;
+                for (int c = 0; c < 3; c++) { x[c] = 0.f; xp[c] = 0.f; }
+                if (ri.real) { x[0] = a.xyzs[3 * (size_t)row]; x[1] = a.xyzs[3 * (size_t)row + 1]; x[2] = a.xyzs[3 * (size_t)row + 2]; }
+                if (a.n_evals > 7 && ri.in_range) {
+                    float z[3];
+                    smooth_z(a.smooth_noise, a.seed, a.noise_mode, row, ri, x, z);
                     #pragma unroll
-                    for (int q = 0; q < 8; q++) if (q == i) { g0 = __uint_as_float(g[2 * q]); g1 = __uint_as_float(g[2 * q + 1]); }
-                    const LevelSm L = lv[half_level(i, half)];
-                    scatter_level_agg(a.g_table, L, u0, u1, u2, g0, g1, in_range, L.scale < kAggScaleMax, lane);
+                    for (int c = 0; c < 3; c++) xp[c] = x[c] + z[c] * kSmoothStd;
                 }
-                if (en < e_end) write_E(f, it + 2);
+            }
+            float p[3];
+            eval_pos(fe, x, xp, a.bound, p);
+            uu[0] = (p[0] + a.bound) / inv2b; uu[1] = (p[1] + a.bound) / inv2b; uu[2] = (p[2] + a.bound) / inv2b;
+            ir = f_in_range;
+            if (ext) load16(a.enc_buf + ((size_t)(ftile - a.tile0) * 13 + fe) * (T * 32) + (size_t)r * 32 + 4 * half, ff);
+            else gather16s(a.table, lv, half, uu[0], uu[1], uu[2], ff);
+            if (++fe == e_end) { fe = 0; ftile += gridDim.x; }
+            return true;
+        };
+        float f[16];
+        uint32_t n_fetched = 0;
+        BWD_CLK_T(clk_role); BWD_CLK_VAR(clk_wait); BWD_CLK_VAR(clk_scatter);
+        if (fetch(f, u[0], inr[0])) {
+            n_fetched++;
+            write_E(f, 0);
+            if (fetch(f, u[1], inr[1])) {
+                n_fetched++;
+                // a1 may run at most one phase ahead of its waiter: F1(0) issued (d1) => the MMA warp has consumed a1 phase 0
+                tc::mbar_wait(d1_full, 0);
+                write_E(f, 1);
             }
         }
+        for (; it < n_fetched; it++) {
+            // dEnc (this thread's 16 columns of its row: 8j + 4 half .. + 3, j = 0..3) into registers
+            BWD_CLK_T(t0);
+            tc::mbar_wait(d4_full, it & 1);
+            BWD_CLK_ACC(clk_wait, t0);
+            uint32_t g[16];
+            #pragma unroll
+            for (int j = 0; j < 4; j++) {
+                const float4 t = *reinterpret_cast<const float4*>(denc + r * 32 + 8 * j + 4 * half);
+                g[4 * j] = __float_as_uint(t.x); g[4 * j + 1] = __float_as_uint(t.y); g[4 * j + 2] = __float_as_uint(t.z); g[4 * j + 3] = __float_as_uint(t.w);
+            }
+            mbar_arrive(denc_free);
+            const bool next = fetch(f, u[2], inr[2]);      // evaluation it+2: loads in flight under the scatter
+            n_fetched += next;
+            BWD_CLK_T(t1);
+            #pragma unroll 1
+            for (int i = 0; i < 8; i++) {
+                float g0 = 0.f, g1 = 0.f;
+                #pragma unroll
+                for (int q = 0; q < 8; q++) if (q == i) { g0 = __uint_as_float(g[2 * q]); g1 = __uint_as_float(g[2 * q + 1]); }
+                const LevelSm L = lv[half_level(i, half)];
+                scatter_level_agg(a.g_table, L, u[0][0], u[0][1], u[0][2], g0, g1, inr[0], L.scale < kAggScaleMax, lane);
+            }
+            BWD_CLK_ACC(clk_scatter, t1);
+            if (next) write_E(f, it + 2);
+            #pragma unroll
+            for (int c = 0; c < 3; c++) { u[0][c] = u[1][c]; u[1][c] = u[2][c]; }
+            inr[0] = inr[1]; inr[1] = inr[2];
+        }
+        BWD_CLK_FLUSH(4, clock64() - clk_role); BWD_CLK_FLUSH(5, clk_wait); BWD_CLK_FLUSH(6, clk_scatter);
     } else {
         // ================================ MMA warpgroup ================================
         // two accumulators plus the resident dW2 / dW1 do not fit the 128-register share of a 512-thread CTA: take the encoders' spare ones
@@ -1367,6 +1431,12 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
             }
         };
         auto rows64 = [](const Operand& o, int h) { return Operand{o.base + 8192u * (uint32_t)h, o.part_stride, o.lbo}; };   // K-major A: rows 64 h ..
+        BWD_CLK_T(clk_role); BWD_CLK_VAR(clk_wait);
+        auto wait_full = [&](uint64_t* bar, uint32_t parity) {
+            BWD_CLK_T(t0);
+            tc::mbar_wait(bar, parity);
+            BWD_CLK_ACC(clk_wait, t0);
+        };
         for (uint32_t tile = a.tile0 + blockIdx.x; tile < a.tile1 && (uint64_t)tile * T < m_pad; tile += gridDim.x) {
             for (int e = 0; e < e_end; e++, it++) {
                 const uint32_t par = it & 1;
@@ -1375,20 +1445,22 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                 const Operand Z{sbase + oZ, (uint32_t)kTile, (uint32_t)kTile};
                 const Operand W1{sbase + oW1, 8192u, 8192u}, W2{sbase + oW2, 8192u, 8192u};
                 float d[2][32];
-                if (e == 0) tc::mbar_wait(a1_full, par);             // e > 0: consumed before d4 of the previous evaluation
-                mbar_arrive(d1_full);
+                if (it == 0) {                                      // it > 0: consumed before d4 of the previous evaluation
+                    wait_full(a1_full, 0);
+                    mbar_arrive(d1_full);                           // the encoders' one wait on d1 (before they write E(1))
+                }
                 wg::fence();
                 #pragma unroll
                 for (int h = 0; h < 2; h++) issue_bf16x3<64, 0, 0>(d[h], rows64(E, h), W1, 32, 0u);   // F1 (K = 32: the zero columns 32..63 are skipped)
                 wg::commit(); wg::wait<0>(); wg::reg_fence(d[0]); wg::reg_fence(d[1]);
                 stage(d);
-                tc::mbar_wait(a2_full, par);
+                wait_full(a2_full, par);
                 wg::fence();
                 #pragma unroll
                 for (int h = 0; h < 2; h++) issue_bf16x3<64, 0, 0>(d[h], rows64(H, h), W2, 64, 0u);   // F2
                 wg::commit(); wg::wait<0>(); wg::reg_fence(d[0]); wg::reg_fence(d[1]);
                 stage(d);
-                tc::mbar_wait(a3_full, par);
+                wait_full(a3_full, par);
                 wg::fence();
                 #pragma unroll
                 for (int h = 0; h < 2; h++) issue_bf16x3<64, 0, 1>(d[h], rows64(Z, h), W2, 64, 0u);   // G2 : dH1 = dZ2 W2
@@ -1398,7 +1470,7 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                 #pragma unroll
                 for (int i = 0; i < 32; i++) dw2[i] += t2[i];
                 stage(d);
-                tc::mbar_wait(a4_full, par);
+                wait_full(a4_full, par);
                 float g1[2][16];
                 wg::fence();
                 #pragma unroll
@@ -1409,12 +1481,17 @@ __global__ void __launch_bounds__(bwdtc::kThreads, 1) k_field_bwd_tc(const BwdAr
                 #pragma unroll
                 for (int i = 0; i < 16; i++) dw1[i] += t1[i];
                 stage_frag<16>(g1, denc_w, 32, 0, 32, wl, lane);                                       // over the dZ tiles, now free
-                // E(it+1) is already there (other half).  Consuming its a1 phase BEFORE releasing d4(it) keeps the encoders,
-                // who arrive for it+2 only after d4(it), from lapping this waiter.
-                if (e + 1 < e_end) tc::mbar_wait(a1_full, par ^ 1u);
+                // E(it+1), of this tile or the next, is already there (other half) or on its way.  Consuming its a1 phase BEFORE
+                // releasing d4(it) keeps the encoders, who arrive for it+2 only after d4(it), from lapping this waiter.
+                const uint32_t ntile = tile + gridDim.x;
+                if (e + 1 < e_end || (ntile < a.tile1 && (uint64_t)ntile * T < m_pad)) wait_full(a1_full, par ^ 1u);
                 mbar_arrive(d4_full);
             }
         }
+        BWD_CLK_FLUSH(2, clock64() - clk_role); BWD_CLK_FLUSH(3, clk_wait);
+#ifdef MI3D_FIELD_BWD_CLOCKS
+        if (warp == 12 && lane == 0) atomicAdd(&g_field_bwd_clocks[7], (unsigned long long)it);
+#endif
         // ---- flush the register-resident weight gradients: dW2 [64 x 64] and dW1 [64 x 32] (row = output feature) ----
         if (it > 0) {
             #pragma unroll
@@ -1663,6 +1740,17 @@ int mi3d_field_backward(const mi3d_field_io* io, const float* table, const mi3d_
     }
     MI3D_RETURN_LAUNCH();
 }
+
+#ifdef MI3D_FIELD_BWD_CLOCKS
+// the counters of g_field_bwd_clocks since the previous call (8 values), then zeroes them; profiling builds only
+extern "C" int mi3d_field_bwd_clocks(unsigned long long* out) {
+    MI3D_CHECK(cudaDeviceSynchronize());
+    MI3D_CHECK(cudaMemcpyFromSymbol(out, g_field_bwd_clocks, sizeof(g_field_bwd_clocks)));
+    const unsigned long long zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    MI3D_CHECK(cudaMemcpyToSymbol(g_field_bwd_clocks, zero, sizeof(zero)));
+    return MI3D_OK;
+}
+#endif
 
 size_t mi3d_field_enc_cache_bytes(uint32_t tiles) { return (size_t)tiles * 13 * T * 32 * sizeof(float); }
 
