@@ -479,8 +479,8 @@ typedef struct {
 size_t mi3d_sd_workspace_bytes(const mi3d_unet_cfg* unet, const mi3d_vae_cfg* vae);
 mi3d_engine_t mi3d_sd_create(const mi3d_unet_cfg* unet, const mi3d_vae_cfg* vae, void* workspace, size_t workspace_bytes);
 /* Parameters are enumerated by their diffusers state_dict names ("down_blocks.0.resnets.0.conv1.weight", VAE names are
- * prefixed as in AutoencoderKL: "encoder....", "quant_conv....").  Graph replay covers the three static launch lists (U-Net,
- * VAE encode, VAE input-gradient).  Debug taps: "unet.mid", "vae.grad_in", ... */
+ * prefixed as in AutoencoderKL: "encoder....", "quant_conv....").  Graph replay covers the static launch lists (U-Net,
+ * VAE encode, VAE input-gradient, VAE decode, sampling step).  Debug taps: "unet.mid", "vae.grad_in", ... */
 
 /* replaces nerf/sd.py:124 (F.interpolate to 512) + :133,212-220 (encode_imgs: vae.encode(2x-1).latent_dist.sample()*0.18215)
  * pred_rgb [1,3,H,W] fp32 in [0,1]; eps_posterior, latents [1,4,h,w] fp32 (h = image_hw/8). */
@@ -499,6 +499,19 @@ int mi3d_sd_unet_sds(mi3d_engine_t h, const float* latents, const float* noise, 
 int mi3d_sd_ddim_step(const float* noise_pred, const float* latents_noisy, const long long* t, const float* alphas_cumprod,
                       float* prev_sample, int n, mi3d_stream_t stream);
 int mi3d_sd_decode(mi3d_engine_t h, const float* latents, float* imgs, mi3d_stream_t stream);
+/* Text-to-latents sampling (produce_latents, nerf/sd.py:176-199): DDIM with eta 0 and classifier-free guidance, n steps without the
+ * host.  One entry of the schedule per step, built by the caller from the scheduler config: t (the U-Net timestep), alpha_t =
+ * alphas_cumprod[t] and alpha_prev = alphas_cumprod[t - T/n], or final_alpha_cumprod when t - T/n < 0. */
+typedef struct {
+    long long t;
+    float alpha_t, alpha_prev;
+} mi3d_sd_schedule;
+/* latents: DEVICE fp32 [1,4,h,w], x_T in, x_0 out.  sched: DEVICE table of n entries (1 <= n <= 1000).  prediction_type: 0 epsilon,
+ * 1 v_prediction.  text_embeddings fp32 [2,77,cross_dim] (uncond first).  Per step: [x, x] -> U-Net at t_i -> CFG
+ * (text + gs*(text - uncond), as the reference writes it) -> DDIMScheduler.step (clip_sample off) written back in place; the step body
+ * is one static launch list that replays as a CUDA graph when graph replay is on.  Nothing is read back to the host. */
+int mi3d_sd_sample(mi3d_engine_t h, float* latents, const mi3d_sd_schedule* sched, int n, int prediction_type, const float* text_embeddings,
+                   float guidance_scale, mi3d_stream_t stream);
 /* live timing of the tensor-core tile kernel: enable=1 starts recording CUDA events around every launch; enable=0 stops and
  * returns the summed kernel time (ms) and launch count (HOST pointers; synchronises on the recorded events). */
 int mi3d_sd_profile(mi3d_engine_t h, int enable, float* gemm_ms_host, int* launches_host);

@@ -187,7 +187,13 @@ struct Builder : mi3d_engine {
         if (dry) return;
         const long long M = x.rows();
         int bw = x.w < 128 ? x.w : 128, bh = 128 / bw; if (bh > x.h) bh = x.h; const int bn_img = 128 / (bw * bh);
-        if (M % 128 || x.c % 64 || bw * bh * bn_img != 128 || x.w % bw || x.h % bh || x.n % bn_img) { err = MI3D_ERR_ARG; return; }
+        if (M % 128 || x.c % 64 || bw * bh * bn_img != 128 || x.w % bw || x.h % bh || x.n % bn_img) {
+            // a width that neither divides 128 nor is a multiple of it (96 / 48 / 24 / 12 for 768 x 768 SD), or pixels off the 128-row
+            // grid: the spatial-block tiles of conv3_block, which overhang the edges instead of spanning whole rows
+            if (x.c % 64) { err = MI3D_ERR_ARG; return; }
+            conv3_block(x, w, Cout, y, bias, tc::EPI_PLAIN, nullptr, residual, row_bias);
+            return;
+        }
         int bn = tc::pick_block_n(Cout, M / 128, num_sms);
         if (!bn) { err = MI3D_ERR_ARG; return; }
         int splits = 1;
@@ -218,7 +224,7 @@ struct Builder : mi3d_engine {
     // fewest rows over the image edge), overhanging tiles load zeros and store only in-image pixels.  mode: EPI_PLAIN (optionally
     // + residual, same layout as y), EPI_RELU, or EPI_RELU_BWD with aux = the mask source.  No split-K (its fp32 RED order varies run to run).
     void conv3_block(const T4& x, const __half* w, int Cout, const T4& y, const float* bias, int mode, const __half* aux = nullptr,
-                     const __half* residual = nullptr) {
+                     const __half* residual = nullptr, const float* row_bias = nullptr) {
         if (dry) return;
         if (x.c % 64 || Cout % 64 || y.n != x.n || y.h != x.h || y.w != x.w || y.c != Cout) { err = MI3D_ERR_ARG; return; }
         int bw = 128, bh = 1; long long best = -1;
@@ -237,7 +243,8 @@ struct Builder : mi3d_engine {
         p.M = (int)(tiles * 128); p.N = Cout; p.K = 9 * x.c; p.num_k_blocks = 9 * (x.c / 64); p.conv = 2;
         p.conv_H = x.h; p.conv_W = x.w; p.conv_bw = bw; p.conv_bh = bh; p.cin_blocks = x.c / 64;
         p.a_z1 = 1; p.b_z1 = 1; p.b_batched = 0; p.out = y.p; p.ldc = Cout; p.out_z1 = 1;
-        p.bias = bias; p.rows_per_group = 1; p.epi_mode = mode; p.alpha = 1.f; p.m_valid = (int)x.rows(); p.splits = 1; p.aux = const_cast<__half*>(aux);
+        p.bias = bias; p.row_bias = row_bias; p.rows_per_group = x.h * x.w;          // row_bias: one row per image
+        p.epi_mode = mode; p.alpha = 1.f; p.m_valid = (int)x.rows(); p.splits = 1; p.aux = const_cast<__half*>(aux);
         p.residual = residual; p.ld_res = Cout;
         push([this, ma, mb, p, bn](cudaStream_t st) { return timed_launch(ma, mb, p, bn, 1, st); });
     }

@@ -16,6 +16,64 @@ namespace sd {
 
 using namespace plan;
 
+// ------------------------------------------------------------------------------------------------------------
+// Sampling step kernels (mi3d_sd_sample).  Both run as ONE CTA: the step index is read by every thread and advanced after a
+// barrier, so no launch in the replayed list depends on a host-side argument.
+// ------------------------------------------------------------------------------------------------------------
+constexpr int kMaxSampleSteps = 1000;                     // num_train_timesteps: set_timesteps accepts n <= T
+struct SampleState { int step; int pred_type; float gs; int pad; };
+
+// call head: the caller's schedule and x_T into the engine's buffers, step index 0
+__global__ void k_sample_begin(const mi3d_sd_schedule* __restrict__ sched, int n, const float* __restrict__ x, mi3d_sd_schedule* __restrict__ tab,
+                               float* __restrict__ lat, int count, SampleState* __restrict__ s, int pred_type, float gs) {
+    const int stride = gridDim.x * blockDim.x;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < max(count, n); i += stride) {
+        if (i < count) lat[i] = x[i];
+        if (i < n) tab[i] = sched[i];
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) *s = SampleState{0, pred_type, gs, 0};
+}
+
+// step head: t_i into the U-Net's timestep slot; U-Net input [x, x] NHWC fp16 from the fp32 NCHW latents (no noise added)
+__global__ void __launch_bounds__(1024) k_sample_in(const mi3d_sd_schedule* __restrict__ tab, const SampleState* __restrict__ s,
+                                                    const float* __restrict__ lat, __half* __restrict__ xin, long long* __restrict__ tslot, int pix) {
+    const int step = s->step;
+    if (threadIdx.x == 0) *tslot = tab[step].t;
+    for (int i = threadIdx.x; i < pix; i += blockDim.x) {
+        __align__(8) __half o[4];
+        #pragma unroll
+        for (int c = 0; c < 4; c++) o[c] = __float2half_rn(lat[(size_t)c * pix + i]);
+        *reinterpret_cast<uint2*>(xin + (size_t)i * 4) = *reinterpret_cast<const uint2*>(o);
+        *reinterpret_cast<uint2*>(xin + ((size_t)pix + i) * 4) = *reinterpret_cast<const uint2*>(o);
+    }
+}
+
+// step tail: CFG as nerf/sd.py:193-194 writes it, then DDIMScheduler.step with eta 0 and clip_sample off:
+//   epsilon:      x0 = (x - sqrt(1 - a_t) e) / sqrt(a_t),   eps = e
+//   v_prediction: x0 = sqrt(a_t) x - sqrt(1 - a_t) e,       eps = sqrt(a_t) e + sqrt(1 - a_t) x
+//   x_prev = sqrt(a_prev) x0 + sqrt(1 - a_prev) eps; in place, then the step index advances
+__global__ void __launch_bounds__(1024) k_sample_step(const float* __restrict__ unet_out /*[2][pix][4]*/, const mi3d_sd_schedule* __restrict__ tab,
+                                                      SampleState* __restrict__ s, float* __restrict__ lat, int pix) {
+    const int step = s->step, v = s->pred_type;
+    const float gs = s->gs, a_t = tab[step].alpha_t, a_p = tab[step].alpha_prev;
+    const float sa = sqrtf(a_t), sb = sqrtf(1.f - a_t), sp = sqrtf(a_p), sq = sqrtf(1.f - a_p);
+    for (int i = threadIdx.x; i < pix; i += blockDim.x) {
+        const float4 un = *reinterpret_cast<const float4*>(unet_out + (size_t)i * 4);
+        const float4 tx = *reinterpret_cast<const float4*>(unet_out + ((size_t)pix + i) * 4);
+        const float u4[4] = {un.x, un.y, un.z, un.w}, t4[4] = {tx.x, tx.y, tx.z, tx.w};
+        #pragma unroll
+        for (int c = 0; c < 4; c++) {
+            const float e = t4[c] + gs * (t4[c] - u4[c]);
+            const float x = lat[(size_t)c * pix + i];
+            const float x0 = v ? sa * x - sb * e : (x - sb * e) / sa;
+            const float eps = v ? sa * e + sb * x : e;
+            lat[(size_t)c * pix + i] = sp * x0 + sq * eps;
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) s->step = step + 1;
+}
+
 struct Engine : Builder {
     mi3d_unet_cfg ucfg; mi3d_vae_cfg vcfg;
     // either part may be absent (NULL); a VAE-only engine takes its GroupNorm group count from the VAE
@@ -646,12 +704,34 @@ struct Engine : Builder {
     }
     float* vae_grad_img = nullptr;
 
+    // ------------------------------------------------------------------------------------------------------
+    // DDIM sampling step (produce_latents, nerf/sd.py:183-197): [x, x] -> U-Net -> CFG + DDIM update in place.  The schedule, the
+    // latents and the step index live in engine buffers, so the list is static and replays as one graph per step.
+    // ------------------------------------------------------------------------------------------------------
+    std::vector<Op> sample_ops;
+    mi3d_sd_schedule* sample_sched = nullptr; float* sample_lat = nullptr; SampleState* sample_state = nullptr;
+    void build_sample() {
+        // allocated after every other list so that the existing buffers keep their offsets
+        const int pix = ucfg.latent_hw * ucfg.latent_hw;
+        sample_sched = (mi3d_sd_schedule*)alloc(kMaxSampleSteps * sizeof(mi3d_sd_schedule));
+        sample_lat = alloc32((size_t)4 * pix);
+        sample_state = (SampleState*)alloc(sizeof(SampleState));
+        cur = &sample_ops;
+        const mi3d_sd_schedule* tab = sample_sched; float* lat = sample_lat; SampleState* s = sample_state;
+        __half* xin = unet_in.p; long long* tslot = t_dev; const float* uo = unet_out;
+        push([=](cudaStream_t st) { k_sample_in<<<1, 1024, 0, st>>>(tab, s, lat, xin, tslot, pix); return (int)cudaGetLastError(); });
+        for (const Op& op : unet_ops) push(op);
+        push([=](cudaStream_t st) { k_sample_step<<<1, 1024, 0, st>>>(uo, tab, s, lat, pix); return (int)cudaGetLastError(); });
+        cur = nullptr;
+    }
+
     int build(bool dry_run) {
         dry = dry_run; off = 0; err = 0; params.clear(); pindex.clear(); unet_ops.clear(); enc_ops.clear(); enc_bwd_ops.clear(); dec_ops.clear();
-        vres.clear(); vdown.clear(); vorder.clear(); named.clear();
+        sample_ops.clear(); vres.clear(); vdown.clear(); vorder.clear(); named.clear();
         splitk_elems = (size_t)2048 * 2560; splitk_ws = alloc32(splitk_elems);       // covers M <= 2048 rows x N <= 2560
         if (ucfg.n_levels > 0) build_unet();
         if (vcfg.n_levels > 0) { build_vae(); build_vae_bwd(); if (vcfg.decoder) build_vae_dec(); }
+        if (ucfg.n_levels > 0 && ucfg.batch == 2 && ucfg.in_ch == 4 && ucfg.out_ch == 4) build_sample();
         return err;
     }
 
@@ -970,6 +1050,23 @@ int mi3d_sd_unet_sds(mi3d_engine_t h, const float* latents, const float* noise, 
     sd::k_ctx_pad<<<sd::Engine::blocks_for((size_t)B * e.ctx_pad * e.ucfg.cross_dim), 256, 0, st>>>(text_embeddings, e.ctx16, B, e.ucfg.ctx_len, e.ctx_pad, e.ucfg.cross_dim);
     int r = e.run(e.unet_ops, st); if (r) return r;
     sd::k_cfg_sds<<<(pix + 127) / 128, 128, 0, st>>>(e.unet_out, noise, alphas_cumprod, e.t_dev, guidance_scale, noise_pred, grad, pix);
+    return (int)cudaGetLastError();
+}
+
+// nerf/sd.py:176-199 produce_latents: n DDIM steps with CFG on the device; the text context is padded once, before the loop
+int mi3d_sd_sample(mi3d_engine_t h, float* latents, const mi3d_sd_schedule* sched, int n, int prediction_type, const float* text_embeddings,
+                   float guidance_scale, mi3d_stream_t stream) {
+    sd::Engine* ep = plan::engine_of<sd::Engine>(h);
+    if (!ep || ep->sample_ops.empty() || !latents || !sched || !text_embeddings || n < 1 || n > sd::kMaxSampleSteps ||
+        (prediction_type != 0 && prediction_type != 1))
+        return MI3D_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream; sd::Engine& e = *ep;
+    const int count = 4 * e.ucfg.latent_hw * e.ucfg.latent_hw, B = e.ucfg.batch;
+    sd::k_sample_begin<<<sd::Engine::blocks_for((size_t)std::max(count, n)), 256, 0, st>>>(sched, n, latents, e.sample_sched, e.sample_lat,
+                                                                                          count, e.sample_state, prediction_type, guidance_scale);
+    sd::k_ctx_pad<<<sd::Engine::blocks_for((size_t)B * e.ctx_pad * e.ucfg.cross_dim), 256, 0, st>>>(text_embeddings, e.ctx16, B, e.ucfg.ctx_len, e.ctx_pad, e.ucfg.cross_dim);
+    for (int i = 0; i < n; i++) { int r = e.run(e.sample_ops, st); if (r) return r; }
+    MI3D_CHECK(cudaMemcpyAsync(latents, e.sample_lat, (size_t)count * sizeof(float), cudaMemcpyDeviceToDevice, st));
     return (int)cudaGetLastError();
 }
 

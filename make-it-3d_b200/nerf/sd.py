@@ -19,12 +19,17 @@ A native `nerf.clip.CLIP` computes them on the CLIP engine (csrc/clip_engine.cu,
 `get_text_embeds` runs the SD text encoder (nerf/sd_text.py, csrc/sd_text_engine.cu) once its weights are loaded with
 `load_diffusers_state_dict(text_encoder_state=...)`; prompts given as strings go through the `tokenizer` passed to the constructor.
 Without text-encoder weights it returns a deterministic stand-in keyed by the prompt strings.
+`produce_latents` / `prompt_to_img` (nerf/sd.py:176-238) sample with DDIM (eta 0) and classifier-free guidance on the device
+(`mi3d_sd_sample`); `from_pretrained(local_dir, device)` loads a local diffusers directory; `python -m mi3d_b200.nerf.sd PROMPT --ckpt DIR`
+is the reference's demo.
 """
 import ctypes as C
 import hashlib
+import json
 import math
 import os
 
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -94,6 +99,144 @@ def alphas_cumprod(num_train_timesteps=1000, beta_start=0.00085, beta_end=0.012)
     return torch.cumprod(1.0 - betas, dim=0)
 
 
+# ---------------------------------------------------------------------------------------------------------------------------------
+# DDIM sampling schedule (produce_latents, nerf/sd.py:176-199) and diffusers checkpoint configs
+# ---------------------------------------------------------------------------------------------------------------------------------
+NUM_TRAIN_TIMESTEPS = 1000
+# SD's scheduler defaults (scheduler_config.json of every SD-1.x / SD-2.x checkpoint but SD-2.1-768's prediction_type)
+SD_SCHEDULER = dict(steps_offset=1, set_alpha_to_one=False, prediction_type="epsilon", timestep_spacing="leading")
+PREDICTION_TYPES = {"epsilon": 0, "v_prediction": 1}
+
+
+class SDSchedule(C.Structure):
+    """mi3d_sd_schedule: one DDIM step of mi3d_sd_sample"""
+    _fields_ = [("t", C.c_longlong), ("alpha_t", C.c_float), ("alpha_prev", C.c_float)]
+
+
+def ddim_timesteps(n, spacing="leading", steps_offset=1, T=NUM_TRAIN_TIMESTEPS):
+    """DDIMScheduler.set_timesteps(n).timesteps (int64, descending) for timestep_spacing 'leading' / 'trailing' / 'linspace'"""
+    if not isinstance(n, int) or not 1 <= n <= T:
+        raise L.Mi3dError(f"num_inference_steps must be an integer in 1..{T}; got {n!r}")
+    if spacing == "leading":
+        ts = (np.arange(0, n) * (T // n)).round()[::-1].astype(np.int64) + int(steps_offset)
+    elif spacing == "trailing":
+        ts = np.round(np.arange(T, 0, -T / n)).astype(np.int64) - 1
+    elif spacing == "linspace":
+        ts = np.linspace(0, T - 1, n).round()[::-1].astype(np.int64)
+    else:
+        raise L.Mi3dError(f"timestep_spacing must be 'leading', 'trailing' or 'linspace'; got {spacing!r}")
+    if ts.min() < 0 or ts.max() >= T:
+        raise L.Mi3dError(f"{n} steps with {spacing!r} spacing and steps_offset {steps_offset} give timesteps outside 0..{T - 1}")
+    return np.ascontiguousarray(ts)
+
+
+def ddim_schedule(n, spacing="leading", steps_offset=1, set_alpha_to_one=False, alphas=None, T=NUM_TRAIN_TIMESTEPS):
+    """the mi3d_sd_schedule table (a numpy record array): t_i, alphas_cumprod[t_i] and alpha_prev_i = alphas_cumprod[t_i - T // n], or
+    final_alpha_cumprod (1 with set_alpha_to_one, else alphas_cumprod[0]) when t_i - T // n < 0"""
+    a = (alphas_cumprod(T) if alphas is None else alphas).detach().cpu().float().numpy()
+    ts = ddim_timesteps(n, spacing, steps_offset, T)
+    prev = ts - T // n
+    final = np.float32(1.0) if set_alpha_to_one else a[0]
+    tab = np.zeros(n, dtype=np.dtype([("t", "<i8"), ("alpha_t", "<f4"), ("alpha_prev", "<f4")]))
+    tab["t"], tab["alpha_t"] = ts, a[ts]
+    tab["alpha_prev"] = np.where(prev >= 0, a[np.maximum(prev, 0)], final)
+    assert tab.dtype.itemsize == C.sizeof(SDSchedule)
+    return tab
+
+
+def _heads(cfg, n_levels):
+    h = cfg["attention_head_dim"]           # diffusers' name; SD's configs store the head COUNT in it
+    h = [h] * n_levels if isinstance(h, int) else list(h)
+    if len(h) != n_levels:
+        raise L.Mi3dError(f"attention_head_dim {cfg['attention_head_dim']} does not match {n_levels} levels")
+    return tuple(int(x) for x in h)
+
+
+def unet_cfg_from_config(cfg):
+    """diffusers' unet/config.json -> the engine's U-Net configuration (sd20_unet_cfg / sd15_unet_cfg form)"""
+    if cfg.get("in_channels", 4) != 4 or cfg.get("out_channels", 4) != 4:
+        raise L.Mi3dError(f"only 4-channel latent U-Nets are supported; got in_channels={cfg.get('in_channels')} (inpainting and "
+                          f"depth-conditioned checkpoints take more) out_channels={cfg.get('out_channels')}")
+    bo = tuple(int(x) for x in cfg["block_out_channels"])
+    if not 1 <= len(bo) <= 4 or not isinstance(cfg.get("cross_attention_dim"), int):
+        raise L.Mi3dError(f"unsupported U-Net topology: block_out_channels {bo}, cross_attention_dim {cfg.get('cross_attention_dim')}")
+    out = dict(in_channels=4, out_channels=4, block_out=bo, layers_per_block=int(cfg["layers_per_block"]), heads=_heads(cfg, len(bo)),
+               cross_dim=int(cfg["cross_attention_dim"]), groups=int(cfg.get("norm_num_groups", 32)), ctx_len=77,
+               latent_hw=int(cfg["sample_size"]))
+    if not cfg.get("use_linear_projection", False):
+        out["proj_conv"] = True                  # SD-1.x: 1x1-conv proj_in / proj_out
+    return out
+
+
+def vae_cfg_from_config(cfg):
+    """diffusers' vae/config.json -> the engine's VAE configuration (sd_vae_cfg form)"""
+    if float(cfg.get("scaling_factor", 0.18215)) != 0.18215:
+        raise L.Mi3dError(f"the VAE's scaling_factor is {cfg['scaling_factor']}; nerf/sd.py scales latents by 0.18215")
+    if cfg.get("in_channels", 3) != 3 or cfg.get("latent_channels", 4) != 4:
+        raise L.Mi3dError("only 3-channel images and 4-channel latents are supported")
+    return dict(in_channels=3, latent_channels=4, block_out=tuple(int(x) for x in cfg["block_out_channels"]),
+                layers_per_block=int(cfg["layers_per_block"]), groups=int(cfg.get("norm_num_groups", 32)), image_hw=int(cfg["sample_size"]))
+
+
+def scheduler_from_config(cfg):
+    """scheduler/scheduler_config.json -> the DDIM settings the sampler reads (DDIMScheduler's defaults for absent keys).  The betas
+    must be SD's scaled_linear 0.00085 / 0.012 over 1000 steps: the SDS path's `alphas` are built from them."""
+    betas = (cfg.get("beta_schedule", "linear"), float(cfg.get("beta_start", 0.0001)), float(cfg.get("beta_end", 0.02)),
+             int(cfg.get("num_train_timesteps", 1000)))
+    if betas != ("scaled_linear", 0.00085, 0.012, 1000) or cfg.get("trained_betas") is not None or cfg.get("rescale_betas_zero_snr", False):
+        raise L.Mi3dError(f"unsupported beta schedule {betas} (trained_betas={cfg.get('trained_betas')}, rescale_betas_zero_snr="
+                          f"{cfg.get('rescale_betas_zero_snr', False)}): SD's is scaled_linear 0.00085 / 0.012 over 1000 steps")
+    if cfg.get("clip_sample", True) or cfg.get("thresholding", False):
+        raise L.Mi3dError("clip_sample / thresholding are not supported (SD's scheduler configs turn both off)")
+    out = dict(steps_offset=int(cfg.get("steps_offset", 0)), set_alpha_to_one=bool(cfg.get("set_alpha_to_one", True)),
+               prediction_type=cfg.get("prediction_type", "epsilon"), timestep_spacing=cfg.get("timestep_spacing", "leading"))
+    if out["prediction_type"] not in PREDICTION_TYPES:
+        raise L.Mi3dError(f"prediction_type must be one of {sorted(PREDICTION_TYPES)}; got {out['prediction_type']!r}")
+    ddim_timesteps(1, out["timestep_spacing"], out["steps_offset"])
+    return out
+
+
+_ST_DTYPES = {"F32": torch.float32, "F16": torch.float16, "BF16": torch.bfloat16, "F64": torch.float64, "I64": torch.int64,
+              "I32": torch.int32}
+
+
+def read_safetensors(path):
+    """name -> CPU tensor from a .safetensors file (an 8-byte little-endian header size, a JSON header, then the raw tensors)"""
+    out = {}
+    with open(path, "rb") as f:
+        n = int.from_bytes(f.read(8), "little")
+        header = json.loads(f.read(n))
+        for name, meta in header.items():
+            if name == "__metadata__":
+                continue
+            if meta["dtype"] not in _ST_DTYPES:
+                raise L.Mi3dError(f"{path}: tensor {name} has unsupported dtype {meta['dtype']}")
+            b, e = meta["data_offsets"]
+            buf = bytearray(e - b)                  # each tensor is read straight into its own buffer: one host copy of the file
+            f.seek(8 + n + b)
+            if f.readinto(buf) != e - b:
+                raise L.Mi3dError(f"{path}: tensor {name} runs past the end of the file")
+            t = torch.frombuffer(buf, dtype=_ST_DTYPES[meta["dtype"]]) if e > b else torch.empty(0, dtype=_ST_DTYPES[meta["dtype"]])
+            out[name] = t.reshape(meta["shape"])
+    return out
+
+
+def _read_weights(folder, stem):
+    """<folder>/<stem>.safetensors, else <stem>.fp16.safetensors; .bin-only folders are refused (pickle files are not read)"""
+    for name in (stem + ".safetensors", stem + ".fp16.safetensors"):
+        p = os.path.join(folder, name)
+        if os.path.exists(p):
+            return read_safetensors(p)
+    raise L.Mi3dError(f"no {stem}[.fp16].safetensors in {folder} (.bin checkpoints are not supported)")
+
+
+def _read_json(path):
+    if not os.path.exists(path):
+        raise L.Mi3dError(f"{path} is missing: from_pretrained needs a local diffusers directory")
+    with open(path) as f:
+        return json.load(f)
+
+
 class SDEngine(L.Engine):
     """The SD engine (mi3d_sd_create): U-Net and VAE launch lists planned in one workspace."""
 
@@ -158,8 +301,10 @@ class _EncodeImgs(torch.autograd.Function):
 
 class StableDiffusion(nn.Module):
     def __init__(self, device, sd_version='2.0', hf_key=None, step_range=[0.2, 0.6], unet_cfg=None, vae_cfg=None, seed=0,
-                 unet_state=None, vae_state=None, graph_replay=True, defer_backward=False, tokenizer=None):
+                 unet_state=None, vae_state=None, graph_replay=True, defer_backward=False, tokenizer=None, strict=False):
         super().__init__()
+        # strict: every registry tensor must come from unet_state / vae_state and no other key is accepted (from_pretrained); by
+        # default absent tensors keep the seeded initialisation.  A tensor whose shape differs from the registry's is always refused.
         # tokenizer: a callable with CLIPTokenizer.__call__'s contract (e.g. CLIPTokenizer.from_pretrained(model_key, subfolder="tokenizer")),
         # used by get_text_embeds for prompts given as strings.  The text encoder itself is created when its weights are loaded.
         self.tokenizer = tokenizer
@@ -202,16 +347,30 @@ class StableDiffusion(nn.Module):
             is_vae = name.split(".")[0] in ("encoder", "quant_conv", "decoder", "post_quant_conv")
             src = (vae_state if is_vae else unet_state)
             # tensors absent from a given state (e.g. an encoder-only VAE state) keep the seeded default initialisation
+            if src is not None and name in src and tuple(src[name].shape) != tuple(shape):
+                raise L.Mi3dError(f"{name}: shape {tuple(src[name].shape)} in the state dict, the engine's configuration has {tuple(shape)}")
+            if strict and (src is None or name not in src):
+                raise L.Mi3dError(f"{name} is missing from the {'VAE' if is_vae else 'U-Net'} state dict")
             t = src[name].detach().float() if (src is not None and name in src) else _default_init(name, shape, gen)
             p = nn.Parameter(t.to(self.device).contiguous(), requires_grad=False)
             (self.vae if is_vae else self.unet)[name.replace(".", "/")] = p
             tensors[name] = p.data
+        if strict:
+            unexpected = sorted(set(unet_state or {}).union(vae_state or {}) - set(tensors))
+            if unexpected:
+                raise L.Mi3dError(f"{len(unexpected)} tensors of the state dicts have no place in the engine's configuration, e.g. {unexpected[:4]}")
         self.engine.load(tensors)
         self.num_train_timesteps = 1000
         self.min_step = int(self.num_train_timesteps * float(step_range[0]))
         self.max_step = int(self.num_train_timesteps * float(step_range[1]))
         self.alphas = alphas_cumprod().to(self.device)
         self._t = torch.zeros(1, dtype=torch.long, device=self.device)
+        # the sampler's DDIM settings (scheduler_config.json; from_pretrained reads them).  train_step never reads them: like the
+        # reference it consumes a v-prediction U-Net's output as epsilon.
+        for k, v in SD_SCHEDULER.items():
+            setattr(self, k, v)
+        self._schedules = {}          # (n, scheduler settings) -> device mi3d_sd_schedule table
+        self._size_engines = {}       # image size -> SDEngine planned on first use by produce_latents / decode_latents
 
     def load_diffusers_state_dict(self, unet_state=None, vae_state=None, text_encoder_state=None):
         """copy tensors named like diffusers' UNet2DConditionModel / AutoencoderKL state_dict()s and push them to the engine;
@@ -236,8 +395,111 @@ class StableDiffusion(nn.Module):
 
     def reload(self):
         """push the current parameter values into the engine again (after load_state_dict)."""
-        tensors = {k.replace("/", "."): v.data for k, v in list(self.unet.items()) + list(self.vae.items())}
-        self.engine.load(tensors)
+        tensors = self._tensors()
+        for eng in [self.engine] + list(self._size_engines.values()):
+            eng.load(tensors)
+
+    def _tensors(self):
+        return {k.replace("/", "."): v.data for k, v in list(self.unet.items()) + list(self.vae.items())}
+
+    def _engine_for(self, size, part):
+        """the engine whose `part` ("unet" or "vae") is planned for size x size images: the constructor's at its own size, else one
+        planned on first use per size and loaded from the same parameter tensors"""
+        if (self.unet_cfg["latent_hw"] * 8 if part == "unet" else self.vae_cfg["image_hw"]) == size:
+            return self.engine
+        eng = self._size_engines.get(size)
+        if eng is None:
+            try:
+                eng = SDEngine(dict(self.unet_cfg, latent_hw=size // 8), dict(self.vae_cfg, image_hw=size), self.device, graph_replay=self.graph_replay)
+            except L.Mi3dError as e:
+                raise L.Mi3dError(f"no SD engine plan for {size}x{size} images") from e
+            eng.load(self._tensors())
+            self._size_engines[size] = eng
+        return eng
+
+    def _schedule(self, n):
+        key = (n, self.timestep_spacing, self.steps_offset, self.set_alpha_to_one)
+        tab = self._schedules.get(key)
+        if tab is None:
+            rec = ddim_schedule(n, self.timestep_spacing, self.steps_offset, self.set_alpha_to_one)
+            tab = torch.from_numpy(rec.view(np.uint8).copy()).to(self.device)
+            self._schedules[key] = tab
+        return tab
+
+    def produce_latents(self, text_embeddings, height=512, width=512, num_inference_steps=50, guidance_scale=7.5, latents=None):
+        """nerf/sd.py:176-199: DDIM (eta 0) with classifier-free guidance from x_T to x_0, on the device (mi3d_sd_sample).
+        text_embeddings [2B,77,D] laid out [uncond x B, cond x B]; latents (x_T) [B,4,H/8,W/8], drawn with torch.randn when None
+        (DDIM's init_noise_sigma is 1).  The B samples run in turn: each is independent in the reference's batch too.  Square sizes
+        only, H a multiple of 64.  Returns fp32 [B,4,H/8,W/8]."""
+        if height != width or height <= 0 or height % 64:
+            raise L.Mi3dError(f"produce_latents takes square sizes with H a multiple of 64; got {height}x{width}")
+        D, hw = self.unet_cfg["cross_dim"], height // 8
+        te = text_embeddings
+        if not torch.is_tensor(te) or te.dim() != 3 or te.shape[0] == 0 or te.shape[0] % 2 or tuple(te.shape[1:]) != (77, D):
+            raise L.Mi3dError(f"text_embeddings must be [2B,77,{D}] ([uncond x B, cond x B]); got {tuple(getattr(te, 'shape', ()))}")
+        B = te.shape[0] // 2
+        if latents is None:
+            latents = torch.randn((B, 4, hw, hw), device=self.device)
+        elif tuple(latents.shape) != (B, 4, hw, hw):
+            raise L.Mi3dError(f"latents must be [{B},4,{hw},{hw}] for {B} prompt(s) at {height}x{width}; got {tuple(latents.shape)}")
+        L.require_cuda(te, latents)
+        sched = self._schedule(num_inference_steps)
+        eng = self._engine_for(height, "unet")
+        ptype = PREDICTION_TYPES[self.prediction_type]
+        te = L.f32c(te.detach())
+        out = latents.detach().to(torch.float32).clone(memory_format=torch.contiguous_format)
+        with eng.on_stream():
+            for b in range(B):
+                ctx = torch.stack([te[b], te[B + b]])
+                L.check(L.lib().mi3d_sd_sample(eng.h, L.ptr(out[b]), L.ptr(sched), C.c_int(num_inference_steps), C.c_int(ptype), L.ptr(ctx),
+                                               C.c_float(float(guidance_scale)), L.stream()), "sd_sample")
+        return out
+
+    def prompt_to_img(self, prompts, negative_prompts='', height=512, width=512, num_inference_steps=50, guidance_scale=7.5, latents=None):
+        """nerf/sd.py:222-238: get_text_embeds per prompt -> produce_latents -> decode_latents -> imgs [B,3,H,W] in [0,1].  prompts /
+        negative_prompts: a string or int64 token ids [1,77] / [77], or a list of them (strings need the tokenizer)."""
+        one = lambda p: [p] if isinstance(p, str) or torch.is_tensor(p) else list(p)
+        prompts, negs = one(prompts), one(negative_prompts)
+        if len(negs) == 1:
+            negs = negs * len(prompts)
+        if len(negs) != len(prompts):
+            raise L.Mi3dError(f"{len(prompts)} prompts but {len(negs)} negative prompts")
+        embeds = [self.get_text_embeds(p, n) for p, n in zip(prompts, negs)]
+        text_embeds = torch.cat([e[:1] for e in embeds] + [e[1:] for e in embeds])
+        latents = self.produce_latents(text_embeds, height=height, width=width, latents=latents, num_inference_steps=num_inference_steps,
+                                       guidance_scale=guidance_scale)
+        return self.decode_latents(latents)
+
+    @classmethod
+    def from_pretrained(cls, local_dir, device, step_range=[0.2, 0.6], graph_replay=True, defer_backward=False):
+        """A local diffusers directory (nothing is downloaded): unet/ and vae/ config.json + diffusion_pytorch_model[.fp16].safetensors,
+        text_encoder/ config.json + model[.fp16].safetensors, scheduler/scheduler_config.json, and tokenizer/ through transformers'
+        CLIPTokenizer when transformers imports (without it prompts must be token ids).  The engine is planned at 512 x 512, the size
+        train_step feeds (nerf/sd.py:124); other sampling sizes are planned on first use."""
+        sub = lambda *p: os.path.join(local_dir, *p)
+        unet_cfg = dict(unet_cfg_from_config(_read_json(sub("unet", "config.json"))), latent_hw=64)
+        vae_cfg = dict(vae_cfg_from_config(_read_json(sub("vae", "config.json"))), image_hw=512)
+        sched = scheduler_from_config(_read_json(sub("scheduler", "scheduler_config.json")))
+        te_cfg = _read_json(sub("text_encoder", "config.json"))
+        unet_state, vae_state = _read_weights(sub("unet"), "diffusion_pytorch_model"), _read_weights(sub("vae"), "diffusion_pytorch_model")
+        te_state = _read_weights(sub("text_encoder"), "model")
+        tokenizer = None
+        if os.path.isdir(sub("tokenizer")):
+            try:
+                from transformers import CLIPTokenizer
+            except ImportError:
+                CLIPTokenizer = None
+            if CLIPTokenizer is not None:
+                tokenizer = CLIPTokenizer.from_pretrained(sub("tokenizer"))
+        sd1 = unet_cfg.get("proj_conv", False)
+        self = cls(device, sd_version="1.5" if sd1 else "2.0", hf_key=os.path.abspath(local_dir), step_range=step_range, unet_cfg=unet_cfg,
+                   vae_cfg=vae_cfg, unet_state=unet_state, vae_state=vae_state, graph_replay=graph_replay, defer_backward=defer_backward,
+                   tokenizer=tokenizer, strict=True)
+        for k, v in sched.items():
+            setattr(self, k, v)
+        act = te_cfg.get("hidden_act", "quick_gelu")
+        self.text_encoder = TextEncoder(self.device, cfg=cfg_from_state_dict(te_state, hidden_act=act), state_dict=te_state, graph_replay=graph_replay)
+        return self
 
     def get_text_embeds(self, prompt, negative_prompt):
         """nerf/sd.py:68-85: [uncond, cond] text embeddings [2,77,D].  prompt / negative_prompt: a string, a list of one string, or
@@ -283,12 +545,17 @@ class StableDiffusion(nn.Module):
         return _EncodeImgs.apply(imgs, L.f32c(eps), self.engine)
 
     def decode_latents(self, latents):
-        """nerf/sd.py:201-210: (vae.decode(latents / 0.18215).sample / 2 + 0.5).clamp(0, 1) -> [1,3,S,S]; no gradient, like the reference"""
+        """nerf/sd.py:201-210: (vae.decode(latents / 0.18215).sample / 2 + 0.5).clamp(0, 1) -> [B,3,S,S]; no gradient, like the reference.
+        latents [B,4,h,w] with h = w a multiple of 8: the engine's own size, or another one planned on first use (S = 8h)."""
         latents = L.f32c(latents.detach())
-        S = self.vae_cfg["image_hw"]
-        imgs = torch.empty(1, 3, S, S, dtype=torch.float32, device=latents.device)
-        with self.engine.on_stream():
-            L.check(L.lib().mi3d_sd_decode(self.engine.h, L.ptr(latents), L.ptr(imgs), L.stream()), "sd_decode")
+        if latents.dim() != 4 or latents.shape[1] != 4 or latents.shape[2] != latents.shape[3] or latents.shape[2] % 8:
+            raise L.Mi3dError(f"decode_latents takes square latents [B,4,h,h] with h a multiple of 8; got {tuple(latents.shape)}")
+        S = latents.shape[2] * 8
+        eng = self._engine_for(S, "vae")
+        imgs = torch.empty(latents.shape[0], 3, S, S, dtype=torch.float32, device=latents.device)
+        with eng.on_stream():
+            for b in range(latents.shape[0]):
+                L.check(L.lib().mi3d_sd_decode(eng.h, L.ptr(latents[b]), L.ptr(imgs[b]), L.stream()), "sd_decode")
         return imgs
 
     def ddim_prev_sample(self, noise_pred, latents_noisy, t_dev):
@@ -387,3 +654,43 @@ class StableDiffusion(nn.Module):
         latents.backward(gradient=grad, retain_graph=True)
         self.last = dict(latents=latents.detach(), noise_pred=noise_pred, grad=grad, t=t_host)
         return loss, imgs
+
+
+def main(argv=None):
+    """nerf/sd.py:241-268: `python -m mi3d_b200.nerf.sd PROMPT --ckpt DIR` writes test_bench/<workspace>/<prompt>_<seed>.png for seeds
+    0..--seeds-1 (the reference's default of 0 writes nothing)"""
+    import argparse
+    parser = argparse.ArgumentParser(description="text-to-image with a local diffusers Stable Diffusion checkpoint")
+    parser.add_argument('prompt', type=str)
+    parser.add_argument('--ckpt', required=True, type=str, help="local diffusers directory (unet/, vae/, text_encoder/, scheduler/, tokenizer/)")
+    parser.add_argument('--negative', default='', type=str)
+    parser.add_argument('--workspace', default='', type=str)
+    parser.add_argument('--sd_version', type=str, default='2.0', choices=['1.5', '2.0'], help="stable diffusion version")
+    parser.add_argument('-H', type=int, default=512)
+    parser.add_argument('-W', type=int, default=512)
+    parser.add_argument('--seeds', type=int, default=0)
+    parser.add_argument('--steps', type=int, default=50)
+    opt = parser.parse_args(argv)
+
+    workspace = os.path.join('test_bench', opt.workspace)
+    os.makedirs(workspace, exist_ok=True)
+    sd = StableDiffusion.from_pretrained(opt.ckpt, torch.device('cuda'))
+    if (opt.sd_version == '1.5') != bool(sd.unet_cfg.get("proj_conv", False)):
+        raise L.Mi3dError(f"--sd_version {opt.sd_version} does not match {opt.ckpt}, an SD-{'1.x' if sd.unet_cfg.get('proj_conv') else '2.x'} U-Net")
+    for seed in range(opt.seeds):
+        torch.manual_seed(seed)
+        np.random.seed(seed)
+        imgs = sd.prompt_to_img(opt.prompt, opt.negative, opt.H, opt.W, opt.steps, guidance_scale=7.5)
+        img = (imgs[0].permute(1, 2, 0).clamp(0, 1) * 255 + 0.5).to(torch.uint8).cpu().numpy()    # torchvision save_image's rounding
+        path = os.path.join(workspace, opt.prompt.replace(" ", "_") + f'_{seed}.png')
+        try:
+            from PIL import Image
+            Image.fromarray(img).save(path)
+        except ImportError:
+            import cv2
+            cv2.imwrite(path, img[..., ::-1])
+        print(path)
+
+
+if __name__ == '__main__':
+    main()
