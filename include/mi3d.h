@@ -352,6 +352,23 @@ int mi3d_sumsq(const float* g, uint64_t n, float* out, int accumulate, void* wor
 int mi3d_adan_step(float* param, float* grad, float* exp_avg, float* exp_avg_sq, float* exp_avg_diff, float* neg_pre_grad, uint64_t n,
                    const float* total_sumsq, const mi3d_adan_cfg* cfg, mi3d_stream_t stream);
 
+/* nn.utils.clip_grad_norm(max_norm) (nerf/utils.py:984) + torch.optim.Adam.step() (main.py:133-134: `--optim adam|adamw`) on one
+ * parameter tensor, for a caller that launches once per tensor of the model. */
+typedef struct {
+    double lr;              /* group['lr'] */
+    double beta1, beta2, eps;   /* (0.9, 0.99), 1e-15 (main.py:134) */
+    int step;               /* the tensor's state['step'] AFTER the increment: 1 on the first call */
+    float clip_grad_norm;   /* Trainer's clip_grad_norm max_norm, 10; 0 = off */
+} mi3d_adam_cfg;
+/* total_sumsq: DEVICE scalar = squared L2 norm of ALL gradients of the model before clipping (mi3d_sumsq over every tensor); may be
+ * NULL when clip_grad_norm == 0.  With clip_grad_norm > 0, coef = clamp(clip_grad_norm / (sqrt(*total_sumsq) + 1e-6), max = 1) in
+ * fp32 and grad is rescaled in place (p.grad ends up clipped, as torch's clip_grad_norm_ leaves it).  Then torch's _multi_tensor_adam
+ * (capturable=False, amsgrad off, no weight decay) in its operation order: exp_avg.lerp_(g, 1 - beta1), exp_avg_sq.mul_(beta2)
+ * .addcmul_(g, g, 1 - beta2), param.addcdiv_(exp_avg, sqrt(exp_avg_sq) / (1 - beta2^step)^0.5 + eps, -lr / (1 - beta1^step)), the
+ * host scalars folded in double.  All n-element fp32 tensors are DEVICE and updated in place. */
+int mi3d_adam_step(float* param, float* grad, float* exp_avg, float* exp_avg_sq, uint64_t n, const float* total_sumsq,
+                   const mi3d_adam_cfg* cfg, mi3d_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------------
  * Planned engines: SD (B3), the SD-2 text encoder (B3'), CLIP (B4), the contextual loss (B6), the refine U-Net (B7), DPT (B8) and
  * BLIP-2 (B9).  Each is made by its mi3d_<engine>_workspace_bytes / mi3d_<engine>_create (HOST: bytes of device workspace the engine

@@ -62,6 +62,12 @@ class AdanCfg(C.Structure):
                 ("step", C.c_int), ("reset_prev", C.c_int)]
 
 
+class AdamCfg(C.Structure):
+    """mi3d_adam_cfg: one clip + torch.optim.Adam step of mi3d_adam_step"""
+    _fields_ = [("lr", C.c_double), ("beta1", C.c_double), ("beta2", C.c_double), ("eps", C.c_double), ("step", C.c_int),
+                ("clip_grad_norm", C.c_float)]
+
+
 class RenderArgs(C.Structure):
     _fields_ = [("rays_o", C.c_void_p), ("rays_d", C.c_void_p), ("depth_scale", C.c_void_p), ("raygen", C.POINTER(RayGen)), ("N", C.c_uint32),
                 ("n_views", C.c_uint32), ("density_bitfield", C.c_void_p), ("C", C.c_uint32), ("H", C.c_uint32), ("bound", C.c_float),
@@ -119,7 +125,7 @@ SYMBOLS = [
     "mi3d_render_workspace_bytes", "mi3d_render_workspace_carve", "mi3d_render_forward", "mi3d_render_backward",
     "mi3d_render_eval_workspace_bytes", "mi3d_render_eval",
     "mi3d_density_grid_workspace_bytes", "mi3d_density_grid_update", "mi3d_version",
-    "mi3d_sumsq_workspace_bytes", "mi3d_sumsq", "mi3d_adan_step",
+    "mi3d_sumsq_workspace_bytes", "mi3d_sumsq", "mi3d_adan_step", "mi3d_adam_step",
     "mi3d_gemm_f16", "mi3d_gemm_f16_splitk", "mi3d_flash_attn_f16", "mi3d_conv3x3_f16", "mi3d_tf32_tile_test", "mi3d_gemm_f16_bt",
     "mi3d_op_gemm", "mi3d_op_conv3", "mi3d_op_conv3_block", "mi3d_op_attention", "mi3d_op_attention_core", "mi3d_op_layernorm", "mi3d_op_layernorm_bwd",
     "mi3d_op_softmax", "mi3d_op_softmax_bwd", "mi3d_op_transpose",

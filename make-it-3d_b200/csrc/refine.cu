@@ -8,14 +8,15 @@
 //   2. k_refine_finish        one CTA: the partial sums in a fixed order -> bg_loss = 1e-3 sum, l1 = 1000 mean
 // Backward: k_refine_image_grad writes dL/dpred of both terms from pred, gt, mask and the saved dilation (torch's op order).
 //
-// Adam (torch.optim.Adam, foreach path, in its operation order): one launch over the concatenation of every parameter tensor, a
-// device table of segments.  Segment 0 may be the refine cloud's [P,19] buffer; its colour columns then get the gradient of the
-// two MSE regularisers added on the fly, and their values are reduced like the image losses.
+// Adam (torch.optim.Adam, foreach path, in its operation order: adam_update.cuh): one launch over the concatenation of every
+// parameter tensor, a device table of segments.  Segment 0 may be the refine cloud's [P,19] buffer; its colour columns then get the
+// gradient of the two MSE regularisers added on the fly, and their values are reduced like the image losses.
 //
 // Compiled with -fmad=false: every element-wise op rounds once, like torch's separate kernels; where torch's own kernels contract
 // to an FMA (lerp, addcmul, addcdiv) the fmaf is written out.
 #include <math.h>
 
+#include "adam_update.cuh"
 #include "mi3d_common.cuh"
 #include "../../include/mi3d.h"
 
@@ -136,14 +137,6 @@ k_refine_image_grad(const float* __restrict__ pred, const float* __restrict__ gt
     }
 }
 
-struct AdamScalars {
-    float w1;          // 1 - beta1: lerp weight
-    float beta2, omb2; // beta2, 1 - beta2
-    float step_size;   // -(lr / (1 - beta1^t))
-    float bc2_sqrt;    // (1 - beta2^t)^0.5
-    float eps;
-};
-
 struct RegArgs {
     const float* origin;     // [P,3] colour origins (NULL: no regulariser)
     uint32_t p_cano, p_novel;
@@ -152,7 +145,7 @@ struct RegArgs {
 };
 
 __global__ void __launch_bounds__(kAdamThreads)
-k_refine_adam(const mi3d_adam_segment* __restrict__ segs, int n_segs, unsigned long long total, AdamScalars a, RegArgs r,
+k_refine_adam(const mi3d_adam_segment* __restrict__ segs, int n_segs, unsigned long long total, const mi3d_adam::Scalars a, RegArgs r,
               double2* __restrict__ partials) {
     __shared__ unsigned long long s_off[kMaxSegs + 1];
     __shared__ double s_a[kAdamThreads], s_b[kAdamThreads];
@@ -172,7 +165,7 @@ k_refine_adam(const mi3d_adam_segment* __restrict__ segs, int n_segs, unsigned l
         }
         const mi3d_adam_segment& s = segs[lo];
         const unsigned long long i = e - s_off[lo];
-        const float p = s.param[i];
+        float p = s.param[i];
         float g = s.grad[i];
         if (lo == 0 && r.origin) {
             const uint32_t row = (uint32_t)(i / kCols), col = (uint32_t)(i % kCols);
@@ -184,12 +177,11 @@ k_refine_adam(const mi3d_adam_segment* __restrict__ segs, int n_segs, unsigned l
                 if (cano) rc += sq; else rn += sq;
             }
         }
-        const float m = fmaf(a.w1, g - s.exp_avg[i], s.exp_avg[i]);
-        const float v = fmaf(a.omb2, g * g, s.exp_avg_sq[i] * a.beta2);
-        const float denom = sqrtf(v) / a.bc2_sqrt + a.eps;
+        float m = s.exp_avg[i], v = s.exp_avg_sq[i];
+        mi3d_adam::update(p, m, v, g, a);
         s.exp_avg[i] = m;
         s.exp_avg_sq[i] = v;
-        s.param[i] = fmaf(a.step_size, m / denom, p);
+        s.param[i] = p;
     }
     if (partials) {
         block_sum2<kAdamThreads>(rc, rn, s_a, s_b);
@@ -244,15 +236,7 @@ int mi3d_refine_adam(const mi3d_adam_segment* segs, int n_segs, unsigned long lo
                      void* workspace, size_t workspace_bytes, mi3d_stream_t stream) {
     if (!segs || n_segs < 1 || n_segs > kMaxSegs || total == 0 || step < 1) return MI3D_ERR_ARG;
     if (origin && (!reg || !workspace || workspace_bytes < mi3d_refine_adam_workspace_bytes(total))) return MI3D_ERR_ARG;
-    // torch.optim.Adam's host scalars, computed as it computes them (Python floats are C doubles; ** is pow)
-    const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
-    AdamScalars a;
-    a.w1 = (float)(1.0 - beta1);
-    a.beta2 = (float)beta2;
-    a.omb2 = (float)(1.0 - beta2);
-    a.step_size = (float)((lr / bc1) * -1.0);
-    a.bc2_sqrt = (float)pow(bc2, 0.5);
-    a.eps = (float)eps;
+    const mi3d_adam::Scalars a = mi3d_adam::host_scalars(lr, beta1, beta2, eps, step);
     RegArgs r;
     r.origin = origin;
     r.p_cano = p_cano;

@@ -6,8 +6,8 @@ nerf/utils.py:461-574, :947-1027) on libmi3d.so.
 * `CoarseStep(model, guidance, clip_model, optimizer, opt, ref_imgs, depth_prediction, depth_mask, text_z, clip_text_tokens)`: the
   state of one coarse run.  `step(data, global_step, ...)` runs one iteration as one autograd graph with ONE backward (the SDS
   gradient enters as `StableDiffusion.train_step(defer=True)`'s surrogate instead of a second walk of the render graph), then one
-  `Adan.step()` with the Trainer's `clip_grad_norm(10)` folded in.  It returns the loss terms as device scalars and never
-  synchronises the host.
+  `Adan.step()` or `Adam.step()` (`--optim adan` / `adam|adamw`) with the Trainer's `clip_grad_norm(10)` folded in.  It returns
+  the loss terms as device scalars and never synchronises the host.
 * `train_step(trainer, data)` / `train_one_epoch(trainer, loader)`: drop-ins for the two Trainer methods.  Swap them together:
   `train_step` already runs the backward and the update, so the reference's `train_one_epoch` must not run them again.
 
@@ -32,7 +32,7 @@ import torch
 import torch.nn.functional as F
 
 from .. import _lib as L
-from ..optimizer import Adan
+from ..optimizer import Adam, Adan
 from .refine import _png
 from .utils import safe_normalize
 
@@ -125,12 +125,13 @@ class CoarseStep:
             raise L.Mi3dError(f"CoarseStep: the reference image must be RGBA [1,4,{REF_HW},{REF_HW}] (main.py:184), got {tuple(ref_imgs.shape)}")
         if depth_prediction.numel() != REF_HW * REF_HW or depth_mask.numel() != REF_HW * REF_HW:
             raise L.Mi3dError(f"CoarseStep: depth_prediction and depth_mask must hold {REF_HW} x {REF_HW} values")
-        if not isinstance(optimizer, Adan):
-            raise L.Mi3dError("CoarseStep: the optimizer must be this package's Adan (optimizer.Adan)")
+        if not isinstance(optimizer, (Adan, Adam)):
+            raise L.Mi3dError("CoarseStep: the optimizer must be this package's Adan or Adam (optimizer.Adan / optimizer.Adam)")
         if optimizer.clip_grad_norm == 0.0:
             optimizer.clip_grad_norm = CLIP_GRAD_NORM            # the Trainer's clip_grad_norm(model.parameters(), 10), folded in
         elif optimizer.clip_grad_norm != CLIP_GRAD_NORM:
-            raise L.Mi3dError(f"CoarseStep: Adan(clip_grad_norm={optimizer.clip_grad_norm}) given; the Trainer clips at {CLIP_GRAD_NORM}")
+            raise L.Mi3dError(f"CoarseStep: {type(optimizer).__name__}(clip_grad_norm={optimizer.clip_grad_norm}) given; "
+                              f"the Trainer clips at {CLIP_GRAD_NORM}")
         tokens = clip_text_tokens.to(torch.long)
         if tokens.dim() != 2 or tokens.shape[0] != len(text_z):
             raise L.Mi3dError(f"CoarseStep: clip_text_tokens must be [{len(text_z)},77] int64, one row per text entry; got {tuple(tokens.shape)}")

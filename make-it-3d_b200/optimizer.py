@@ -13,6 +13,8 @@ Multi-GPU (`group=` / an initialised default process group with world_size > 1),
     small tensors (the 6 MLP tensors, 26 KB): all-reduce(SUM), identical replicated update on every rank.
 Call it INSTEAD of parallel.GradientAllReduce + a separate optimizer step.  The result equals the single-process reference update on
 the summed gradients (tests/test_adan_gpu.py, tests/golden/adan.npz recorded from the reference's optimizer.py).
+
+`Adam`: torch.optim.Adam for `--optim adam|adamw` (main.py:133-134), single-GPU, with the same clip folded in (csrc/adam.cu).
 """
 import ctypes as C
 
@@ -133,3 +135,113 @@ class Adan(torch.optim.Optimizer):
             elif g.data_ptr() != p.grad.data_ptr():
                 p.grad.copy_(g.view_as(p.grad))
         return loss
+
+
+class Adam(torch.optim.Optimizer):
+    """`torch.optim.Adam` for `--optim adam|adamw` (main.py:133-134: Adam(model.get_params(opt.lr), betas=(0.9, 0.99), eps=1e-15)) on
+    libmi3d.so, with the Trainer's `nn.utils.clip_grad_norm(model.parameters(), max_norm)` (nerf/utils.py:984) folded in when
+    clip_grad_norm > 0.
+
+    One `step()` = one deterministic sum-of-squares pass per tensor into a device scalar (mi3d_sumsq, only when clipping), then one
+    elementwise launch per tensor (mi3d_adam_step): clip, then torch's foreach Adam in its operation order.  The host never
+    synchronises.  Parameter groups, `group['lr']` (read every step, so lr schedulers work) and the per-parameter state (`step` a
+    CPU fp32 scalar tensor, `exp_avg`, `exp_avg_sq`) are torch's, so state dicts interchange with `torch.optim.Adam` both ways.
+    Parameters whose `.grad` is None are skipped, as torch skips them.  Refused with Mi3dError: weight decay, amsgrad, maximize,
+    capturable, differentiable, fused=True, parameters that are not contiguous fp32 CUDA tensors, and a process group of more than
+    one rank."""
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, amsgrad=False, *, foreach=None, maximize=False,
+                 capturable=False, differentiable=False, fused=None, decoupled_weight_decay=False, clip_grad_norm=0.0):
+        if not 0.0 <= lr or not 0.0 <= eps or not all(0.0 <= b < 1.0 for b in betas) or not 0.0 <= weight_decay:
+            raise ValueError("invalid Adam hyper-parameter")
+        if not 0.0 <= clip_grad_norm:
+            raise ValueError(f"invalid clip_grad_norm: {clip_grad_norm}")
+        defaults = dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, amsgrad=amsgrad, maximize=maximize, foreach=foreach,
+                        capturable=capturable, differentiable=differentiable, fused=fused, decoupled_weight_decay=decoupled_weight_decay)
+        _adam_check_world()
+        super().__init__(params, defaults)
+        self.clip_grad_norm = float(clip_grad_norm)
+        self._scratch = {}
+
+    def add_param_group(self, param_group):
+        super().add_param_group(param_group)
+        group = self.param_groups[-1]
+        _adam_check_group(group)
+        for p in group["params"]:
+            _adam_check_param(p)
+
+    def _dev_scratch(self, device):
+        key = str(device)
+        if key not in self._scratch:
+            self._scratch[key] = dict(ws=torch.empty(L.lib().mi3d_sumsq_workspace_bytes(), dtype=torch.uint8, device=device),
+                                      sumsq=torch.zeros(1, dtype=torch.float32, device=device))
+        return self._scratch[key]
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        _adam_check_world()
+        items = []          # (group, param, contiguous fp32 grad)
+        for group in self.param_groups:
+            _adam_check_group(group)
+            for p in group["params"]:
+                if p.grad is None:
+                    continue
+                _adam_check_param(p)
+                L.require_cuda(p.grad)
+                items.append((group, p, L.f32c(p.grad)))
+        if not items:
+            return loss
+        lib = L.lib()
+        devices = {p.device for _, p, _ in items}
+        if len(devices) != 1:
+            raise L.Mi3dError("Adam: all parameters must be on one GPU")
+        sumsq = None
+        if self.clip_grad_norm > 0:
+            sc = self._dev_scratch(items[0][1].device)
+            sumsq = sc["sumsq"]
+            for k, (_, _, g) in enumerate(items):
+                L.check(lib.mi3d_sumsq(L.ptr(g), C.c_uint64(g.numel()), L.ptr(sumsq), C.c_int(1 if k else 0), L.ptr(sc["ws"]), L.stream()),
+                        "sumsq")
+        for group, p, g in items:
+            st = self.state[p]
+            if len(st) == 0:                                              # torch's Adam._init_group
+                st["step"] = torch.tensor(0.0, dtype=torch.float32)
+                st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+            if st["step"].is_cuda:
+                raise L.Mi3dError("Adam: state['step'] must be a CPU tensor (a capturable / fused state dict was loaded)")
+            st["step"] += 1                                               # CPU tensor: no synchronisation
+            cfg = L.AdamCfg()
+            cfg.lr = float(group["lr"]); cfg.beta1, cfg.beta2 = (float(b) for b in group["betas"]); cfg.eps = float(group["eps"])
+            cfg.step = int(st["step"].item()); cfg.clip_grad_norm = self.clip_grad_norm
+            L.check(lib.mi3d_adam_step(L.ptr(p.data), L.ptr(g), L.ptr(st["exp_avg"]), L.ptr(st["exp_avg_sq"]), C.c_uint64(p.numel()),
+                                       L.ptr(sumsq), C.byref(cfg), L.stream()), "adam_step")
+            if sumsq is not None and g.data_ptr() != p.grad.data_ptr():
+                p.grad.copy_(g.view_as(p.grad))
+        return loss
+
+
+def _adam_check_world():
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+        raise L.Mi3dError("Adam: multi-GPU (a process group of more than one rank) is not built; use Adan(group=...) there")
+
+
+def _adam_check_group(group):
+    for key, refused in (("amsgrad", True), ("maximize", True), ("capturable", True), ("differentiable", True), ("fused", True)):
+        if group.get(key) == refused:
+            raise L.Mi3dError(f"Adam: {key}=True is not built")
+    if group.get("weight_decay", 0) != 0:
+        raise L.Mi3dError(f"Adam: weight_decay={group['weight_decay']} is not built (main.py's Adam has none)")
+    if torch.is_tensor(group["lr"]) and group["lr"].is_cuda:
+        raise L.Mi3dError("Adam: a CUDA tensor lr would synchronise the host every step")
+
+
+def _adam_check_param(p):
+    if p.dtype != torch.float32 or not p.is_contiguous():
+        raise L.Mi3dError("Adam: parameters must be contiguous fp32")
+    if not p.is_cuda:
+        raise L.Mi3dError("Adam: parameters must be CUDA tensors (there is no CPU path)")
