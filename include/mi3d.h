@@ -398,37 +398,14 @@ int mi3d_engine_debug_tensor(mi3d_engine_t h, const char* name, void** ptr, size
  * B3: Stable-Diffusion guidance  (replaces the diffusers/cuDNN/cuBLAS calls behind nerf/sd.py:117-174, :212-220)
  * ------------------------------------------------------------------------------------------------------ */
 
-/* The one tensor-core tile kernel (wgmma with register accumulators + TMA operand staging) exposed directly:
- *   out[M,N] = alpha * A[M,K] . B[N,K]^T + bias[N] (+ residual[M,N]);  A, B fp16 K-major; out fp16 or fp32.
- * Stands in for the cuBLAS GEMM under every nn.Linear of diffusers' UNet2DConditionModel / AutoencoderKL
- * (nerf/sd.py:146, :217).  M % 128 == 0, K % 64 == 0, N % block_n == 0 (block_n in {64,128,160,256}; 0 = auto).
- * epi_mode: 0 plain, 1 GEGLU (rows of B interleaved value/gate; out is [M, N/2]), 2 transposed store (out is [N, M]). */
-int mi3d_gemm_f16(const void* a, const void* b, void* out, int out_is_f32, int M, int N, int K, int block_n, float alpha,
-                  const float* bias, const void* residual, int epi_mode, mi3d_stream_t stream);
-
-/* Split-K form used for the deep U-Net levels (M = 128 .. 512 rows, K up to 23 040): `splits` K-ranges per output tile run on
- * different SMs and meet by fp32 RED in ws ([M][N] floats, zeroed inside); bias / residual / fp16 conversion happen in a
- * second pass.  fp16 output, plain epilogue only. */
-int mi3d_gemm_f16_splitk(const void* a, const void* b, void* out, int M, int N, int K, int block_n, int splits, float alpha,
-                         const float* bias, const void* residual, void* ws, mi3d_stream_t stream);
-
-/* Fused multi-head attention, head_dim 64 (stands in for diffusers' attention processor inside BasicTransformerBlock.attn1 /
- * .attn2, nerf/sd.py:146): o = softmax(q k^T / 8) v per (batch, head), scores kept in registers.  Other head dims: mi3d_op_attention_core.
- * q [B*T, ldq], k and v [B*Tk, ldk / ldv], o [B*T, ldo], fp16, head h at columns [64h, 64h+64); only the first Tk_valid keys of
- * every batch take part (77 of the 128 padded text rows for cross attention).  All ld % 8 == 0. */
-int mi3d_flash_attn_f16(const void* q, const void* k, const void* v, void* o, int B, int T, int Tk, int Tk_valid, int heads,
-                        int ldq, int ldk, int ldv, int ldo, mi3d_stream_t stream);
-
-/* Implicit-GEMM 3x3 stride-1 pad-1 convolution on the same kernel (stands in for the cuDNN conv under diffusers'
- * ResnetBlock2D / Downsample2D / Upsample2D): x [N,H,W,Cin] fp16 NHWC, w [Cout][3][3][Cin] fp16, y [N,H,W,Cout] fp16. */
-/* test path: out[M,N] (fp32) = A[M,K] . Bt[K,N], B consumed as an MN-major UMMA operand */
-int mi3d_gemm_f16_bt(const void* a, const void* bt, void* out, int M, int N, int K, int block_n, mi3d_stream_t stream);
-
-int mi3d_conv3x3_f16(const void* x, const void* w, void* y, int Nimg, int H, int W, int Cin, int Cout, int block_n,
-                     const float* bias, const void* residual, mi3d_stream_t stream);
-
-/* Test path: one op of the engines' shared op layer (plan::Builder / plan::TowerBuilder), recorded through the same builder method
- * the engines call (block-N choice, split-K planning, m_valid and tensor-map encoding included) and run eagerly on `stream`.
+/* The op layer every planned engine is built on, one op at a time: the test surface of the tensor-core tile kernel (wgmma with
+ * register accumulators + TMA operand staging; the GEMMs and implicit 3x3 convs that stand in for cuBLAS / cuDNN under diffusers'
+ * UNet2DConditionModel / AutoencoderKL, nerf/sd.py:146, :217), of the fused attention and of the row kernels.  Each call records one
+ * op through the same plan::Builder / plan::TowerBuilder method the engines call (block-N choice, split-K planning, m_valid and
+ * tensor-map encoding included) and runs it eagerly on `stream`.
+ * mi3d_op_gemm: y = alpha * A . B^T + bias[N] + row_bias[m / rows_per_group] (+ residual), A [a_rows][K] and B [N][K] fp16 K-major,
+ * out fp16 (out16) or fp32 (out32).  mode: 0 plain, 1 GEGLU (rows of B interleaved value / gate; out is [M, N/2]), 2 transposed
+ * store (out is [N, M]), 3 / 4 quick-GELU and its input gradient (aux: the pre-activation), 7 GELU.
  * plan (nullable, int[2]): receives the tile kernel's block-N and split count the builder planned.
  * splitk_ws / splitk_bytes: the fp32 split-K scratch the builder may plan into (NULL / 0: no split-K). */
 typedef struct {

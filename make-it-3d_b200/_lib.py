@@ -126,7 +126,7 @@ SYMBOLS = [
     "mi3d_render_eval_workspace_bytes", "mi3d_render_eval",
     "mi3d_density_grid_workspace_bytes", "mi3d_density_grid_update", "mi3d_version",
     "mi3d_sumsq_workspace_bytes", "mi3d_sumsq", "mi3d_adan_step", "mi3d_adam_step",
-    "mi3d_gemm_f16", "mi3d_gemm_f16_splitk", "mi3d_flash_attn_f16", "mi3d_conv3x3_f16", "mi3d_tf32_tile_test", "mi3d_gemm_f16_bt",
+    "mi3d_tf32_tile_test",
     "mi3d_op_gemm", "mi3d_op_conv3", "mi3d_op_conv3_block", "mi3d_op_attention", "mi3d_op_attention_core", "mi3d_op_layernorm", "mi3d_op_layernorm_bwd",
     "mi3d_op_softmax", "mi3d_op_softmax_bwd", "mi3d_op_transpose",
     "mi3d_engine_destroy", "mi3d_engine_num_params", "mi3d_engine_param_name", "mi3d_engine_param_shape", "mi3d_engine_load_param",

@@ -49,7 +49,6 @@ struct GemmParams {
     int conv_H, conv_W, conv_bw, conv_bh, cin_blocks;
     int a_z1, b_z1;              // batch decomposition of blockIdx.z for A and B maps; b_batched = 0 -> weights shared
     int b_batched;
-    int b_mn;                    // 1: B is given as [K][N] (N contiguous) and used as an MN-major operand (test path)
     // epilogue
     __half* out;                 // fp16 output or nullptr
     float* out_f32;              // fp32 output or nullptr
@@ -131,13 +130,13 @@ __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + er
 __device__ __forceinline__ float quick_gelu(float x) { return x / (1.f + __expf(-1.702f * x)); }
 __device__ __forceinline__ float quick_gelu_grad(float x) { const float s = 1.f / (1.f + __expf(-1.702f * x)); return s * (1.f + 1.702f * x * (1.f - s)); }
 
-// acc (+)= A[64 x 16] . B[BLOCK_N x 16]^T ; TB = 1: B is MN-major
-template <int BLOCK_N, int TB>
+// acc (+)= A[64 x 16] . B[BLOCK_N x 16]^T, both K-major
+template <int BLOCK_N>
 __device__ __forceinline__ void mma_tile(float (&acc)[BLOCK_N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
-    if constexpr (BLOCK_N == 64) wg::wgmma_f16_n64<0, TB>(acc, da, db, accumulate);
-    else if constexpr (BLOCK_N == 128) wg::wgmma_f16_n128<0, TB>(acc, da, db, accumulate);
-    else if constexpr (BLOCK_N == 160) wg::wgmma_f16_n160<0, TB>(acc, da, db, accumulate);
-    else wg::wgmma_f16_n256<0, TB>(acc, da, db, accumulate);
+    if constexpr (BLOCK_N == 64) wg::wgmma_f16_n64<0, 0>(acc, da, db, accumulate);
+    else if constexpr (BLOCK_N == 128) wg::wgmma_f16_n128<0, 0>(acc, da, db, accumulate);
+    else if constexpr (BLOCK_N == 160) wg::wgmma_f16_n160<0, 0>(acc, da, db, accumulate);
+    else wg::wgmma_f16_n256<0, 0>(acc, da, db, accumulate);
 }
 
 // The kernel body.  kQuickGelu: the instantiation that also carries the EPI_QUICKGELU* epilogues; kVgg: the one that carries the
@@ -195,10 +194,6 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUt
                 if (elect_one()) {
                     mbar_arrive_expect_tx(&full_bar[stage], C::kStageBytes);
                     tma_load_4d(&map_a, &full_bar[stage], sa, c0, c1, c2, c3);
-                    if (p.b_mn) {
-                        #pragma unroll
-                        for (int nb = 0; nb < BLOCK_N / 64; nb++) tma_load_4d(&map_b, &full_bar[stage], sb + nb * 8192, n0 + nb * 64, kb * BLOCK_K, 0, 0);
-                    } else
                     tma_load_4d(&map_b, &full_bar[stage], sb, kb * BLOCK_K, n0, bz0, bz1);
                 }
                 __syncwarp();
@@ -223,17 +218,10 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUt
                 const uint32_t sa = tiles_u + (uint32_t)stage * (uint32_t)C::kStageBytes;
                 const uint64_t da = wg::desc_sw128(sa + (uint32_t)g * 8192u);            // 64 rows x 128 B further down the A tile
                 wg::fence();
-                if (p.b_mn) {
-                    const uint64_t db = wg::desc_sw128(sa + C::kABytes, 8192u);
-                    #pragma unroll
-                    for (int k = 0; k < BLOCK_K / MMA_K; k++)                              // MN-major B: 16 K-rows = 2048 B (>>4 => +128)
-                        mma_tile<BLOCK_N, 1>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(128 * k), (kb > kb0 || k > 0) ? 1u : 0u);
-                } else {
-                    const uint64_t db = wg::desc_sw128(sa + C::kABytes);
-                    #pragma unroll
-                    for (int k = 0; k < BLOCK_K / MMA_K; k++)                              // +32 B inside the swizzle row (>>4 => +2)
-                        mma_tile<BLOCK_N, 0>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb > kb0 || k > 0) ? 1u : 0u);
-                }
+                const uint64_t db = wg::desc_sw128(sa + C::kABytes);
+                #pragma unroll
+                for (int k = 0; k < BLOCK_K / MMA_K; k++)                                  // +32 B inside the swizzle row (>>4 => +2)
+                    mma_tile<BLOCK_N>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb > kb0 || k > 0) ? 1u : 0u);
                 wg::commit();
                 wg::wait<1>();                                   // the previous stage's MMAs have retired: hand its buffers back
                 if (prev >= 0 && lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&empty_bar[prev])) : "memory");

@@ -91,7 +91,6 @@ inline int launch_bn(const CUtensorMap& ma, const CUtensorMap& mb, const GemmPar
 
 inline int launch(const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams& p, int block_n, int batch, cudaStream_t st) {
     if (p.K % BLOCK_K || p.N % block_n || p.out_z1 < 1) return MI3D_ERR_ARG;
-    if (p.b_mn && block_n % 64) return MI3D_ERR_ARG;                                   // MN-major B is loaded in 64-column boxes
     if (((uintptr_t)p.bias | (uintptr_t)p.row_bias | (uintptr_t)p.splitk_ws) & 15) return MI3D_ERR_ARG;     // read / RED-added 16 bytes at a time
     if (p.conv == 2 || p.epi_mode == EPI_RELU || p.epi_mode == EPI_RELU_BWD) {
         if (p.splits > 1 || (p.epi_mode == EPI_RELU_BWD && !p.aux)) return MI3D_ERR_ARG;

@@ -41,7 +41,7 @@ __device__ __forceinline__ void issue_3tf32(float (&d)[N / 2], uint32_t a_hi, ui
 // ---------------------------------------------------------------------------------------------------------------------
 // bf16 3-way split tiles (wgmma bf16): x = h + m + l (each bf16, together ~24 bits) -> fp32-class products,
 // used by the fused field BACKWARD because 16-bit operands may be consumed MN-major (tf32 wgmma is K-major only;
-// the 16-bit MN-major descriptor form is also exercised by mi3d_gemm_f16_bt).
+// the MN-major operands are held element-wise to fp64 by the field backward's parity tests).
 // Storage: [rows][64 bf16] = 128-byte rows, 8-row swizzle atoms; the same tile is read K-major (rows = M/N, +32 B per
 // K = 16 step) or MN-major (rows = K, +2048 B per K = 16 step, LBO = distance to the next 64-column block).
 // ---------------------------------------------------------------------------------------------------------------------

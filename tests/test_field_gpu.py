@@ -1,7 +1,8 @@
-"""GPU parity (through the C ABI): hash grid, fused field forward/backward, fused render step vs the oracle and vs the
-golden vectors recorded from the reference's Python.  Tolerances (fp32 path): 1e-3 relative is BASELINE.json's bar; these
-tests hold the fp32 kernels to much tighter bounds and say so per assertion."""
+"""GPU parity (through the C ABI): hash grid, the field forward's tf32 split tiles, fused field forward/backward, fused render
+step vs the oracle and vs the golden vectors recorded from the reference's Python.  Tolerances (fp32 path): 1e-3 relative is
+BASELINE.json's bar; these tests hold the fp32 kernels to much tighter bounds and say so per assertion."""
 import argparse
+import ctypes as C
 import importlib
 
 import numpy as np
@@ -12,6 +13,11 @@ from conftest import load_golden
 from helpers import field_from_golden, fr, make_table, max_abs, orm, rel_err, sphere_bitfield
 
 pytestmark = pytest.mark.gpu
+
+
+@pytest.fixture(scope="module")
+def L():
+    return importlib.import_module("make-it-3d_b200._lib")
 
 
 def _cu(a):
@@ -90,6 +96,19 @@ def test_field_forward_backward_vs_torch_oracle(shading, ratio):
             assert max_abs(p.grad.cpu(), q.grad) / scale < 2e-3, (lyr, tuple(q.shape))
     gt, gr = net.encoder.params.grad.cpu().numpy(), field.encoder.params.grad.numpy()
     assert max_abs(gt, gr) / max(1e-6, np.abs(gr).max()) < 2e-3
+
+
+@pytest.mark.parametrize("N,K", [(64, 32), (64, 64), (32, 64), (16, 64), (64, 128), (32, 128)])
+def test_tf32_split_tiles(L, N, K):
+    """Hand-written wgmma tf32 tiles of the field FORWARD kernel (K-major operands): the 3-term split must be fp32-class.
+    (tf32 wgmma reads K-major operands only, which is why the backward uses bf16 tiles.)"""
+    g = torch.Generator(device="cuda").manual_seed(N + K)
+    a = torch.randn(128, K, device="cuda", generator=g); b = torch.randn(N, K, device="cuda", generator=g); ref = a.double() @ b.double().t()
+    d = torch.empty(128, N, device="cuda")
+    L.check(L.lib().mi3d_tf32_tile_test(L.ptr(a), L.ptr(b), L.ptr(d), C.c_int(N), C.c_int(K), C.c_int(0), L.stream()), "tf32_tile_test")
+    torch.cuda.synchronize()
+    err = (d.double() - ref).abs().max().item()
+    assert err < 2e-5 * max(1.0, ref.abs().max().item()), (N, K, err)     # plain tf32 would be ~1e-2
 
 
 def test_density_matches_oracle_and_k1_backward():
