@@ -21,6 +21,8 @@
 #pragma once
 #include <cmath>
 #include "tc_host.cuh"
+#include "tma.cuh"
+#include "wgmma.cuh"
 
 namespace attn {
 using namespace tc;
@@ -39,8 +41,6 @@ template <int D> struct Shape {
     static_assert(D % 8 == 0 && D >= 16 && kChunks <= 3 && (kTail == 64 || kTail == 40 || kTail == 32 || kTail == 16), "head_dim");
     static_assert(kSmemBytes <= 227 * 1024, "shared memory");
 };
-
-inline bool supported(int d) { return d == 40 || d == 64 || d == 80 || d == 160; }
 
 struct Params {
     int T;              // queries per (batch, head)
@@ -226,50 +226,6 @@ k_flash_attn(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ 
             for (int jj = 0; jj < D / 8; jj++)
                 *reinterpret_cast<__half2*>(dst + 8 * jj) = __floats2half2_rn(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
         }
-    }
-}
-
-struct Maps { CUtensorMap q, k, v; int d = 64; };
-
-// token matrices: x[(b * tokens + t) * ld + h * d + i]; every ld and the head stride 2 d bytes are multiples of 16 bytes
-inline int make_maps(Maps* m, const __half* q, long long ldq, const __half* k, long long ldk, const __half* v, long long ldv,
-                     int B, int T, int Tk, int heads, int d) {
-    if (!supported(d)) return MI3D_ERR_ARG;
-    m->d = d;
-    const uint32_t kv_rows = d > 128 ? 64 : 128;          // Shape<d>::kKeys
-    auto one = [&](CUtensorMap* map, const __half* base, long long ld, int tokens, uint32_t rows) {
-        const uint64_t dims[4] = {(uint64_t)d, (uint64_t)tokens, (uint64_t)heads, (uint64_t)B};
-        const uint64_t str[4] = {2, (uint64_t)ld * 2, (uint64_t)d * 2, (uint64_t)tokens * (uint64_t)ld * 2};
-        const uint32_t box[4] = {64, rows, 1, 1};
-        return make_map_f16(map, base, dims, str, box);
-    };
-    int r = one(&m->q, q, ldq, T, 128);
-    if (r) return r;
-    r = one(&m->k, k, ldk, Tk, kv_rows);
-    if (r) return r;
-    return one(&m->v, v, ldv, Tk, kv_rows);
-}
-
-template <int D> static inline int launch_d(const Maps& m, __half* o, long long ldo, int B, int T, int kv_valid, int heads, cudaStream_t st) {
-    static bool attr = false;
-    if (!attr) {
-        MI3D_CHECK(cudaFuncSetAttribute(k_flash_attn<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Shape<D>::kSmemBytes));
-        attr = true;
-    }
-    Params p; p.T = T; p.kv_valid = kv_valid; p.ldo = (int)ldo; p.scale_log2e = (float)(1.4426950408889634 / std::sqrt((double)D)); p.o = o;
-    dim3 grid((unsigned)((T + 127) / 128), (unsigned)heads, (unsigned)B);
-    k_flash_attn<D><<<grid, kThreads, Shape<D>::kSmemBytes, st>>>(m.q, m.k, m.v, p);
-    return (int)cudaGetLastError();
-}
-
-static inline int launch(const Maps& m, __half* o, long long ldo, int B, int T, int kv_valid, int heads, cudaStream_t st) {
-    if (kv_valid < 1 || T < 1) return MI3D_ERR_ARG;
-    switch (m.d) {
-        case 40: return launch_d<40>(m, o, ldo, B, T, kv_valid, heads, st);
-        case 64: return launch_d<64>(m, o, ldo, B, T, kv_valid, heads, st);
-        case 80: return launch_d<80>(m, o, ldo, B, T, kv_valid, heads, st);
-        case 160: return launch_d<160>(m, o, ldo, B, T, kv_valid, heads, st);
-        default: return MI3D_ERR_ARG;
     }
 }
 

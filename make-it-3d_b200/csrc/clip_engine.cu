@@ -10,6 +10,7 @@
 // fp16 copies (plus transposed copies for the input-gradient GEMMs) of the fp32 openai parameters.  The CLIP weights are frozen: the
 // backward computes the input gradient only.  No split-K and no atomics: results are bit-reproducible run to run and under graph replay.
 #include "transformer_plan.cuh"
+#include "clip_kernels.cuh"
 
 namespace clip {
 
@@ -61,13 +62,6 @@ struct Engine : TowerBuilder {
         return a;
     }
 
-    // dx = LayerNorm input gradient of dy (+ add)
-    void layernorm_bwd(const __half* x, const __half* dy, const float* gamma, const __half* add, __half* dx, long long rows, int C) {
-        push([=](cudaStream_t st) {
-            clipk::k_layernorm_bwd<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(x, dy, gamma, add, dx, (int)rows, C, 1e-5f);
-            return (int)cudaGetLastError();
-        });
-    }
     void block_bwd(const Tower& t, const BlockW& w, const BlockA& a, int n, const __half* dout, __half* dx) {
         const int C = t.C, Tp = t.Tpad; const long long M = (long long)n * Tp;
         {   // c_proj input gradient, times QuickGELU'(pre-activation)
@@ -84,13 +78,7 @@ struct Engine : TowerBuilder {
         bgemm(heads_rows(bw.dao, C, t), heads_rows(a.qkv + 2 * C, 3 * C, t), Tp, bw.dS, Tp, 0, (long long)Tp * Tp, 1, n, t);
         transpose(a.S, bw.PT, n * t.heads, Tp, Tp);
         bgemm(scores(bw.PT, t), heads_cols(bw.daoT, C, t), 64, bw.dqkv + 2 * C, 3 * C, 64, (long long)Tp * 3 * C, t.heads, n, t);
-        {
-            const __half* P = a.S; __half* dS = bw.dS; const size_t rows = (size_t)n * t.heads * Tp;
-            push([=](cudaStream_t st) {
-                sdk::k_softmax_bwd<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(P, dS, rows, Tp, 0.125f);
-                return (int)cudaGetLastError();
-            });
-        }
+        softmax_bwd(a.S, bw.dS, (size_t)n * t.heads * Tp, Tp, 0.125f);
         bgemm(scores(bw.dS, t), heads_cols(a.qkvT + (long long)C * Tp, 3 * C, t), 64, bw.dqkv, 3 * C, 64, (long long)Tp * 3 * C, t.heads, n, t);
         transpose(bw.dS, bw.dST, n * t.heads, Tp, Tp);
         bgemm(scores(bw.dST, t), heads_cols(a.qkvT, 3 * C, t), 64, bw.dqkv + C, 3 * C, 64, (long long)Tp * 3 * C, t.heads, n, t);
@@ -206,13 +194,9 @@ struct Engine : TowerBuilder {
         txt_fwd.assign(Bm, {});
         for (int B = 1; B <= Bm; B++) {
             cur = &txt_fwd[B - 1];
-            const long long* tk = tokens; __half* xx = tx0; const int Tp = t.Tpad, T = t.T, V = c.vocab;
-            push([=](cudaStream_t st) {
-                clipk::k_text_embed<<<blocks_for((size_t)B * Tp * C / 8), 256, 0, st>>>(tk, tok, pos, xx, B, T, Tp, C, V);
-                return (int)cudaGetLastError();
-            });
+            text_embed(tokens, tok, pos, tx0, B, t.T, t.Tpad, C, c.vocab);
             for (int i = 0; i < t.L; i++) block_fwd(t, tw[i], ta[i], B, 2, tc::EPI_QUICKGELU);
-            __half* rows = eot;
+            const long long* tk = tokens; __half* rows = eot; const int Tp = t.Tpad, T = t.T;
             push([=](cudaStream_t st) {
                 clipk::k_text_eot_rows<<<B, 128, 0, st>>>(tk, r_last, rows, T, Tp, C);
                 return (int)cudaGetLastError();

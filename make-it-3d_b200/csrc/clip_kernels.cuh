@@ -1,16 +1,16 @@
-// clip_kernels.cuh -- the memory-bound kernels of the CLIP engine (clip_engine.cu) that the SD kernels do not already provide:
-// image preprocessing (resize / normalise / patchify) and its input gradient, token / class / positional embeddings, the EOT-row
-// select, LayerNorm backward and the causal softmax of the text tower.  Activations are token rows of fp16 ("tokens x C"),
+// clip_kernels.cuh -- the memory-bound kernels of the CLIP engine (clip_engine.cu) that the op layer (plan.cu) does not provide:
+// image preprocessing (resize / normalise / patchify) and its input gradient, the feature-gradient scaling, the class / positional
+// embedding of the image tower and the EOT-row select of the text tower.  Activations are token rows of fp16 ("tokens x C"),
 // reductions are fp32, and every output element is written by exactly one thread (no atomics: run-to-run deterministic).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "sd_kernels.cuh"
+#include "warp_reduce.cuh"
 
 namespace clipk {
-namespace {   // internal linkage: the CLIP engine and the SD-2 text encoder both include these kernels
+namespace {
 
 // openai CLIP's Normalize constants
 __device__ __forceinline__ float norm_mean(int c) { return c == 0 ? 0.48145466f : (c == 1 ? 0.4578275f : 0.40821073f); }
@@ -97,12 +97,12 @@ __global__ void k_grad_in(const float* __restrict__ g, int n, __half* __restrict
     __shared__ float s_max[32];
     float m = 0.f;
     for (int i = threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, fabsf(g[i]));
-    m = sdk::warp_max(m);
+    m = warp_max(m);
     if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = m;
     __syncthreads();
     if (threadIdx.x < 32) {
         m = threadIdx.x < (blockDim.x >> 5) ? s_max[threadIdx.x] : 0.f;
-        m = sdk::warp_max(m);
+        m = warp_max(m);
         if (threadIdx.x == 0) {
             int e = 0;
             if (m > 0.f && isfinite(m)) frexpf(m, &e);
@@ -135,28 +135,6 @@ __global__ void k_image_embed(const __half* __restrict__ patch, const float* __r
     }
 }
 
-// x[b*Tpad + t] = tok_emb[tokens[b, t]] + pos[t] for t < L; rows L .. Tpad-1 are zero.  Token ids outside [0, vocab) are clamped
-// into it (never read out of bounds).
-__global__ void k_text_embed(const long long* __restrict__ tokens, const float* __restrict__ tok_emb, const float* __restrict__ pos,
-                             __half* __restrict__ x, int B, int L, int Tpad, int C, int vocab) {
-    const int vc = C / 8;
-    const size_t total = (size_t)B * Tpad * vc;
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int v = (int)(i % vc); const size_t r = i / vc;
-        const int t = (int)(r % Tpad), b = (int)(r / Tpad);
-        __align__(16) __half o[8];
-        if (t < L) {
-            const long long id = min(max(tokens[(size_t)b * L + t], 0ll), (long long)vocab - 1);
-            #pragma unroll
-            for (int k = 0; k < 8; k++) o[k] = __float2half_rn(tok_emb[(size_t)id * C + v * 8 + k] + pos[(size_t)t * C + v * 8 + k]);
-        } else {
-            #pragma unroll
-            for (int k = 0; k < 8; k++) o[k] = __float2half_rn(0.f);
-        }
-        *reinterpret_cast<uint4*>(x + i * 8) = *reinterpret_cast<const uint4*>(o);
-    }
-}
-
 // out[b] = x[b*Tpad + argmax_t tokens[b, t]] (the first maximum, like torch.argmax): the EOT token's row.  One block per b.
 __global__ void k_text_eot_rows(const long long* __restrict__ tokens, const __half* __restrict__ x, __half* __restrict__ out, int L, int Tpad, int C) {
     const int b = blockIdx.x;
@@ -169,77 +147,6 @@ __global__ void k_text_eot_rows(const long long* __restrict__ tokens, const __ha
     __syncthreads();
     const __half* src = x + ((size_t)b * Tpad + s_arg) * C;
     for (int c = threadIdx.x; c < C; c += blockDim.x) out[(size_t)b * C + c] = src[c];
-}
-
-// LayerNorm input gradient, one warp per row (statistics recomputed from x exactly as k_layernorm computes them):
-// dx = rstd * (g - mean(g) - xhat * mean(g * xhat)) (+ add),  g = dy * gamma.
-__global__ void k_layernorm_bwd(const __half* __restrict__ x, const __half* __restrict__ dy, const float* __restrict__ gamma,
-                                const __half* __restrict__ add, __half* __restrict__ dx, int rows, int C, float eps) {
-    const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (row >= rows) return;
-    const __half* xr = x + (size_t)row * C; const __half* dr = dy + (size_t)row * C;
-    float mean, rstd;
-    sdk::row_stats(xr, C, eps, lane, mean, rstd);
-    float g1 = 0.f, g2 = 0.f;
-    for (int c = lane * 8; c < C; c += 256) {
-        const uint4 rx = *reinterpret_cast<const uint4*>(xr + c), rd = *reinterpret_cast<const uint4*>(dr + c);
-        const __half* hx = reinterpret_cast<const __half*>(&rx); const __half* hd = reinterpret_cast<const __half*>(&rd);
-        #pragma unroll
-        for (int k = 0; k < 8; k++) {
-            const float g = __half2float(hd[k]) * gamma[c + k];
-            g1 += g; g2 += g * (__half2float(hx[k]) - mean) * rstd;
-        }
-    }
-    g1 = sdk::warp_sum(g1) / C; g2 = sdk::warp_sum(g2) / C;
-    for (int c = lane * 8; c < C; c += 256) {
-        const uint4 rx = *reinterpret_cast<const uint4*>(xr + c), rd = *reinterpret_cast<const uint4*>(dr + c);
-        const __half* hx = reinterpret_cast<const __half*>(&rx); const __half* hd = reinterpret_cast<const __half*>(&rd);
-        uint4 ra = make_uint4(0, 0, 0, 0);
-        if (add) ra = *reinterpret_cast<const uint4*>(add + (size_t)row * C + c);
-        const __half* ha = reinterpret_cast<const __half*>(&ra);
-        __align__(16) __half o[8];
-        #pragma unroll
-        for (int k = 0; k < 8; k++) {
-            const float xh = (__half2float(hx[k]) - mean) * rstd;
-            o[k] = __float2half_rn(rstd * (__half2float(hd[k]) * gamma[c + k] - g1 - xh * g2) + __half2float(ha[k]));
-        }
-        *reinterpret_cast<uint4*>(dx + (size_t)row * C + c) = *reinterpret_cast<const uint4*>(o);
-    }
-}
-
-// Causal row softmax in place over [Z][tq][cols] scores: row r (query q = r % tq) keeps keys j <= q (and j < valid); the other
-// columns are written as 0.  One warp per row.
-__global__ void k_softmax_causal(__half* __restrict__ s, size_t rows, int cols, int valid, int tq, float scale) {
-    const size_t row = blockIdx.x * (size_t)(blockDim.x >> 5) + (threadIdx.x >> 5);
-    const int lane = threadIdx.x & 31;
-    if (row >= rows) return;
-    const int lim = min(valid, (int)(row % tq) + 1);
-    __half* r = s + row * cols;
-    float mx = -INFINITY;
-    for (int c = lane * 8; c < cols; c += 256) {
-        const uint4 raw = *reinterpret_cast<const uint4*>(r + c);
-        const __half* h = reinterpret_cast<const __half*>(&raw);
-        #pragma unroll
-        for (int k = 0; k < 8; k++) if (c + k < lim) mx = fmaxf(mx, __half2float(h[k]) * scale);
-    }
-    mx = sdk::warp_max(mx);
-    float sum = 0.f;
-    for (int c = lane * 8; c < cols; c += 256) {
-        const uint4 raw = *reinterpret_cast<const uint4*>(r + c);
-        const __half* h = reinterpret_cast<const __half*>(&raw);
-        #pragma unroll
-        for (int k = 0; k < 8; k++) if (c + k < lim) sum += __expf(__half2float(h[k]) * scale - mx);
-    }
-    sum = sdk::warp_sum(sum);
-    const float inv = 1.f / sum;
-    for (int c = lane * 8; c < cols; c += 256) {
-        const uint4 raw = *reinterpret_cast<const uint4*>(r + c);
-        const __half* h = reinterpret_cast<const __half*>(&raw);
-        __align__(16) __half o[8];
-        #pragma unroll
-        for (int k = 0; k < 8; k++) o[k] = __float2half_rn(c + k < lim ? __expf(__half2float(h[k]) * scale - mx) * inv : 0.f);
-        *reinterpret_cast<uint4*>(r + c) = *reinterpret_cast<const uint4*>(o);
-    }
 }
 
 }  // namespace

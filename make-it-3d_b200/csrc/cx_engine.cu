@@ -66,11 +66,9 @@ struct Engine : Builder {
                 if (idx == 0) {
                     const float* w = (const float*)param(L.w + ".weight", {cout, cin, 3, 3}, PK_CX_CONV_IN).dst;
                     param(L.w + ".weight#dgrad", {4, cout, 3, 3}, PK_CX_CONV_IN_DGRAD);
-                    const T4 a = L.in, o = L.out;
-                    const size_t sm = (size_t)cout * 9 * 4 * sizeof(float);
-                    const int grid = small_cin_grid(o.numel(), sm);
+                    const T4 o = L.out;
+                    conv_small_cin(L.in, w, bias, o);
                     push([=](cudaStream_t st) {
-                        sdk::k_conv_small_cin<4><<<grid, 256, sm, st>>>(a.p, w, bias, o.p, a.n, a.h, a.w, o.c);
                         cxk::k_relu<<<blocks_for(o.numel() / 8), 256, 0, st>>>(o.p, o.numel() / 8);
                         return (int)cudaGetLastError();
                     });
@@ -148,12 +146,7 @@ struct Engine : Builder {
             } else {
                 g4 = alloc32((size_t)N * cfg.H * cfg.W * 4);
                 const __half* w = (const __half*)params[pindex[L.w + ".weight#dgrad"]].dst;
-                const T4 d = dy; float* o = g4;
-                const int grid = small_cout_grid((size_t)d.rows(), d.c);
-                push([=](cudaStream_t st) {
-                    sdk::k_conv_small_cout<4><<<grid, 256, (size_t)4 * 9 * d.c * 2, st>>>(d.p, w, nullptr, o, d.n, d.h, d.w, d.c);
-                    return (int)cudaGetLastError();
-                });
+                conv_small_cout(dy, w, nullptr, g4, 4);
             }
         }
         cur = nullptr;

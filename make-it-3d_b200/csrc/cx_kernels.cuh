@@ -10,7 +10,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "sd_kernels.cuh"
+#include "warp_reduce.cuh"
 
 namespace cxk {
 
@@ -100,8 +100,8 @@ __global__ void k_maxpool2_bwd(const __half* __restrict__ dout, const __half* __
     }
 }
 
-// conv1_1 OIHW fp32 [64][3][3][3] -> fp32 [64][3][3][4] (input channels padded to 4) for sdk::k_conv_small_cin<4>, and the
-// flipped fp16 copy [4][2-ky][2-kx][64] for its input gradient through sdk::k_conv_small_cout<4>
+// conv1_1 OIHW fp32 [64][3][3][3] -> fp32 [64][3][3][4] (input channels padded to 4) for Builder::conv_small_cin, and the
+// flipped fp16 copy [4][2-ky][2-kx][64] for its input gradient through Builder::conv_small_cout
 __global__ void k_conv1_w(const float* __restrict__ src, float* __restrict__ fwd, __half* __restrict__ dgrad, int O) {
     const int n = O * 4 * 9;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -135,7 +135,7 @@ __global__ void k_normalize(const __half* __restrict__ F, const float* __restric
     const __half* f = F + (size_t)row * C;
     float ss = 0.f;
     for (int c = lane; c < C; c += 32) { const float v = __half2float(f[c]) - ymu[c]; ss += v * v; }
-    ss = sdk::warp_sum(ss);
+    ss = warp_sum(ss);
     const float nr = sqrtf(ss), den = fmaxf(nr, 1e-12f);
     for (int c = lane; c < C; c += 32) xh[(size_t)row * C + c] = (__half2float(f[c]) - ymu[c]) / den;
     if (lane == 0) nrm[row] = nr;
@@ -185,7 +185,7 @@ __global__ void __launch_bounds__(256) k_sgemm(const float* __restrict__ A, long
 
 // block-wide (256 threads) fixed-order reductions
 __device__ __forceinline__ float block_sum(float v, float* sh) {
-    v = sdk::warp_sum(v);
+    v = warp_sum(v);
     __syncthreads();
     if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
     __syncthreads();
@@ -289,7 +289,7 @@ __global__ void k_normalize_bwd(float* __restrict__ dxh, const float* __restrict
     float* d = dxh + (size_t)row * C; const float* x = xh + (size_t)row * C; const __half* f = F + (size_t)row * C;
     float dot = 0.f;
     for (int c = lane; c < C; c += 32) dot += x[c] * d[c];
-    dot = sdk::warp_sum(dot);
+    dot = warp_sum(dot);
     const float nr = nrm[row];
     float mx = 0.f;
     for (int c = lane; c < C; c += 32) {
@@ -297,7 +297,7 @@ __global__ void k_normalize_bwd(float* __restrict__ dxh, const float* __restrict
         const float v = __half2float(f[c]) > 0.f ? g : 0.f;
         d[c] = v; mx = fmaxf(mx, fabsf(v));
     }
-    mx = sdk::warp_max(mx);
+    mx = warp_max(mx);
     if (lane == 0) rowmax[row] = mx;
 }
 
@@ -307,7 +307,7 @@ __global__ void k_grad_scale(const float* __restrict__ rowmax, int rows, float* 
     __shared__ float sh[8];
     float m = 0.f;
     for (int r = threadIdx.x; r < rows; r += blockDim.x) m = fmaxf(m, rowmax[r]);
-    m = sdk::warp_max(m);
+    m = warp_max(m);
     if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = m;
     __syncthreads();
     if (threadIdx.x == 0) {

@@ -3,26 +3,27 @@
 // What the reference's `DPTDepthModel(backbone="vitb_rn50_384", non_negative=True)` computes (main.py:111-127, 196-214) for one
 // normalised 384 x 384 image: a ResNet-50v2 trunk with weight-standardised convs and GroupNorm, a 12-layer ViT-B/16 on its 24 x 24
 // features (577 tokens), the reassemble stage, four RefineNet fusion blocks and the depth head (oracle/dpt_ref.py restates it).  One
-// statically planned list of launches: the tile GEMM for every 1x1 conv and linear (a stride-2 3x3 conv goes through sdk::k_im2col_s2),
+// statically planned list of launches: the tile GEMM for every 1x1 conv and linear (a stride-2 3x3 conv goes through Builder::conv3_s2),
 // its spatial-block mode for the stride-1 3x3 convs, the pre-LN blocks of transformer_plan.cuh with fused attention and the EPI_GELU
 // epilogue, and the memory-bound kernels below.  Activations NHWC fp16, statistics and accumulation fp32, GEMM weights fp16 (norms,
 // biases, cls / pos_embed and the final 32 -> 1 conv fp32).  Forward only, at the reference's one shape.  No split-K and no atomics:
 // the output is bit-identical run to run.
 #include "transformer_plan.cuh"
+#include "warp_reduce.cuh"
 
 namespace dptk {
 namespace {
 
 __device__ __forceinline__ float block_sum(float v, float* red) {       // fixed-order reduction over the block (blockDim.x <= 1024)
     const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    v = sdk::warp_sum(v);
+    v = warp_sum(v);
     __syncthreads();
     if (lane == 0) red[w] = v;
     __syncthreads();
     float s = 0.f;
     if (w == 0) {
         s = lane < (int)(blockDim.x >> 5) ? red[lane] : 0.f;
-        s = sdk::warp_sum(s);
+        s = warp_sum(s);
         if (lane == 0) red[32] = s;
     }
     __syncthreads();
@@ -149,7 +150,7 @@ __global__ void k_cls_bias(const __half* __restrict__ W, const float* __restrict
     const __half* wr = W + (size_t)n * 2 * C + C;
     float s = 0.f;
     for (int k = lane; k < C; k += 32) s = fmaf(__half2float(wr[k]), __half2float(cls[k]), s);
-    s = sdk::warp_sum(s);
+    s = warp_sum(s);
     if (lane == 0) bb[n] = b[n] + s;
 }
 
@@ -252,13 +253,6 @@ struct Engine : TowerBuilder {
         launch([=](cudaStream_t st) { dptk::k_gn<<<32, 1024, 0, st>>>(xp, yp, ga, be, res, HW, C, 1e-5f, relu ? 1 : 0); });
     }
     void conv1x1(const T4& x, const __half* wt, const T4& y, const float* bias = nullptr) { linear(x.p, x.rows(), x.c, wt, y.c, y.p, bias); }
-    // 3x3 stride-2 conv: im2col (pad_lo 0: TF-"same" on an even input, 1: symmetric padding 1) + GEMM
-    void conv3_s2(const T4& x, const __half* wt, const T4& y, const float* bias, int pad_lo) {
-        __half* col = alloc16((size_t)y.h * y.w * 9 * x.c);
-        const __half* xp = x.p; const int H = x.h, W = x.w, C = x.c, Ho = y.h, Wo = y.w;
-        launch([=](cudaStream_t st) { sdk::k_im2col_s2<<<grid((size_t)Ho * Wo * 9 * C / 8), 256, 0, st>>>(xp, col, 1, H, W, C, Ho, Wo, pad_lo); });
-        linear(col, (long long)Ho * Wo, 9 * C, wt, y.c, y.p, bias);
-    }
 
     T4 bottleneck(const T4& x, const std::string& p, int mid, int cout, int stride, bool first) {
         const int Ho = x.h / stride, Wo = x.w / stride;

@@ -11,6 +11,7 @@
 // Activations: NHWC fp16.  Accumulation / statistics: fp32 (fp64 group sums).  Weights: fp16 copies of the fp32
 // diffusers parameters, re-laid-out at load time (conv OIHW -> O,ky,kx,I ; GEGLU rows interleaved ; dgrad copies).
 #include "engine_plan.cuh"
+#include "sd_kernels.cuh"
 
 namespace sd {
 
@@ -247,17 +248,10 @@ struct Engine : Builder {
     }
 
     T4 downsample(const std::string& pre, const T4& x, int pad_lo, bool both, __half** col_out = nullptr) {
-        const int Ho = x.h / 2, Wo = x.w / 2, C = x.c;
-        const long long Mo = (long long)x.n * Ho * Wo;
-        __half* col = alloc16((size_t)Mo * 9 * C);
-        const T4 xx = x;
-        push([=](cudaStream_t st) {
-            sdk::k_im2col_s2<<<blocks_for((size_t)Mo * 9 * C / 8), 256, 0, st>>>(xx.p, col, xx.n, xx.h, xx.w, C, Ho, Wo, pad_lo);
-            return (int)cudaGetLastError();
-        });
+        const int C = x.c;
         Param& w = param(pre + ".conv.weight", {C, C, 3, 3}, both ? PK_CONV3_S2_BOTH : PK_CONV3);
-        T4 y = act(x.n, Ho, Wo, C);
-        linear(col, Mo, 9 * C, (const __half*)w.dst, C, y.p, pf(pre + ".conv.bias", {C}));
+        T4 y = act(x.n, x.h / 2, x.w / 2, C);
+        __half* col = conv3_s2(x, (const __half*)w.dst, y, pf(pre + ".conv.bias", {C}), pad_lo);
         if (col_out) *col_out = col;
         return y;
     }
@@ -306,13 +300,8 @@ struct Engine : Builder {
         {
             const float* w = (const float*)param("conv_in.weight", {c0, c.in_ch, 3, 3}, PK_CONV_F32_OHWI).dst;
             const float* b = pf("conv_in.bias", {c0});
-            const T4 xin = unet_in, ho = h; const int cin = c.in_ch;
-            push([=](cudaStream_t st) {
-                if (cin != 4 || c0 % 8) return (int)MI3D_ERR_ARG;
-                const size_t sm = (size_t)c0 * 9 * 4 * sizeof(float);
-                sdk::k_conv_small_cin<4><<<small_cin_grid(ho.numel(), sm), 256, sm, st>>>(xin.p, w, b, ho.p, xin.n, xin.h, xin.w, c0);
-                return (int)cudaGetLastError();
-            });
+            if (c.in_ch != 4) err = MI3D_ERR_ARG;
+            conv_small_cin(unet_in, w, b, h);
         }
         tap("unet.conv_in", h.p, h.numel() * 2);
         std::vector<T4> skips; skips.push_back(h);
@@ -363,13 +352,8 @@ struct Engine : Builder {
         {
             const __half* w = (const __half*)param("conv_out.weight", {c.out_ch, c0, 3, 3}, PK_CONV_SMALL_COUT).dst;
             const float* b = pf("conv_out.bias", {c.out_ch});
-            float* o = unet_out; const int oc = c.out_ch;
-            push([=](cudaStream_t st) {
-                if (oc != 4) return (int)MI3D_ERR_ARG;
-                const size_t pix = (size_t)a.rows();
-                sdk::k_conv_small_cout<4><<<small_cout_grid(pix, a.c), 256, (size_t)4 * 9 * a.c * 2, st>>>(a.p, w, b, o, a.n, a.h, a.w, a.c);
-                return (int)cudaGetLastError();
-            });
+            if (c.out_ch != 4) err = MI3D_ERR_ARG;
+            conv_small_cout(a, w, b, unet_out, 4);
         }
         if (temb_jobs.size() > 64) err = MI3D_ERR_ARG;
         if (!dry && !err && !temb_jobs.empty())
@@ -422,13 +406,7 @@ struct Engine : Builder {
         {
             const float* w = (const float*)param("encoder.conv_in.weight", {c.block_out[0], c.in_ch, 3, 3}, PK_CONV_F32_OHWI).dst;
             const float* b = pf("encoder.conv_in.bias", {c.block_out[0]});
-            const T4 xin = vae_in, ho = h; const int co = c.block_out[0];
-            push([=](cudaStream_t st) {
-                if (co % 8) return (int)MI3D_ERR_ARG;
-                const size_t sm = (size_t)co * 9 * 4 * sizeof(float);
-                sdk::k_conv_small_cin<4><<<small_cin_grid(ho.numel(), sm), 256, sm, st>>>(xin.p, w, b, ho.p, 1, xin.h, xin.w, co);
-                return (int)cudaGetLastError();
-            });
+            conv_small_cin(vae_in, w, b, h);
         }
         v_conv_in_out = h;
         int ch = c.block_out[0];
@@ -482,12 +460,8 @@ struct Engine : Builder {
         {
             const __half* w = (const __half*)param("encoder.conv_out.weight", {l2, ch, 3, 3}, PK_CONV_SMALL_COUT_BOTH).dst;
             const float* b = pf("encoder.conv_out.bias", {l2});
-            const T4 a = v_a_out;
-            push([=](cudaStream_t st) {
-                if (l2 != 8) return (int)MI3D_ERR_ARG;
-                sdk::k_conv_small_cout<8><<<small_cout_grid((size_t)a.rows(), a.c), 256, (size_t)8 * 9 * a.c * 2, st>>>(a.p, w, b, co, a.n, a.h, a.w, a.c);
-                return (int)cudaGetLastError();
-            });
+            if (l2 != 8) err = MI3D_ERR_ARG;
+            conv_small_cout(v_a_out, w, b, co, 8);
         }
         vae_moments = co;
         pf("quant_conv.weight", {l2, l2, 1, 1}); pf("quant_conv.bias", {l2});
@@ -528,14 +502,8 @@ struct Engine : Builder {
         {
             const float* w = (const float*)param("decoder.conv_in.weight", {ch, c.latent_ch, 3, 3}, PK_CONV_F32_OHWI).dst;
             const float* b = pf("decoder.conv_in.bias", {ch});
-            const T4 xin = dec_in, ho = h; const int co = ch, lc = c.latent_ch;
-            push([=](cudaStream_t st) {
-                if (lc != 4 || co % 8) return (int)MI3D_ERR_ARG;
-                const size_t sm = (size_t)co * 9 * 4 * sizeof(float);
-                if (sm > 100 * 1024) return (int)MI3D_ERR_ARG;
-                sdk::k_conv_small_cin<4><<<small_cin_grid(ho.numel(), sm), 256, sm, st>>>(xin.p, w, b, ho.p, 1, xin.h, xin.w, co);
-                return (int)cudaGetLastError();
-            });
+            if (c.latent_ch != 4) err = MI3D_ERR_ARG;
+            conv_small_cin(dec_in, w, b, h);
         }
         h = dec_resnet("decoder.mid_block.resnets.0", h, ch);
         {   // single-head attention over all pixels (same construction as the encoder's, no tape)
@@ -584,12 +552,8 @@ struct Engine : Builder {
             alloc16((size_t)9 * ch);
             const float* b = pf("decoder.conv_out.bias", {c.in_ch});
             alloc32(4);
-            float* o = dec_out; const int ic = c.in_ch;
-            push([=](cudaStream_t st) {
-                if (ic != 3) return (int)MI3D_ERR_ARG;
-                sdk::k_conv_small_cout<4><<<small_cout_grid((size_t)a.rows(), a.c), 256, (size_t)4 * 9 * a.c * 2, st>>>(a.p, w, b, o, a.n, a.h, a.w, a.c);
-                return (int)cudaGetLastError();
-            });
+            if (c.in_ch != 3) err = MI3D_ERR_ARG;
+            conv_small_cout(a, w, b, dec_out, 4);
         }
         cur = nullptr;
     }
@@ -604,16 +568,9 @@ struct Engine : Builder {
         T4 g8 = act(hl.n, hl.h, hl.w, 8);
         T4 da = act(hl.n, hl.h, hl.w, ch);
         {
-            float* gm = vae_gmoments; const T4 g8c = g8, dac = da;
             const float* wf = (const float*)param("encoder.conv_out.weight#dgrad_f32", {ch, 8, 3, 3}, PK_CONV_F32_OHWI).dst;
-            push([=](cudaStream_t st) {
-                // fp32 -> fp16 staging of the 8-channel gradient
-                sdk::k_f32_to_f16<<<blocks_for(g8c.numel()), 256, 0, st>>>(gm, g8c.p, g8c.numel());
-                if (ch % 8) return (int)MI3D_ERR_ARG;
-                const size_t sm = (size_t)ch * 9 * 8 * sizeof(float);
-                sdk::k_conv_small_cin<8><<<small_cin_grid(dac.numel(), sm), 256, sm, st>>>(g8c.p, wf, nullptr, dac.p, g8c.n, g8c.h, g8c.w, ch);
-                return (int)cudaGetLastError();
-            });
+            f32_to_f16(vae_gmoments, g8.p, g8.numel());          // fp32 -> fp16 staging of the 8-channel gradient
+            conv_small_cin(g8, wf, nullptr, da);
         }
         T4 dh = act(hl.n, hl.h, hl.w, ch);
         groupnorm_bwd(vgn_out, da.p, nullptr, dh.p);
@@ -645,7 +602,7 @@ struct Engine : Builder {
                 const DownTape& d = vdown[di--];
                 const int C = d.x.c; const long long Mo = d.y.rows();
                 Param& w = params[pindex[d.pre + ".conv.weight"]];
-                // dcol[Mo, 9C] = dy[Mo, C] . Wt   with Wt = [9C][C]  (dst2 of a PK_CONV3_S2_BOTH weight = plain transpose, see load_param)
+                // dcol[Mo, 9C] = dy[Mo, C] . Wt   with Wt = [9C][C]  (dst2 of a PK_CONV3_S2_BOTH weight = plain transpose, see Builder::load_param)
                 __half* dcol = alloc16((size_t)Mo * 9 * C);
                 linear(dh.p, Mo, C, (const __half*)w.dst2, 9 * C, dcol);
                 T4 dx = act(d.x.n, d.x.h, d.x.w, C);
@@ -669,7 +626,7 @@ struct Engine : Builder {
                 __half* dP = alloc16((size_t)M * M);
                 { Mat A{dao, C, M, C}; Mat Bm{a.v, C, M, C}; Out oo; oo.p16 = dP; oo.ldc = M; Epi e; gemm(A, Bm, (int)M, oo, e); }
                 const float scale = 1.0f / sqrtf((float)C);
-                { const __half* Pp = a.P; push([=](cudaStream_t st) { sdk::k_softmax_bwd<<<(unsigned)((M + 7) / 8), 256, 0, st>>>(Pp, dP, (size_t)M, (int)M, scale); return (int)cudaGetLastError(); }); }
+                softmax_bwd(a.P, dP, (size_t)M, (int)M, scale);
                 // dQ = dS K ; dK = dS^T Q
                 __half* kT = alloc16(M * C); transpose(a.k, kT, 1, (int)M, C);
                 __half* qT = alloc16(M * C); transpose(a.q, qT, 1, (int)M, C);
@@ -693,11 +650,7 @@ struct Engine : Builder {
         named["vae.grad_in"] = {gimg, (size_t)vae_in.rows() * 4 * sizeof(float)};
         {
             const __half* w = (const __half*)param("encoder.conv_in.weight#dgrad", {4, c.block_out[0], 3, 3}, PK_CONV_SMALL_COUT).dst;
-            const T4 d = dh;
-            push([=](cudaStream_t st) {
-                sdk::k_conv_small_cout<4><<<small_cout_grid((size_t)d.rows(), d.c), 256, (size_t)4 * 9 * d.c * 2, st>>>(d.p, w, nullptr, gimg, d.n, d.h, d.w, d.c);
-                return (int)cudaGetLastError();
-            });
+            conv_small_cout(dh, w, nullptr, gimg, 4);
         }
         vae_grad_img = gimg;
         cur = nullptr;
@@ -739,12 +692,6 @@ struct Engine : Builder {
         const int nb = blocks_for(P.numel);
         using namespace sdk;
         switch (P.kind) {
-            case PK_CONV3_S2_BOTH:
-                // dgrad of the im2col GEMM needs the plain transpose of the [Cout][9*Cin] matrix: [9*Cin][Cout]
-                // (k_conv_w wrote [O][ky][kx][I]; transpose that fp16 matrix)
-                k_conv_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.shape[0], P.shape[1], 0);
-                k_transpose<<<dim3((9 * P.shape[1] + 31) / 32, (P.shape[0] + 31) / 32, 1), dim3(32, 8), 0, st>>>((const __half*)P.dst, (__half*)P.dst2, P.shape[0], 9 * P.shape[1]);
-                break;
             case PK_GEGLU_W: {
                 if (!partner) return MI3D_ERR_ARG;
                 const Param& Bp = params[pindex[P.partner]];
@@ -776,7 +723,7 @@ struct Engine : Builder {
             }
             case PK_CONV_SMALL_COUT: case PK_CONV_SMALL_COUT_BOTH: {
                 const bool dg = P.name.find("#dgrad") != std::string::npos;
-                if (!dg) k_conv_w<<<nb, 256, 0, st>>>(src, (__half*)P.dst, P.shape[0], P.shape[1], 0);
+                if (!dg) return Builder::load_param(P, src, partner, st);
                 else {
                     // conv_in transposed: src conv_in OIHW [c0][3][3][3]; want [4 (padded cin)][2-ky][2-kx][c0] fp16
                     const int c0 = P.shape[1];
@@ -956,13 +903,7 @@ extern "C" {
 size_t mi3d_sd_workspace_bytes(const mi3d_unet_cfg* u, const mi3d_vae_cfg* v) { return plan::workspace_bytes<sd::Engine>(u, v); }
 
 mi3d_engine_t mi3d_sd_create(const mi3d_unet_cfg* u, const mi3d_vae_cfg* v, void* workspace, size_t workspace_bytes) {
-    sd::Engine* e = plan::create<sd::Engine>(workspace, workspace_bytes, u, v);
-    if (!e) return nullptr;
-    cudaFuncSetAttribute(sdk::k_conv_small_cin<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(sdk::k_conv_small_cin<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-    cudaFuncSetAttribute(sdk::k_conv_small_cout<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-    cudaFuncSetAttribute(sdk::k_conv_small_cout<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-    return e;
+    return plan::create<sd::Engine>(workspace, workspace_bytes, u, v);
 }
 
 int mi3d_sd_profile(mi3d_engine_t h, int enable, float* gemm_ms, int* launches) { return mi3d_sd_profile_dump(h, enable, gemm_ms, launches, nullptr); }

@@ -4,11 +4,12 @@
 // (width 1024, 16 heads of 64, MLP 4096 with exact GELU, causal attention, no padding mask), then final_layer_norm over every one of
 // the 77 positions (last_hidden_state; no EOT pooling, no projection).  SD-1.x ships OpenAI CLIP ViT-L/14's text tower instead (12
 // layers, width 768, 12 heads of 64, quick-GELU; act = 1), otherwise the same computation.  A statically planned list of
-// launches: the token embedding (clipk::k_text_embed), the pre-LN blocks of transformer_plan.cuh with the tile GEMM's EPI_GELU or
+// launches: the token embedding (Builder::text_embed), the pre-LN blocks of transformer_plan.cuh with the tile GEMM's EPI_GELU or
 // EPI_QUICKGELU epilogue, and a final LayerNorm that writes fp32.  Activations fp16, statistics and accumulation fp32, weights fp16 (the embeddings and LayerNorms fp32).  Forward only
 // (the encoder is frozen), so all blocks share one set of activation buffers.  No split-K and no atomics: results are bit-identical
 // run to run, under graph replay, and for a sequence whether it is encoded alone or in a batch.
 #include "transformer_plan.cuh"
+#include "warp_reduce.cuh"
 
 namespace sdtext {
 
@@ -21,7 +22,7 @@ __global__ void k_layernorm_rows_f32(const __half* __restrict__ x, const float* 
     if (row >= B * T) return;
     const __half* xr = x + ((size_t)(row / T) * Tpad + row % T) * C;
     float mean, rstd;
-    sdk::row_stats(xr, C, eps, lane, mean, rstd);
+    row_stats(xr, C, eps, lane, mean, rstd);
     float* yr = out + (size_t)row * C;
     for (int c = lane * 8; c < C; c += 256) {
         const uint4 raw = *reinterpret_cast<const uint4*>(xr + c);
@@ -94,11 +95,8 @@ struct Engine : TowerBuilder {
         fwd.assign(Bm, {});
         for (int B = 1; B <= Bm; B++) {
             cur = &fwd[B - 1];
-            const long long* tk = tokens; __half* x0 = r[0]; float* o = out; const int Tp = t.Tpad, T = t.T, V = c.vocab;
-            push([=](cudaStream_t st) {
-                clipk::k_text_embed<<<blocks_for((size_t)B * Tp * C / 8), 256, 0, st>>>(tk, tok, pos, x0, B, T, Tp, C, V);
-                return (int)cudaGetLastError();
-            });
+            text_embed(tokens, tok, pos, r[0], B, t.T, t.Tpad, C, c.vocab);
+            float* o = out; const int Tp = t.Tpad, T = t.T;
             for (int i = 0; i < t.L; i++) block_fwd(t, w[i], a[i], B, 2, act ? tc::EPI_QUICKGELU : tc::EPI_GELU);
             push([=](cudaStream_t st) {
                 k_layernorm_rows_f32<<<(unsigned)((B * T + 7) / 8), 256, 0, st>>>(r_last, lnf, lnf_b, o, B, T, Tp, C, 1e-5f);

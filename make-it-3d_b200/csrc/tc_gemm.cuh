@@ -23,99 +23,14 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "tc_host.cuh"
+#include "tma.cuh"
 #include "wgmma.cuh"
 
 namespace tc {
 
-constexpr int BLOCK_M = 128;
-constexpr int BLOCK_K = 64;          // 64 fp16 = 128 B = one swizzle-128B atom row
 constexpr int MMA_K = 16;
 constexpr int kThreads = 384;
-
-// EPI_QUICKGELU: out = y * sigmoid(1.702 y) (CLIP's MLP activation), y = alpha * acc + bias; the pre-activation y is also stored to aux
-//                when aux is set (the input-gradient pass needs it).
-// EPI_QUICKGELU_BWD: out = y * QuickGELU'(aux), aux = the saved pre-activation (same layout as out).
-// EPI_RELU: out = max(y, 0) (VGG's convs).  EPI_RELU_BWD: out = y * (aux > 0), aux = the saved post-ReLU input of the conv whose
-//                input gradient this is (same layout as out).  Both only in k_tc_gemm_vgg.
-// EPI_GELU: out = 0.5 y (1 + erf(y / sqrt 2)) (exact GELU, the SD-2 text encoder's MLP activation), y = alpha * acc + bias, in fp32,
-//                stored fp16.  Forward only; only in k_tc_gemm_gelu.
-enum EpiMode : int { EPI_PLAIN = 0, EPI_GEGLU = 1, EPI_TRANSPOSED = 2, EPI_QUICKGELU = 3, EPI_QUICKGELU_BWD = 4, EPI_RELU = 5, EPI_RELU_BWD = 6,
-                     EPI_GELU = 7 };
-
-struct GemmParams {
-    int M, N, K;                 // per-batch extents; N multiple of BLOCK_N, K multiple of 64, M multiple of 128 (rows may be padded)
-    int num_k_blocks;
-    int conv;                    // 0 plain, 1 implicit 3x3 conv, 2 implicit 3x3 conv over spatial blocks (k_tc_gemm_vgg)
-    int conv_H, conv_W, conv_bw, conv_bh, cin_blocks;
-    int a_z1, b_z1;              // batch decomposition of blockIdx.z for A and B maps; b_batched = 0 -> weights shared
-    int b_batched;
-    // epilogue
-    __half* out;                 // fp16 output or nullptr
-    float* out_f32;              // fp32 output or nullptr
-    long long ldc;               // row stride (elements) of out
-    int out_z1;                  // blockIdx.z -> out offset (z % out_z1) * out_s_lo + (z / out_z1) * out_s_hi (elements)
-    long long out_s_lo, out_s_hi;
-    const float* bias;           // [N] fp32 or nullptr
-    const float* row_bias;       // [M / rows_per_group][N] fp32 (time-embedding term) or nullptr
-    int rows_per_group;
-    const __half* residual;      // same layout as out, or nullptr
-    long long ld_res;
-    int epi_mode;
-    float alpha;                 // scales the accumulator before bias
-    int m_valid;                 // rows >= m_valid (per batch) are not stored
-    int splits, kb_per_split;     // split-K: work item t -> (t % splits) K-range, partial sums RED-added (fp32) into splitk_ws[M][N]
-    float* splitk_ws;
-    int m_tiles, n_tiles, num_tiles;   // persistent tile loop: tile t -> n_blk = t % n_tiles, m_blk = (t / n_tiles) % m_tiles, z = t / (n_tiles * m_tiles)
-    __half* aux;                 // QuickGELU modes: pre-activation, same layout as out; EPI_RELU_BWD: the ReLU mask source
-};
-
-// ----------------------------------------------------------------------------------------------------------------
-// PTX wrappers
-// ----------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ uint32_t mbar_try(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    return ok;
-}
-// Bounded wait: a pipeline bug must surface as a trapped kernel (CUDA error at the caller's next sync), never as a hung GPU.
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    if (mbar_try(bar, parity)) return;
-    const long long t0 = clock64();
-    while (!mbar_try(bar, parity)) {
-        if (clock64() - t0 > 4000000000LL) __trap();
-    }
-}
-
-__device__ __forceinline__ void tma_load_4d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-
-__device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
-}
-
-// One lane of a converged warp (the lowest): callers keep the whole warp on the (warp-uniform) control path and predicate only the
-// TMA issue on it.
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
 
 template <int BLOCK_N> struct Cfg {
     static constexpr int kStages = BLOCK_N == 256 ? 4 : (BLOCK_N == 128 ? 6 : (BLOCK_N == 160 ? 5 : 4));   // BN=64: 96 KB -> 2 CTAs/SM

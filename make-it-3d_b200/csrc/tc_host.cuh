@@ -1,10 +1,54 @@
-// tc_host.cuh -- host side of the tensor-core tile kernel: TMA descriptor encoding + launch
+// tc_host.cuh -- host side of the tensor-core tile kernel (tc_gemm.cuh) and the fused attention (attn.cuh): their parameter types,
+// TMA descriptor encoding and tile planning.  Includable anywhere: the kernels and their launchers are compiled once, in plan.cu.
 #pragma once
-#include "tc_gemm.cuh"
+#include <cuda.h>
+#include <cuda_fp16.h>
+#include <cuda_runtime.h>
+#include <stdint.h>
 #include "mi3d_common.cuh"
 #include <cudaTypedefs.h>
 
 namespace tc {
+
+constexpr int BLOCK_M = 128;
+constexpr int BLOCK_K = 64;          // 64 fp16 = 128 B = one swizzle-128B atom row
+
+// EPI_QUICKGELU: out = y * sigmoid(1.702 y) (CLIP's MLP activation), y = alpha * acc + bias; the pre-activation y is also stored to aux
+//                when aux is set (the input-gradient pass needs it).
+// EPI_QUICKGELU_BWD: out = y * QuickGELU'(aux), aux = the saved pre-activation (same layout as out).
+// EPI_RELU: out = max(y, 0) (VGG's convs).  EPI_RELU_BWD: out = y * (aux > 0), aux = the saved post-ReLU input of the conv whose
+//                input gradient this is (same layout as out).  Both only in k_tc_gemm_vgg.
+// EPI_GELU: out = 0.5 y (1 + erf(y / sqrt 2)) (exact GELU, the SD-2 text encoder's MLP activation), y = alpha * acc + bias, in fp32,
+//                stored fp16.  Forward only; only in k_tc_gemm_gelu.
+enum EpiMode : int { EPI_PLAIN = 0, EPI_GEGLU = 1, EPI_TRANSPOSED = 2, EPI_QUICKGELU = 3, EPI_QUICKGELU_BWD = 4, EPI_RELU = 5, EPI_RELU_BWD = 6,
+                     EPI_GELU = 7 };
+
+struct GemmParams {
+    int M, N, K;                 // per-batch extents; N multiple of BLOCK_N, K multiple of 64, M multiple of 128 (rows may be padded)
+    int num_k_blocks;
+    int conv;                    // 0 plain, 1 implicit 3x3 conv, 2 implicit 3x3 conv over spatial blocks (k_tc_gemm_vgg)
+    int conv_H, conv_W, conv_bw, conv_bh, cin_blocks;
+    int a_z1, b_z1;              // batch decomposition of blockIdx.z for A and B maps; b_batched = 0 -> weights shared
+    int b_batched;
+    // epilogue
+    __half* out;                 // fp16 output or nullptr
+    float* out_f32;              // fp32 output or nullptr
+    long long ldc;               // row stride (elements) of out
+    int out_z1;                  // blockIdx.z -> out offset (z % out_z1) * out_s_lo + (z / out_z1) * out_s_hi (elements)
+    long long out_s_lo, out_s_hi;
+    const float* bias;           // [N] fp32 or nullptr
+    const float* row_bias;       // [M / rows_per_group][N] fp32 (time-embedding term) or nullptr
+    int rows_per_group;
+    const __half* residual;      // same layout as out, or nullptr
+    long long ld_res;
+    int epi_mode;
+    float alpha;                 // scales the accumulator before bias
+    int m_valid;                 // rows >= m_valid (per batch) are not stored
+    int splits, kb_per_split;     // split-K: work item t -> (t % splits) K-range, partial sums RED-added (fp32) into splitk_ws[M][N]
+    float* splitk_ws;
+    int m_tiles, n_tiles, num_tiles;   // persistent tile loop: tile t -> n_blk = t % n_tiles, m_blk = (t / n_tiles) % m_tiles, z = t / (n_tiles * m_tiles)
+    __half* aux;                 // QuickGELU modes: pre-activation, same layout as out; EPI_RELU_BWD: the ReLU mask source
+};
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -53,7 +97,7 @@ inline int make_map_nhwc(CUtensorMap* map, const __half* base, int C, int W, int
     return make_map_f16(map, base, dims, str, box);
 }
 
-// Only the plain kernel has a 160-wide instantiation (launch() below): epilogues PLAIN, GEGLU, TRANSPOSED, conv 0 or 1.
+// Only the plain kernel has a 160-wide instantiation (tc::launch in plan.cu): epilogues PLAIN, GEGLU, TRANSPOSED, conv 0 or 1.
 inline bool has_block_n_160(int epi_mode, int conv) { return conv != 2 && (epi_mode == EPI_PLAIN || epi_mode == EPI_GEGLU || epi_mode == EPI_TRANSPOSED); }
 
 inline int pick_block_n(int N, long long m_tiles_times_batch, int num_sms, bool allow_160 = true) {
@@ -65,71 +109,8 @@ inline int pick_block_n(int N, long long m_tiles_times_batch, int num_sms, bool 
     return 0;
 }
 
-template <int BN, bool kQuickGelu = false, bool kVgg = false, bool kGelu = false>
-inline int launch_bn(const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams& p, int batch, cudaStream_t st) {
-    static bool attr = false;
-    auto kernel = [] {
-        if constexpr (kVgg) return k_tc_gemm_vgg<BN>;
-        else if constexpr (kGelu) return k_tc_gemm_gelu<BN>;
-        else return k_tc_gemm<BN, kQuickGelu>;
-    }();
-    if (!attr) {
-        MI3D_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg<BN>::kSmemBytes));
-        attr = true;
-    }
-    GemmParams q = p;
-    q.m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M; q.n_tiles = p.N / BN;
-    if (q.splits <= 1) { q.splits = 1; q.kb_per_split = q.num_k_blocks; }
-    q.num_tiles = q.m_tiles * q.n_tiles * batch * q.splits;
-    static int sms = 0;
-    if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
-    const int resident = (Cfg<BN>::kSmemBytes <= 110 * 1024) ? 2 : 1;       // persistent grid: one (or two) CTAs per SM loop over the tiles
-    const int grid = q.num_tiles < sms * resident ? q.num_tiles : sms * resident;
-    kernel<<<grid, kThreads, Cfg<BN>::kSmemBytes, st>>>(ma, mb, q);
-    return (int)cudaGetLastError();
-}
-
-inline int launch(const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams& p, int block_n, int batch, cudaStream_t st) {
-    if (p.K % BLOCK_K || p.N % block_n || p.out_z1 < 1) return MI3D_ERR_ARG;
-    if (((uintptr_t)p.bias | (uintptr_t)p.row_bias | (uintptr_t)p.splitk_ws) & 15) return MI3D_ERR_ARG;     // read / RED-added 16 bytes at a time
-    if (p.conv == 2 || p.epi_mode == EPI_RELU || p.epi_mode == EPI_RELU_BWD) {
-        if (p.splits > 1 || (p.epi_mode == EPI_RELU_BWD && !p.aux)) return MI3D_ERR_ARG;
-        switch (block_n) {
-            case 64: return launch_bn<64, false, true>(ma, mb, p, batch, st);
-            case 128: return launch_bn<128, false, true>(ma, mb, p, batch, st);
-            case 256: return launch_bn<256, false, true>(ma, mb, p, batch, st);
-        }
-        return MI3D_ERR_ARG;
-    }
-    if (p.epi_mode == EPI_QUICKGELU || p.epi_mode == EPI_QUICKGELU_BWD) {
-        if (p.splits > 1) return MI3D_ERR_ARG;
-        switch (block_n) {
-            case 64: return launch_bn<64, true>(ma, mb, p, batch, st);
-            case 128: return launch_bn<128, true>(ma, mb, p, batch, st);
-            case 256: return launch_bn<256, true>(ma, mb, p, batch, st);
-        }
-        return MI3D_ERR_ARG;
-    }
-    if (p.epi_mode == EPI_GELU) {
-        if (p.splits > 1 || p.conv || !p.out) return MI3D_ERR_ARG;
-        switch (block_n) {
-            case 64: return launch_bn<64, false, false, true>(ma, mb, p, batch, st);
-            case 128: return launch_bn<128, false, false, true>(ma, mb, p, batch, st);
-            case 256: return launch_bn<256, false, false, true>(ma, mb, p, batch, st);
-        }
-        return MI3D_ERR_ARG;
-    }
-    switch (block_n) {
-        case 64: return launch_bn<64>(ma, mb, p, batch, st);
-        case 128: return launch_bn<128>(ma, mb, p, batch, st);
-        case 160: return launch_bn<160>(ma, mb, p, batch, st);
-        case 256: return launch_bn<256>(ma, mb, p, batch, st);
-    }
-    return MI3D_ERR_ARG;
-}
-
 // Split-K for the deep U-Net / VAE levels (M = 128 .. 512 rows): a handful of output tiles with K = 3 000 .. 23 000 would otherwise
-// run on a handful of SMs.  ws: fp32 [M][N] scratch (zeroed here).  Only plain fp16-output GEMMs / convs with batch == 1.
+// run on a handful of SMs.  Only plain fp16-output GEMMs / convs with batch == 1.
 inline int plan_splits(long long tiles, int num_k_blocks, int num_sms) {
     if (tiles * 2 > num_sms || num_k_blocks < 48) return 1;      // the zero-fill + finish passes are two more launches: only deep K pays
     int s = (int)(num_sms / tiles);
@@ -137,17 +118,33 @@ inline int plan_splits(long long tiles, int num_k_blocks, int num_sms) {
     while (s > 1 && num_k_blocks / s < 8) s--;
     return s;
 }
-inline int launch_splitk(const CUtensorMap& ma, const CUtensorMap& mb, GemmParams p, int block_n, int splits, float* ws, cudaStream_t st) {
-    p.kb_per_split = (p.num_k_blocks + splits - 1) / splits;
-    p.splits = (p.num_k_blocks + p.kb_per_split - 1) / p.kb_per_split;          // every K-range non-empty
-    p.splitk_ws = ws;
-    MI3D_CHECK(cudaMemsetAsync(ws, 0, (size_t)p.M * p.N * sizeof(float), st));
-    int r = launch(ma, mb, p, block_n, 1, st);
-    if (r) return r;
-    p.splits = 1;
-    const size_t total = (size_t)p.m_valid * p.N / 8;
-    k_splitk_finish<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(ws, p);
-    return (int)cudaGetLastError();
-}
 
 }  // namespace tc
+
+// The fused attention's Q / K / V maps; head_dim d: 40, 64, 80 or 160.
+namespace attn {
+
+inline bool supported(int d) { return d == 40 || d == 64 || d == 80 || d == 160; }
+
+struct Maps { CUtensorMap q, k, v; int d = 64; };
+
+// token matrices: x[(b * tokens + t) * ld + h * d + i]; every ld and the head stride 2 d bytes are multiples of 16 bytes
+inline int make_maps(Maps* m, const __half* q, long long ldq, const __half* k, long long ldk, const __half* v, long long ldv,
+                     int B, int T, int Tk, int heads, int d) {
+    if (!supported(d)) return MI3D_ERR_ARG;
+    m->d = d;
+    const uint32_t kv_rows = d > 128 ? 64 : 128;          // Shape<d>::kKeys
+    auto one = [&](CUtensorMap* map, const __half* base, long long ld, int tokens, uint32_t rows) {
+        const uint64_t dims[4] = {(uint64_t)d, (uint64_t)tokens, (uint64_t)heads, (uint64_t)B};
+        const uint64_t str[4] = {2, (uint64_t)ld * 2, (uint64_t)d * 2, (uint64_t)tokens * (uint64_t)ld * 2};
+        const uint32_t box[4] = {64, rows, 1, 1};
+        return tc::make_map_f16(map, base, dims, str, box);
+    };
+    int r = one(&m->q, q, ldq, T, 128);
+    if (r) return r;
+    r = one(&m->k, k, ldk, Tk, kv_rows);
+    if (r) return r;
+    return one(&m->v, v, ldv, Tk, kv_rows);
+}
+
+}  // namespace attn

@@ -1,8 +1,6 @@
 // tc_test.cu -- C-ABI entry points that run single ops of the engines' op layer (plan::Builder / plan::TowerBuilder) through the
 // builder methods the engines call (the tile GEMM, both implicit convs and both attention paths planned as in production, and the row
 // kernels), for the parity tests and for tools/ timing.
-#include "tc_host.cuh"
-#include "attn.cuh"
 #include "transformer_plan.cuh"
 #include "../../include/mi3d.h"
 
@@ -90,26 +88,23 @@ int mi3d_op_layernorm(const void* x, void* y, const float* gamma, const float* b
 int mi3d_op_layernorm_bwd(const void* x, const void* dy, const float* gamma, const void* add, void* dx, int rows, int C, float eps,
                           mi3d_stream_t stream) {
     if (rows < 1 || C % 8) return MI3D_ERR_ARG;
-    clipk::k_layernorm_bwd<<<(unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream>>>((const __half*)x, (const __half*)dy, gamma,
-                                                                                         (const __half*)add, (__half*)dx, rows, C, eps);
-    return (int)cudaGetLastError();
+    OneOp op;
+    op.b.layernorm_bwd((const __half*)x, (const __half*)dy, gamma, (const __half*)add, (__half*)dx, rows, C, eps);
+    return op.run(stream);
 }
 
 int mi3d_op_softmax(void* s, size_t rows, int cols, int valid, int causal_tq, float scale, mi3d_stream_t stream) {
     if (rows < 1 || cols % 8 || valid < 1 || valid > cols) return MI3D_ERR_ARG;
-    if (causal_tq > 0) {
-        clipk::k_softmax_causal<<<(unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream>>>((__half*)s, rows, cols, valid, causal_tq, scale);
-        return (int)cudaGetLastError();
-    }
     OneOp op;
-    op.b.softmax((__half*)s, rows, cols, valid, scale);
+    op.b.softmax((__half*)s, rows, cols, valid, scale, causal_tq);
     return op.run(stream);
 }
 
 int mi3d_op_softmax_bwd(const void* p, void* dp, size_t rows, int cols, float scale, mi3d_stream_t stream) {
     if (rows < 1 || cols % 8) return MI3D_ERR_ARG;
-    sdk::k_softmax_bwd<<<(unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream>>>((const __half*)p, (__half*)dp, rows, cols, scale);
-    return (int)cudaGetLastError();
+    OneOp op;
+    op.b.softmax_bwd((const __half*)p, (__half*)dp, rows, cols, scale);
+    return op.run(stream);
 }
 
 int mi3d_op_transpose(const void* in, void* out, int Z, int R, int C, mi3d_stream_t stream) {

@@ -4,7 +4,9 @@
 // atoms, block stride = rows * 128 B), written by ordinary threads through sw_off().  tf32 wgmma reads both operands K-major:
 // rows = M or N index, columns = K (descriptor: SBO = 1024 B, K advances by +32 B inside the row).
 #pragma once
-#include "tc_gemm.cuh"
+#include <cuda_runtime.h>
+#include "tma.cuh"
+#include "wgmma.cuh"
 
 namespace ftc {
 

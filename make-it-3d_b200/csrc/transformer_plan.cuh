@@ -5,7 +5,6 @@
 // valid row.  Per-head products run as batched tile GEMMs over z = b * heads + h; head_dim is 64.
 #pragma once
 #include "engine_plan.cuh"
-#include "clip_kernels.cuh"
 
 namespace plan {
 
@@ -46,16 +45,7 @@ struct TowerBuilder : Builder {
         const int C = t.C, Tp = t.Tpad;
         transpose(a.qkv, a.qkvT, B, Tp, 3 * C);                                          // [b][3C][Tpad]
         bgemm(heads_rows(a.qkv, 3 * C, t), heads_rows(a.qkv + C, 3 * C, t), Tp, a.S, Tp, 0, (long long)Tp * Tp, 1, B, t);
-        const size_t rows = (size_t)B * t.heads * Tp;
-        if (causal) {
-            __half* s = a.S; const int T = t.T;
-            push([=](cudaStream_t st) {
-                clipk::k_softmax_causal<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(s, rows, Tp, T, Tp, 0.125f);
-                return (int)cudaGetLastError();
-            });
-        } else {
-            softmax(a.S, rows, Tp, t.T, 0.125f);
-        }
+        softmax(a.S, (size_t)B * t.heads * Tp, Tp, t.T, 0.125f, causal ? Tp : 0);
         bgemm(scores(a.S, t), heads_cols(a.qkvT + 2LL * C * Tp, 3 * C, t), 64, a.ao, C, 64, (long long)Tp * C, t.heads, B, t);
     }
 

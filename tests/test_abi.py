@@ -1,7 +1,12 @@
 """CPU: the C-ABI library builds for sm_90a, loads without a GPU, and exports exactly what include/mi3d.h declares."""
+import collections
 import ctypes
 import os
 import re
+import shutil
+import subprocess
+
+import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -20,6 +25,22 @@ def test_library_exports_every_declared_symbol(mi3d):
         assert hasattr(lib, s), f"libmi3d.so does not export {s}"
     assert sorted(mi3d._lib.SYMBOLS) == syms
     assert b"sm_90a" in lib.mi3d_version()
+
+
+def test_each_kernel_is_compiled_once(mi3d):
+    """Every kernel has one home: a kernel that several translation units compile shows up once per unit in the library's SASS."""
+    cuda_bin = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin")
+    cuobjdump = shutil.which("cuobjdump") or shutil.which("cuobjdump", path=cuda_bin)
+    cufilt = shutil.which("cu++filt") or shutil.which("cu++filt", path=cuda_bin)
+    if not cuobjdump or not cufilt:
+        pytest.skip("cuobjdump / cu++filt from the CUDA toolkit not found")
+    sass = subprocess.run([cuobjdump, "-sass", mi3d._lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
+    mangled = re.findall(r"^\s*Function : (\S+)", sass, flags=re.M)
+    assert mangled
+    names = subprocess.run([cufilt], input="\n".join(mangled), capture_output=True, text=True, check=True).stdout.splitlines()
+    names = [n.replace("(anonymous namespace)::", "").replace("<unnamed>::", "") for n in names]
+    repeated = {n: c for n, c in collections.Counter(names).items() if c > 1}
+    assert not repeated, f"kernels compiled more than once: {repeated}"
 
 
 def test_workspace_queries_are_pure_host(mi3d):
