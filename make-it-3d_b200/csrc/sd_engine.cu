@@ -145,9 +145,16 @@ struct Engine : Builder {
     }
 
     // ------------------------------------------------------------------------------------------------------
-    // U-Net pieces (diffusers naming)
+    // diffusers blocks (diffusers naming)
     // ------------------------------------------------------------------------------------------------------
-    T4 resnet(const std::string& pre, const T4& x, int cout, bool has_temb, float eps, std::vector<GN>* tape = nullptr, std::vector<T4>* acts = nullptr) {
+    // Each param() / pf() is a statement of its own, never another call's argument: the seeded stand-in weights are drawn in registry order.
+    // what the VAE encoder's input-gradient pass (build_vae_bwd) reads of a forward block
+    struct ResTape { std::string pre; T4 x; int cout; GN g1, g2; };
+    struct AttnTape { std::string pre; T4 x; GN g; __half *q, *k, *v, *P; };
+
+    // ResnetBlock2D: the U-Net's (has_temb, eps 1e-5), the VAE encoder's (tape: weights with a dgrad copy, *tape filled) and the
+    // VAE decoder's (eps 1e-6)
+    T4 resnet(const std::string& pre, const T4& x, int cout, bool has_temb, float eps, ResTape* tape = nullptr) {
         const int cin = x.c;
         T4 a1 = act(x.n, x.h, x.w, cin);
         GN g1 = groupnorm(x, pre + ".norm1", eps, 1, a1);
@@ -161,24 +168,26 @@ struct Engine : Builder {
             temb_max_n = std::max(temb_max_n, cout);
             rb = tp;
         }
-        const bool both = tape != nullptr;
-        Param& w1 = param(pre + ".conv1.weight", {cout, cin, 3, 3}, both ? PK_CONV3_BOTH : PK_CONV3);
+        const PKind k3 = tape ? PK_CONV3_BOTH : PK_CONV3, k1 = tape ? PK_CONV1_BOTH : PK_CONV1;
+        const __half* w1 = (const __half*)param(pre + ".conv1.weight", {cout, cin, 3, 3}, k3).dst;
         T4 h1 = act(x.n, x.h, x.w, cout);
-        conv3(a1, (const __half*)w1.dst, cout, h1, pf(pre + ".conv1.bias", {cout}), rb);
+        const float* b1 = pf(pre + ".conv1.bias", {cout});
+        conv3(a1, w1, cout, h1, b1, rb);
         T4 a2 = act(x.n, x.h, x.w, cout);
         GN g2 = groupnorm(h1, pre + ".norm2", eps, 1, a2);
         const __half* sc = x.p;
         if (cin != cout) {
-            Param& ws = param(pre + ".conv_shortcut.weight", {cout, cin, 1, 1}, both ? PK_CONV1_BOTH : PK_CONV1);
+            const __half* ws = (const __half*)param(pre + ".conv_shortcut.weight", {cout, cin, 1, 1}, k1).dst;
             T4 s = act(x.n, x.h, x.w, cout);
-            linear(x.p, x.rows(), cin, (const __half*)ws.dst, cout, s.p, pf(pre + ".conv_shortcut.bias", {cout}));
+            const float* bs = pf(pre + ".conv_shortcut.bias", {cout});
+            linear(x.p, x.rows(), cin, ws, cout, s.p, bs);
             sc = s.p;
         }
-        Param& w2 = param(pre + ".conv2.weight", {cout, cout, 3, 3}, both ? PK_CONV3_BOTH : PK_CONV3);
+        const __half* w2 = (const __half*)param(pre + ".conv2.weight", {cout, cout, 3, 3}, k3).dst;
         T4 out = act(x.n, x.h, x.w, cout);
-        conv3(a2, (const __half*)w2.dst, cout, out, pf(pre + ".conv2.bias", {cout}), nullptr, sc);
-        if (tape) { tape->push_back(g1); tape->push_back(g2); }
-        if (acts) { acts->push_back(a1); acts->push_back(a2); }
+        const float* b2 = pf(pre + ".conv2.bias", {cout});
+        conv3(a2, w2, cout, out, b2, nullptr, sc);
+        if (tape) *tape = ResTape{pre, x, cout, g1, g2};
         return out;
     }
 
@@ -191,47 +200,46 @@ struct Engine : Builder {
         // proj_in / proj_out: Linear [C, C] (SD-2.x) or 1x1 Conv2d [C, C, 1, 1] (SD-1.x), the same [C][C] fp16 matrix either way
         const std::vector<int> pshape = ucfg.proj_conv ? std::vector<int>{C, C, 1, 1} : std::vector<int>{C, C};
         const PKind pkind = ucfg.proj_conv ? PK_CONV1 : PK_LINEAR;
-        linear(n.p, M, C, (const __half*)param(pre + ".proj_in.weight", pshape, pkind).dst, C, h, pf(pre + ".proj_in.bias", {C}));
+        const float* b_in = pf(pre + ".proj_in.bias", {C});
+        const __half* w_in = (const __half*)param(pre + ".proj_in.weight", pshape, pkind).dst;
+        linear(n.p, M, C, w_in, C, h, b_in);
         const std::string tb = pre + ".transformer_blocks.0";
         // ---- self attention ----
         __half* ln = alloc16(M * C);
         layernorm(h, M, C, tb + ".norm1", ln);
-        // to_q / to_k / to_v weights are allocated back to back ([3C][C]): one GEMM produces q | k | v side by side
+        // to_q / to_k / to_v are registered back to back, and each starts on an alloc() boundary: for C % 32 == 0 they are one [3C][C]
+        // matrix, and one GEMM produces q | k | v side by side.  Any other layout fails the build.
         const __half* wq = (const __half*)param(tb + ".attn1.to_q.weight", {C, C}, PK_LINEAR).dst;
         const __half* wk = (const __half*)param(tb + ".attn1.to_k.weight", {C, C}, PK_LINEAR).dst;
         const __half* wv = (const __half*)param(tb + ".attn1.to_v.weight", {C, C}, PK_LINEAR).dst;
+        if (wk != wq + (size_t)C * C || wv != wk + (size_t)C * C) err = MI3D_ERR_ARG;
         __half* ao = alloc16(M * C);
-        if (wk == wq + (size_t)C * C && wv == wk + (size_t)C * C) {
-            __half* qkv = alloc16(M * 3 * C);
-            linear(ln, M, C, wq, 3 * C, qkv);
-            attention_core(qkv, 3 * C, qkv + C, 3 * C, qkv + 2 * C, 3 * C, B, T, T, T, heads, d, ao, C);
-        } else {
-            __half* qb = alloc16(M * C); __half* kb = alloc16(M * C); __half* vb = alloc16(M * C);
-            linear(ln, M, C, wq, C, qb); linear(ln, M, C, wk, C, kb); linear(ln, M, C, wv, C, vb);
-            attention_core(qb, C, kb, C, vb, C, B, T, T, T, heads, d, ao, C);
-        }
+        __half* qkv = alloc16(M * 3 * C);
+        linear(ln, M, C, wq, 3 * C, qkv);
+        attention_core(qkv, 3 * C, qkv + C, 3 * C, qkv + 2 * C, 3 * C, B, T, T, T, heads, d, ao, C);
         __half* h2 = alloc16(M * C);
-        linear(ao, M, C, (const __half*)param(tb + ".attn1.to_out.0.weight", {C, C}, PK_LINEAR).dst, C, h2, pf(tb + ".attn1.to_out.0.bias", {C}), h);
+        const float* bo1 = pf(tb + ".attn1.to_out.0.bias", {C});
+        const __half* wo1 = (const __half*)param(tb + ".attn1.to_out.0.weight", {C, C}, PK_LINEAR).dst;
+        linear(ao, M, C, wo1, C, h2, bo1, h);
         // ---- cross attention (keys/values from the text context, padded to ctx_pad rows per batch) ----
         __half* ln2 = alloc16(M * C);
         layernorm(h2, M, C, tb + ".norm2", ln2);
         const long long Mc = (long long)B * ctx_pad;
         __half* q2 = alloc16(M * C);
-        linear(ln2, M, C, (const __half*)param(tb + ".attn2.to_q.weight", {C, C}, PK_LINEAR).dst, C, q2);
+        const __half* wq2 = (const __half*)param(tb + ".attn2.to_q.weight", {C, C}, PK_LINEAR).dst;
+        linear(ln2, M, C, wq2, C, q2);
+        // to_k / to_v likewise one [2C][cross] matrix (C * cross % 512 == 0): one GEMM produces k | v
         const __half* wk2 = (const __half*)param(tb + ".attn2.to_k.weight", {C, cross}, PK_LINEAR).dst;
         const __half* wv2 = (const __half*)param(tb + ".attn2.to_v.weight", {C, cross}, PK_LINEAR).dst;
+        if (wv2 != wk2 + (size_t)C * cross) err = MI3D_ERR_ARG;
         __half* ao2 = alloc16(M * C);
-        if (wv2 == wk2 + (size_t)C * cross) {
-            __half* kv = alloc16(Mc * 2 * C);
-            linear(ctx16, Mc, cross, wk2, 2 * C, kv);
-            attention_core(q2, C, kv, 2 * C, kv + C, 2 * C, B, T, ctx_pad, ucfg.ctx_len, heads, d, ao2, C);
-        } else {
-            __half* k2 = alloc16(Mc * C); __half* v2 = alloc16(Mc * C);
-            linear(ctx16, Mc, cross, wk2, C, k2); linear(ctx16, Mc, cross, wv2, C, v2);
-            attention_core(q2, C, k2, C, v2, C, B, T, ctx_pad, ucfg.ctx_len, heads, d, ao2, C);
-        }
+        __half* kv = alloc16(Mc * 2 * C);
+        linear(ctx16, Mc, cross, wk2, 2 * C, kv);
+        attention_core(q2, C, kv, 2 * C, kv + C, 2 * C, B, T, ctx_pad, ucfg.ctx_len, heads, d, ao2, C);
         __half* h3 = alloc16(M * C);
-        linear(ao2, M, C, (const __half*)param(tb + ".attn2.to_out.0.weight", {C, C}, PK_LINEAR).dst, C, h3, pf(tb + ".attn2.to_out.0.bias", {C}), h2);
+        const float* bo2 = pf(tb + ".attn2.to_out.0.bias", {C});
+        const __half* wo2 = (const __half*)param(tb + ".attn2.to_out.0.weight", {C, C}, PK_LINEAR).dst;
+        linear(ao2, M, C, wo2, C, h3, bo2, h2);
         // ---- GEGLU feed-forward ----
         __half* ln3 = alloc16(M * C);
         layernorm(h3, M, C, tb + ".norm3", ln3);
@@ -241,18 +249,37 @@ struct Engine : Builder {
         __half* f1 = alloc16(M * 4 * C);
         linear(ln3, M, C, (const __half*)wg.dst, 8 * C, f1, (const float*)bg.dst, nullptr, tc::EPI_GEGLU);
         __half* h4 = alloc16(M * C);
-        linear(f1, M, 4 * C, (const __half*)param(tb + ".ff.net.2.weight", {C, 4 * C}, PK_LINEAR).dst, C, h4, pf(tb + ".ff.net.2.bias", {C}), h3);
+        const float* bf = pf(tb + ".ff.net.2.bias", {C});
+        const __half* wf = (const __half*)param(tb + ".ff.net.2.weight", {C, 4 * C}, PK_LINEAR).dst;
+        linear(f1, M, 4 * C, wf, C, h4, bf, h3);
         T4 out = act(x.n, x.h, x.w, C);
-        linear(h4, M, C, (const __half*)param(pre + ".proj_out.weight", pshape, pkind).dst, C, out.p, pf(pre + ".proj_out.bias", {C}), x.p);
+        const float* b_out = pf(pre + ".proj_out.bias", {C});
+        const __half* w_out = (const __half*)param(pre + ".proj_out.weight", pshape, pkind).dst;
+        linear(h4, M, C, w_out, C, out.p, b_out, x.p);
         return out;
     }
 
-    T4 downsample(const std::string& pre, const T4& x, int pad_lo, bool both, __half** col_out = nullptr) {
+    T4 downsample(const std::string& pre, const T4& x, int pad_lo, bool both) {
         const int C = x.c;
-        Param& w = param(pre + ".conv.weight", {C, C, 3, 3}, both ? PK_CONV3_S2_BOTH : PK_CONV3);
+        const __half* w = (const __half*)param(pre + ".conv.weight", {C, C, 3, 3}, both ? PK_CONV3_S2_BOTH : PK_CONV3).dst;
         T4 y = act(x.n, x.h / 2, x.w / 2, C);
-        __half* col = conv3_s2(x, (const __half*)w.dst, y, pf(pre + ".conv.bias", {C}), pad_lo);
-        if (col_out) *col_out = col;
+        const float* b = pf(pre + ".conv.bias", {C});
+        conv3_s2(x, w, y, b, pad_lo);
+        return y;
+    }
+
+    // Upsample2D: nearest 2x, then a 3x3 conv
+    T4 upsample(const std::string& pre, const T4& x) {
+        T4 up = act(x.n, x.h * 2, x.w * 2, x.c);
+        const T4 xx = x;
+        push([=](cudaStream_t st) {
+            sdk::k_upsample2x<<<blocks_for(up.numel() / 8), 256, 0, st>>>(xx.p, up.p, xx.n, xx.h, xx.w, xx.c);
+            return (int)cudaGetLastError();
+        });
+        T4 y = act(up.n, up.h, up.w, up.c);
+        const float* b = pf(pre + ".conv.bias", {x.c});
+        const __half* w = (const __half*)param(pre + ".conv.weight", {x.c, x.c, 3, 3}, PK_CONV3).dst;
+        conv3(up, w, x.c, y, b);
         return y;
     }
 
@@ -284,8 +311,12 @@ struct Engine : Builder {
                 sdk::k_time_proj<<<(B * c0 / 2 + 127) / 128, 128, 0, st>>>(tptr, tproj, B, c0);
                 return (int)cudaGetLastError();
             });
-            linear_small(tproj, (const __half*)param("time_embedding.linear_1.weight", {tdim, c0}, PK_LINEAR).dst, pf("time_embedding.linear_1.bias", {tdim}), t1, B, tdim, c0, 0, 1);
-            linear_small(t1, (const __half*)param("time_embedding.linear_2.weight", {tdim, tdim}, PK_LINEAR).dst, pf("time_embedding.linear_2.bias", {tdim}), temb, B, tdim, tdim, 0, 0);
+            const float* b1 = pf("time_embedding.linear_1.bias", {tdim});
+            const __half* w1 = (const __half*)param("time_embedding.linear_1.weight", {tdim, c0}, PK_LINEAR).dst;
+            linear_small(tproj, w1, b1, t1, B, tdim, c0, 0, 1);
+            const float* b2 = pf("time_embedding.linear_2.bias", {tdim});
+            const __half* w2 = (const __half*)param("time_embedding.linear_2.weight", {tdim, tdim}, PK_LINEAR).dst;
+            linear_small(t1, w2, b2, temb, B, tdim, tdim, 0, 0);
             temb_jobs.clear(); temb_max_n = 0;
             temb_jobs_dev = (sdk::SmallLinearJob*)alloc(64 * sizeof(sdk::SmallLinearJob));
             const float* te = temb;
@@ -332,18 +363,7 @@ struct Engine : Builder {
                 h = resnet("up_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), cat, c.block_out[lev], true, 1e-5f);
                 if (has_attn) h = transformer("up_blocks." + std::to_string(i) + ".attentions." + std::to_string(j), h, c.heads[lev]);
             }
-            if (i < nlev - 1) {
-                T4 up = act(h.n, h.h * 2, h.w * 2, h.c);
-                const T4 hh = h;
-                push([=](cudaStream_t st) {
-                    sdk::k_upsample2x<<<blocks_for(up.numel() / 8), 256, 0, st>>>(hh.p, up.p, hh.n, hh.h, hh.w, hh.c);
-                    return (int)cudaGetLastError();
-                });
-                T4 y = act(up.n, up.h, up.w, up.c);
-                const std::string up_pre = "up_blocks." + std::to_string(i) + ".upsamplers.0.conv";
-                conv3(up, (const __half*)param(up_pre + ".weight", {h.c, h.c, 3, 3}, PK_CONV3).dst, h.c, y, pf(up_pre + ".bias", {h.c}));
-                h = y;
-            }
+            if (i < nlev - 1) h = upsample("up_blocks." + std::to_string(i) + ".upsamplers.0", h);
             tap("unet.up" + std::to_string(i), h.p, h.numel() * 2);
         }
         T4 a = act(h.n, h.h, h.w, h.c);
@@ -364,37 +384,49 @@ struct Engine : Builder {
     // ------------------------------------------------------------------------------------------------------
     // VAE encoder forward + input-gradient backward (AutoencoderKL.encode, nerf/sd.py:212-220)
     // ------------------------------------------------------------------------------------------------------
-    struct ResTape { T4 x, a1, h1, a2, out; GN g1, g2; bool shortcut; std::string pre; int cin, cout; };
     struct DownTape { T4 x, y; std::string pre; };
-    struct AttnTape { T4 x, n; GN g; __half *q, *k, *v, *P, *ao; int C, T; std::string pre; };
 
     std::vector<ResTape> vres; std::vector<DownTape> vdown; AttnTape vattn; GN vgn_out; T4 v_a_out, v_h_last, v_conv_in_out;
     std::vector<int> vorder;   // 0 = res, 1 = down, 2 = attn ; forward order for the reverse walk
 
-    T4 vae_resnet(const std::string& pre, const T4& x, int cout) {
-        ResTape t; t.pre = pre; t.x = x; t.cin = x.c; t.cout = cout; t.shortcut = x.c != cout;
-        std::vector<GN> gns; std::vector<T4> acts;
-        // re-implemented inline (needs h1 for the tape)
-        const int cin = x.c;
-        t.a1 = act(x.n, x.h, x.w, cin);
-        t.g1 = groupnorm(x, pre + ".norm1", 1e-6f, 1, t.a1);
-        Param& w1 = param(pre + ".conv1.weight", {cout, cin, 3, 3}, PK_CONV3_BOTH);
-        t.h1 = act(x.n, x.h, x.w, cout);
-        conv3(t.a1, (const __half*)w1.dst, cout, t.h1, pf(pre + ".conv1.bias", {cout}));
-        t.a2 = act(x.n, x.h, x.w, cout);
-        t.g2 = groupnorm(t.h1, pre + ".norm2", 1e-6f, 1, t.a2);
-        const __half* sc = x.p;
-        if (t.shortcut) {
-            Param& ws = param(pre + ".conv_shortcut.weight", {cout, cin, 1, 1}, PK_CONV1_BOTH);
-            T4 s = act(x.n, x.h, x.w, cout);
-            linear(x.p, x.rows(), cin, (const __half*)ws.dst, cout, s.p, pf(pre + ".conv_shortcut.bias", {cout}));
-            sc = s.p;
-        }
-        Param& w2 = param(pre + ".conv2.weight", {cout, cout, 3, 3}, PK_CONV3_BOTH);
-        t.out = act(x.n, x.h, x.w, cout);
-        conv3(t.a2, (const __half*)w2.dst, cout, t.out, pf(pre + ".conv2.bias", {cout}), nullptr, sc);
-        vres.push_back(t); vorder.push_back(0);
-        return t.out;
+    // the VAE's Attention: one head over all pixels (tape: weights with a transposed copy, *tape filled)
+    T4 vae_attention(const std::string& pre, const T4& x, AttnTape* tape) {
+        const PKind kind = tape ? PK_LINEAR_BOTH : PK_LINEAR;
+        const long long M = x.rows(); const int C = x.c;
+        T4 n = act(x.n, x.h, x.w, C);
+        GN g = groupnorm(x, pre + ".group_norm", 1e-6f, 0, n);
+        __half *q = alloc16(M * C), *k = alloc16(M * C), *v = alloc16(M * C), *vT = alloc16(M * C);
+        const float* bq = pf(pre + ".to_q.bias", {C});
+        const __half* wq = (const __half*)param(pre + ".to_q.weight", {C, C}, kind).dst;
+        linear(n.p, M, C, wq, C, q, bq);
+        const float* bk = pf(pre + ".to_k.bias", {C});
+        const __half* wk = (const __half*)param(pre + ".to_k.weight", {C, C}, kind).dst;
+        linear(n.p, M, C, wk, C, k, bk);
+        const float* bv = pf(pre + ".to_v.bias", {C});
+        const __half* wv = (const __half*)param(pre + ".to_v.weight", {C, C}, kind).dst;
+        linear(n.p, M, C, wv, C, v, bv);
+        transpose(v, vT, 1, (int)M, C);
+        __half* P = alloc16((size_t)M * M);
+        { Mat qa{q, C, M, C}; Mat kb{k, C, M, C}; Out oo; oo.p16 = P; oo.ldc = M; Epi e; gemm(qa, kb, (int)M, oo, e); }
+        softmax(P, (size_t)M, (int)M, (int)M, 1.0f / sqrtf((float)C));
+        __half* ao = alloc16(M * C);
+        { Mat pa{P, M, M, (int)M}; Mat vb{vT, M, C, (int)M}; Out oo; oo.p16 = ao; oo.ldc = C; Epi e; gemm(pa, vb, C, oo, e); }
+        T4 out = act(x.n, x.h, x.w, C);
+        const float* bo = pf(pre + ".to_out.0.bias", {C});
+        const __half* wo = (const __half*)param(pre + ".to_out.0.weight", {C, C}, kind).dst;
+        linear(ao, M, C, wo, C, out.p, bo, x.p);
+        if (tape) *tape = AttnTape{pre, x, g, q, k, v, P};
+        return out;
+    }
+
+    // the VAE's mid block: resnet, attention, resnet; taped (the encoder's) in vres / vattn / vorder for build_vae_bwd
+    T4 vae_mid(const std::string& pre, T4 h, bool taped) {
+        ResTape t0, t1;
+        h = resnet(pre + ".resnets.0", h, h.c, false, 1e-6f, taped ? &t0 : nullptr);
+        h = vae_attention(pre + ".attentions.0", h, taped ? &vattn : nullptr);
+        h = resnet(pre + ".resnets.1", h, h.c, false, 1e-6f, taped ? &t1 : nullptr);
+        if (taped) { vres.push_back(t0); vres.push_back(t1); vorder.insert(vorder.end(), {0, 2, 0}); }
+        return h;
     }
 
     void build_vae() {
@@ -409,11 +441,11 @@ struct Engine : Builder {
             conv_small_cin(vae_in, w, b, h);
         }
         v_conv_in_out = h;
-        int ch = c.block_out[0];
         for (int i = 0; i < nlev; i++) {
             for (int j = 0; j < L; j++) {
-                h = vae_resnet("encoder.down_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), h, c.block_out[i]);
-                ch = c.block_out[i];
+                ResTape t;
+                h = resnet("encoder.down_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), h, c.block_out[i], false, 1e-6f, &t);
+                vres.push_back(t); vorder.push_back(0);
             }
             if (i < nlev - 1) {
                 DownTape d; d.x = h; d.pre = "encoder.down_blocks." + std::to_string(i) + ".downsamplers.0";
@@ -421,36 +453,8 @@ struct Engine : Builder {
                 d.y = h; vdown.push_back(d); vorder.push_back(1);
             }
         }
-        h = vae_resnet("encoder.mid_block.resnets.0", h, ch);
-        {   // single-head attention over all pixels
-            AttnTape& a = vattn; a.pre = "encoder.mid_block.attentions.0"; a.x = h; a.C = ch; a.T = h.h * h.w;
-            const long long M = h.rows(); const int C = ch;
-            a.n = act(h.n, h.h, h.w, C);
-            a.g = groupnorm(h, a.pre + ".group_norm", 1e-6f, 0, a.n);
-            a.q = alloc16(M * C); a.k = alloc16(M * C); a.v = alloc16(M * C);
-            __half* vT = alloc16(M * C);
-            linear(a.n.p, M, C, (const __half*)param(a.pre + ".to_q.weight", {C, C}, PK_LINEAR_BOTH).dst, C, a.q, pf(a.pre + ".to_q.bias", {C}));
-            linear(a.n.p, M, C, (const __half*)param(a.pre + ".to_k.weight", {C, C}, PK_LINEAR_BOTH).dst, C, a.k, pf(a.pre + ".to_k.bias", {C}));
-            linear(a.n.p, M, C, (const __half*)param(a.pre + ".to_v.weight", {C, C}, PK_LINEAR_BOTH).dst, C, a.v, pf(a.pre + ".to_v.bias", {C}));
-            transpose(a.v, vT, 1, (int)M, C);
-            a.P = alloc16((size_t)M * M);
-            {
-                Mat qa{a.q, C, M, C}; Mat kb{a.k, C, M, C};
-                Out oo; oo.p16 = a.P; oo.ldc = M; Epi e;
-                gemm(qa, kb, (int)M, oo, e);
-            }
-            softmax(a.P, (size_t)M, (int)M, (int)M, 1.0f / sqrtf((float)C));
-            a.ao = alloc16(M * C);
-            {
-                Mat pa{a.P, M, M, (int)M}; Mat vb{vT, M, C, (int)M};
-                Out oo; oo.p16 = a.ao; oo.ldc = C; Epi e;
-                gemm(pa, vb, C, oo, e);
-            }
-            T4 out = act(h.n, h.h, h.w, C);
-            linear(a.ao, M, C, (const __half*)param(a.pre + ".to_out.0.weight", {C, C}, PK_LINEAR_BOTH).dst, C, out.p, pf(a.pre + ".to_out.0.bias", {C}), h.p);
-            h = out; vorder.push_back(2);
-        }
-        h = vae_resnet("encoder.mid_block.resnets.1", h, ch);
+        h = vae_mid("encoder.mid_block", h, true);
+        const int ch = h.c;
         v_h_last = h;
         v_a_out = act(h.n, h.h, h.w, ch);
         vgn_out = groupnorm(h, "encoder.conv_norm_out", 1e-6f, 1, v_a_out);
@@ -471,26 +475,6 @@ struct Engine : Builder {
     // ------------------------------------------------------------------------------------------------------
     // VAE decoder (diffusers AutoencoderKL.decode: post_quant_conv folded into the API kernel, then Decoder): forward only.
     // ------------------------------------------------------------------------------------------------------
-    T4 dec_resnet(const std::string& pre, const T4& x, int cout) {
-        const int cin = x.c;
-        T4 a1 = act(x.n, x.h, x.w, cin);
-        groupnorm(x, pre + ".norm1", 1e-6f, 1, a1);
-        T4 h1 = act(x.n, x.h, x.w, cout);
-        conv3(a1, (const __half*)param(pre + ".conv1.weight", {cout, cin, 3, 3}, PK_CONV3).dst, cout, h1, pf(pre + ".conv1.bias", {cout}));
-        T4 a2 = act(x.n, x.h, x.w, cout);
-        groupnorm(h1, pre + ".norm2", 1e-6f, 1, a2);
-        const __half* sc = x.p;
-        if (cin != cout) {
-            T4 sh = act(x.n, x.h, x.w, cout);
-            linear(x.p, x.rows(), cin, (const __half*)param(pre + ".conv_shortcut.weight", {cout, cin, 1, 1}, PK_CONV1).dst, cout, sh.p,
-                   pf(pre + ".conv_shortcut.bias", {cout}));
-            sc = sh.p;
-        }
-        T4 out = act(x.n, x.h, x.w, cout);
-        conv3(a2, (const __half*)param(pre + ".conv2.weight", {cout, cout, 3, 3}, PK_CONV3).dst, cout, out, pf(pre + ".conv2.bias", {cout}), nullptr, sc);
-        return out;
-    }
-
     void build_vae_dec() {
         begin_list(&dec_ops);
         const mi3d_vae_cfg& c = vcfg;
@@ -505,43 +489,12 @@ struct Engine : Builder {
             if (c.latent_ch != 4) err = MI3D_ERR_ARG;
             conv_small_cin(dec_in, w, b, h);
         }
-        h = dec_resnet("decoder.mid_block.resnets.0", h, ch);
-        {   // single-head attention over all pixels (same construction as the encoder's, no tape)
-            const std::string pre = "decoder.mid_block.attentions.0";
-            const long long M = h.rows(); const int C = ch;
-            T4 n = act(h.n, h.h, h.w, C);
-            groupnorm(h, pre + ".group_norm", 1e-6f, 0, n);
-            __half *q = alloc16(M * C), *k = alloc16(M * C), *v = alloc16(M * C), *vT = alloc16(M * C);
-            linear(n.p, M, C, (const __half*)param(pre + ".to_q.weight", {C, C}, PK_LINEAR).dst, C, q, pf(pre + ".to_q.bias", {C}));
-            linear(n.p, M, C, (const __half*)param(pre + ".to_k.weight", {C, C}, PK_LINEAR).dst, C, k, pf(pre + ".to_k.bias", {C}));
-            linear(n.p, M, C, (const __half*)param(pre + ".to_v.weight", {C, C}, PK_LINEAR).dst, C, v, pf(pre + ".to_v.bias", {C}));
-            transpose(v, vT, 1, (int)M, C);
-            __half* P = alloc16((size_t)M * M);
-            { Mat qa{q, C, M, C}; Mat kb{k, C, M, C}; Out oo; oo.p16 = P; oo.ldc = M; Epi e; gemm(qa, kb, (int)M, oo, e); }
-            softmax(P, (size_t)M, (int)M, (int)M, 1.0f / sqrtf((float)C));
-            __half* ao = alloc16(M * C);
-            { Mat pa{P, M, M, (int)M}; Mat vb{vT, M, C, (int)M}; Out oo; oo.p16 = ao; oo.ldc = C; Epi e; gemm(pa, vb, C, oo, e); }
-            T4 out = act(h.n, h.h, h.w, C);
-            linear(ao, M, C, (const __half*)param(pre + ".to_out.0.weight", {C, C}, PK_LINEAR).dst, C, out.p, pf(pre + ".to_out.0.bias", {C}), h.p);
-            h = out;
-        }
-        h = dec_resnet("decoder.mid_block.resnets.1", h, ch);
+        h = vae_mid("decoder.mid_block", h, false);
         for (int i = 0; i < nlev; i++) {
             const int co = c.block_out[nlev - 1 - i];
-            for (int j = 0; j < L + 1; j++) h = dec_resnet("decoder.up_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), h, co);
+            for (int j = 0; j < L + 1; j++) h = resnet("decoder.up_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), h, co, false, 1e-6f);
             ch = co;
-            if (i < nlev - 1) {
-                T4 up = act(h.n, h.h * 2, h.w * 2, h.c);
-                const T4 hh = h;
-                push([=](cudaStream_t st) {
-                    sdk::k_upsample2x<<<blocks_for(up.numel() / 8), 256, 0, st>>>(hh.p, up.p, hh.n, hh.h, hh.w, hh.c);
-                    return (int)cudaGetLastError();
-                });
-                T4 y = act(up.n, up.h, up.w, up.c);
-                const std::string up_pre = "decoder.up_blocks." + std::to_string(i) + ".upsamplers.0.conv";
-                conv3(up, (const __half*)param(up_pre + ".weight", {h.c, h.c, 3, 3}, PK_CONV3).dst, h.c, y, pf(up_pre + ".bias", {h.c}));
-                h = y;
-            }
+            if (i < nlev - 1) h = upsample("decoder.up_blocks." + std::to_string(i) + ".upsamplers.0", h);
         }
         T4 a = act(h.n, h.h, h.w, h.c);
         groupnorm(h, "decoder.conv_norm_out", 1e-6f, 1, a);
@@ -579,23 +532,23 @@ struct Engine : Builder {
         for (int oi = (int)vorder.size() - 1; oi >= 0; oi--) {
             const int kind = vorder[oi];
             if (kind == 0) {
-                const ResTape& t = vres[ri--];
+                const ResTape& t = vres[ri--]; const int cin = t.x.c, cout = t.cout;
                 // out = sc(x) + conv2(a2) ; a2 = silu(gn2(h1)) ; h1 = conv1(a1) ; a1 = silu(gn1(x))
-                T4 da2 = act(t.x.n, t.x.h, t.x.w, t.cout);
-                conv3_dgrad(dh, t.pre + ".conv2.weight", t.cout, da2);
-                T4 dh1 = act(t.x.n, t.x.h, t.x.w, t.cout);
+                T4 da2 = act(t.x.n, t.x.h, t.x.w, cout);
+                conv3_dgrad(dh, t.pre + ".conv2.weight", cout, da2);
+                T4 dh1 = act(t.x.n, t.x.h, t.x.w, cout);
                 groupnorm_bwd(t.g2, da2.p, nullptr, dh1.p);
-                T4 da1 = act(t.x.n, t.x.h, t.x.w, t.cin);
-                conv3_dgrad(dh1, t.pre + ".conv1.weight", t.cin, da1);
+                T4 da1 = act(t.x.n, t.x.h, t.x.w, cin);
+                conv3_dgrad(dh1, t.pre + ".conv1.weight", cin, da1);
                 // shortcut branch gradient
                 const __half* dsc = dh.p;
-                if (t.shortcut) {
+                if (cin != cout) {
                     Param& ws = params[pindex[t.pre + ".conv_shortcut.weight"]];
-                    T4 d = act(t.x.n, t.x.h, t.x.w, t.cin);
-                    linear(dh.p, t.x.rows(), t.cout, (const __half*)ws.dst2, t.cin, d.p);     // dst2 = W^T [cin][cout]
+                    T4 d = act(t.x.n, t.x.h, t.x.w, cin);
+                    linear(dh.p, t.x.rows(), cout, (const __half*)ws.dst2, cin, d.p);     // dst2 = W^T [cin][cout]
                     dsc = d.p;
                 }
-                T4 dx = act(t.x.n, t.x.h, t.x.w, t.cin);
+                T4 dx = act(t.x.n, t.x.h, t.x.w, cin);
                 groupnorm_bwd(t.g1, da1.p, dsc, dx.p);
                 dh = dx;
             } else if (kind == 1) {
@@ -613,7 +566,7 @@ struct Engine : Builder {
                 });
                 dh = dx;
             } else {
-                const AttnTape& a = vattn; const int C = a.C; const long long M = a.x.rows();
+                const AttnTape& a = vattn; const int C = a.x.c; const long long M = a.x.rows();
                 auto W2 = [&](const std::string& n) { return (const __half*)params[pindex[a.pre + n]].dst2; };   // transposed copies [in][out]
                 // out = x + ao Wo^T + b
                 __half* dao = alloc16(M * C);

@@ -16,6 +16,8 @@ Measured on an H100 80GB HBM3 (sm_90a, 400 W power limit), engine (fp16-storage 
 2.9e-4 .. 1.9e-3 (2.1e-4 .. 1.3e-3), CFG noise_pred 1.08e-2 (9.0e-3), SDS grad 4.7e-3 (3.9e-3), latents 3.8e-4 (3.3e-4), d pred_rgb
 3.3e-3 (2.7e-3): the engine sits within 1.5x of the fp16-storage floor everywhere; the 1e-3 figure of north_star is not reachable by ANY fp16-activation execution of this network."""
 import importlib
+import json
+import os
 import time
 
 import pytest
@@ -24,6 +26,7 @@ import torch
 from oracle import sd_ref
 
 pytestmark = pytest.mark.gpu
+REGISTRY = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "sd20_registry.json")
 
 
 def _rel(a, b):
@@ -136,3 +139,14 @@ def test_full_size_vae_encode_and_input_gradient(full):
     # the engine also stores the BACKWARD activations in fp16, which the hooked oracle does not emulate: allow 4x
     assert e <= max(4 * e16, 1e-3)
     assert torch.isfinite(r_cu.grad).all()
+
+
+def test_registry_order_is_pinned(full):
+    """StableDiffusion.__init__ draws the seeded stand-in weights in registry order, so the SD-2.0 registry keeps its names and
+    shapes in the recorded order (tests/golden/make_golden_sd_registry.py); it does not depend on which state dicts were loaded"""
+    sdm, g, unet, vae = full
+    with open(REGISTRY) as f:
+        ref = json.load(f)
+    assert len(g.engine.names) == len(ref) == 936
+    assert g.engine.names == [n for n, _ in ref]
+    assert g.engine.shapes == [tuple(s) for _, s in ref]
