@@ -454,7 +454,8 @@ typedef struct {
     int ctx_len;              /* 77 text tokens */
     int groups;               /* 32 */
     int latent_hw;            /* 64 (nerf/sd.py:124 always feeds 512x512 -> 64x64 latents) */
-    int batch;                /* 2 = [uncond, text] (nerf/sd.py:143) */
+    int batch;                /* 2G: [uncond_0..uncond_{G-1}, text_0..text_{G-1}] for G views at one timestep (nerf/sd.py:143 is G = 1); the
+                                 sampler (mi3d_sd_sample) is planned at batch 2 only */
     int proj_conv;            /* transformer proj_in / proj_out: 0 = Linear [C, C] (SD-2.x, use_linear_projection), 1 = 1x1 Conv2d
                                  [C, C, 1, 1] (SD-1.x); the same GEMM either way, only the registered parameter shape differs */
 } mi3d_unet_cfg;
@@ -467,6 +468,7 @@ typedef struct {
     int groups;               /* 32 */
     int image_hw;             /* 512 */
     int decoder;              /* != 0: also plan the decoder (mi3d_sd_decode; the denoise side branch of nerf/sd.py:153-159) */
+    int batch;                /* images per encode / encode backward (G); 0 or 1 = one image.  The decoder always takes one image. */
 } mi3d_vae_cfg;
 
 /* weights + activations + tapes; nothing else is ever allocated */
@@ -476,19 +478,22 @@ mi3d_engine_t mi3d_sd_create(const mi3d_unet_cfg* unet, const mi3d_vae_cfg* vae,
  * prefixed as in AutoencoderKL: "encoder....", "quant_conv....").  Graph replay covers the static launch lists (U-Net,
  * VAE encode, VAE input-gradient, VAE decode, sampling step).  Debug taps: "unet.mid", "vae.grad_in", ... */
 
-/* replaces nerf/sd.py:124 (F.interpolate to 512) + :133,212-220 (encode_imgs: vae.encode(2x-1).latent_dist.sample()*0.18215)
- * pred_rgb [1,3,H,W] fp32 in [0,1]; eps_posterior, latents [1,4,h,w] fp32 (h = image_hw/8). */
+/* replaces nerf/sd.py:124 (F.interpolate to 512) + :133,212-220 (encode_imgs: vae.encode(2x-1).latent_dist.sample()*0.18215), for the
+ * G = mi3d_vae_cfg.batch images the engine is planned for, each on its own (convs, GroupNorm and the mid-block attention are per image).
+ * pred_rgb [G,3,H,W] fp32 in [0,1]; eps_posterior, latents [G,4,h,w] fp32 (h = image_hw/8). */
 int mi3d_sd_encode(mi3d_engine_t h, const float* pred_rgb, int H, int W, const float* eps_posterior, float* latents, mi3d_stream_t stream);
-/* the autograd half of latents.backward(gradient=grad) (nerf/sd.py:171): d latents -> d pred_rgb, weights frozen */
+/* the autograd half of latents.backward(gradient=grad) (nerf/sd.py:171): d latents -> d pred_rgb, weights frozen; [G,...] buffers as above */
 int mi3d_sd_encode_backward(mi3d_engine_t h, const float* grad_latents, const float* eps_posterior, int H, int W, float* grad_pred_rgb,
                             mi3d_stream_t stream);
 /* replaces nerf/sd.py:138-170: scheduler.add_noise, unet([x,x], t, text_embeddings).sample, CFG (text + gs*(text-uncond)),
- * w = 1 - alphas[t], grad = nan_to_num(w*(noise_pred - noise)).  t: DEVICE int64 scalar; alphas_cumprod: DEVICE fp32 [1000];
- * text_embeddings fp32 [2,77,cross_dim] (uncond first); noise_pred / grad (nullable) fp32 [1,4,h,w]. */
+ * w = 1 - alphas[t], grad = nan_to_num(w*(noise_pred - noise)), for G = mi3d_unet_cfg.batch / 2 views at ONE shared timestep.
+ * t: DEVICE int64 scalar; alphas_cumprod: DEVICE fp32 [1000]; latents / noise fp32 [G,4,h,w]; text_embeddings fp32 [2G,77,cross_dim]
+ * laid out [uncond_0..uncond_{G-1}, cond_0..cond_{G-1}] (view v's CFG pairs U-Net rows v and G+v); noise_pred / grad (nullable)
+ * fp32 [G,4,h,w]. */
 int mi3d_sd_unet_sds(mi3d_engine_t h, const float* latents, const float* noise, const long long* t, const float* alphas_cumprod,
                      const float* text_embeddings, float guidance_scale, float* noise_pred, float* grad, mi3d_stream_t stream);
 /* The "denoise" side branch of train_step (nerf/sd.py:153-159), taken on non-large views when t <= 0.4 T:
- * replaces scheduler.step (DDIM, eta 0, t -> t-1; fp32 [1,4,h,w], n = 4*h*w elements) and decode_latents (nerf/sd.py:201-210:
+ * replaces scheduler.step (DDIM, eta 0, t -> t-1; fp32 [G,4,h,w], n = 4*h*w*G elements, element-wise) and decode_latents (nerf/sd.py:201-210:
  * vae.decode(latents / 0.18215) -> (x/2 + 0.5).clamp(0,1); imgs fp32 [1,3,image_hw,image_hw]).  Forward only, like the reference. */
 int mi3d_sd_ddim_step(const float* noise_pred, const float* latents_noisy, const long long* t, const float* alphas_cumprod,
                       float* prev_sample, int n, mi3d_stream_t stream);

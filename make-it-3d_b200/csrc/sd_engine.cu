@@ -82,16 +82,20 @@ struct Engine : Builder {
         if (v && !u) ucfg.groups = v->groups;
     }
     std::vector<Op> unet_ops, enc_ops, enc_bwd_ops;
-    // GroupNorm statistics of one op list live in one pool, cleared by a single memset at the head of the list
-    uint8_t* pool = nullptr; size_t pool_used = 0; static constexpr size_t kPoolBytes = 256 * 1024;
+    // GroupNorm statistics of one op list live in one pool, cleared by a single memset at the head of the list.  Each GroupNorm takes
+    // 2 * n * groups doubles, so the pool grows with the batch: a measuring pass of build() records what each list needs, and the pool is
+    // that size, at least kPoolBytes (so a batch-2 U-Net / one-image VAE keeps the buffer offsets it always had).
+    uint8_t* pool = nullptr; size_t pool_used = 0, pool_cap = 0; static constexpr size_t kPoolBytes = 256 * 1024;
+    bool measuring = false; std::map<const std::vector<Op>*, size_t> pool_need;
     void begin_list(std::vector<Op>* l) {
-        cur = l; pool = (uint8_t*)alloc(kPoolBytes); pool_used = 0;
-        uint8_t* pp = pool;
-        push([pp](cudaStream_t st) { return (int)cudaMemsetAsync(pp, 0, kPoolBytes, st); });
+        cur = l; pool_cap = std::max(kPoolBytes, pool_need[l]); pool = (uint8_t*)alloc(pool_cap); pool_used = 0;
+        uint8_t* pp = pool; const size_t bytes = pool_cap;
+        push([pp, bytes](cudaStream_t st) { return (int)cudaMemsetAsync(pp, 0, bytes, st); });
     }
     double* pool_stats(size_t n_doubles) {
         const size_t b = n_doubles * sizeof(double);
-        if (pool_used + b > kPoolBytes) { err = MI3D_ERR_ARG; return (double*)pool; }
+        if (measuring) pool_need[cur] = pool_used + b;
+        else if (pool_used + b > pool_cap) { err = MI3D_ERR_ARG; return (double*)pool; }
         double* p = (double*)(pool + pool_used); pool_used += b; return p;
     }
     // per-ResBlock time-embedding projections of the whole U-Net, evaluated by one grouped launch right after the embedding MLP
@@ -389,10 +393,11 @@ struct Engine : Builder {
     std::vector<ResTape> vres; std::vector<DownTape> vdown; AttnTape vattn; GN vgn_out; T4 v_a_out, v_h_last, v_conv_in_out;
     std::vector<int> vorder;   // 0 = res, 1 = down, 2 = attn ; forward order for the reverse walk
 
-    // the VAE's Attention: one head over all pixels (tape: weights with a transposed copy, *tape filled)
+    // the VAE's Attention: one head over the pixels of each image (batched over x.n images; P is [n][pix][pix]) (tape: weights with a
+    // transposed copy, *tape filled)
     T4 vae_attention(const std::string& pre, const T4& x, AttnTape* tape) {
         const PKind kind = tape ? PK_LINEAR_BOTH : PK_LINEAR;
-        const long long M = x.rows(); const int C = x.c;
+        const long long M = x.rows(); const int C = x.c, nb = x.n, pix = x.h * x.w;
         T4 n = act(x.n, x.h, x.w, C);
         GN g = groupnorm(x, pre + ".group_norm", 1e-6f, 0, n);
         __half *q = alloc16(M * C), *k = alloc16(M * C), *v = alloc16(M * C), *vT = alloc16(M * C);
@@ -405,18 +410,25 @@ struct Engine : Builder {
         const float* bv = pf(pre + ".to_v.bias", {C});
         const __half* wv = (const __half*)param(pre + ".to_v.weight", {C, C}, kind).dst;
         linear(n.p, M, C, wv, C, v, bv);
-        transpose(v, vT, 1, (int)M, C);
-        __half* P = alloc16((size_t)M * M);
-        { Mat qa{q, C, M, C}; Mat kb{k, C, M, C}; Out oo; oo.p16 = P; oo.ldc = M; Epi e; gemm(qa, kb, (int)M, oo, e); }
-        softmax(P, (size_t)M, (int)M, (int)M, 1.0f / sqrtf((float)C));
+        transpose(v, vT, nb, pix, C);
+        __half* P = alloc16((size_t)M * pix);
+        per_image_gemm(q, C, pix, C, k, C, pix, P, pix, nb);
+        softmax(P, (size_t)M, pix, pix, 1.0f / sqrtf((float)C));
         __half* ao = alloc16(M * C);
-        { Mat pa{P, M, M, (int)M}; Mat vb{vT, M, C, (int)M}; Out oo; oo.p16 = ao; oo.ldc = C; Epi e; gemm(pa, vb, C, oo, e); }
+        per_image_gemm(P, pix, pix, pix, vT, pix, C, ao, C, nb);
         T4 out = act(x.n, x.h, x.w, C);
         const float* bo = pf(pre + ".to_out.0.bias", {C});
         const __half* wo = (const __half*)param(pre + ".to_out.0.weight", {C, C}, kind).dst;
         linear(ao, M, C, wo, C, out.p, bo, x.p);
         if (tape) *tape = AttnTape{pre, x, g, q, k, v, P};
         return out;
+    }
+    // out_i[rows][N] = A_i[rows][K] B_i[N][K]^T for the nb images i: A_i = a + i * rows * K, B_i = b + i * N * K, out_i = o + i * rows * N
+    // (every operand packed per image).  One image is the plain GEMM.
+    void per_image_gemm(const __half* a, long long lda, long long rows, int K, const __half* b, long long ldb, int N, __half* o, long long ldo, int nb) {
+        Mat am{a, lda, rows, K}; Mat bm{b, ldb, N, K}; am.z1 = nb; bm.z1 = nb;
+        Out oo; oo.p16 = o; oo.ldc = ldo; oo.z1 = nb; oo.s_lo = rows * ldo;
+        Epi e; gemm(am, bm, N, oo, e, nb, nb > 1);
     }
 
     // the VAE's mid block: resnet, attention, resnet; taped (the encoder's) in vres / vattn / vorder for build_vae_bwd
@@ -432,9 +444,9 @@ struct Engine : Builder {
     void build_vae() {
         begin_list(&enc_ops);
         const mi3d_vae_cfg& c = vcfg;
-        const int S = c.image_hw, nlev = c.n_levels, L = c.layers_per_block;
-        vae_in = act(1, S, S, 4);          // 3 channels padded to 4 (the 4th is zero)
-        T4 h = act(1, S, S, c.block_out[0]);
+        const int S = c.image_hw, nlev = c.n_levels, L = c.layers_per_block, nb = vae_images();
+        vae_in = act(nb, S, S, 4);         // 3 channels padded to 4 (the 4th is zero)
+        T4 h = act(nb, S, S, c.block_out[0]);
         {
             const float* w = (const float*)param("encoder.conv_in.weight", {c.block_out[0], c.in_ch, 3, 3}, PK_CONV_F32_OHWI).dst;
             const float* b = pf("encoder.conv_in.bias", {c.block_out[0]});
@@ -566,27 +578,27 @@ struct Engine : Builder {
                 });
                 dh = dx;
             } else {
-                const AttnTape& a = vattn; const int C = a.x.c; const long long M = a.x.rows();
+                const AttnTape& a = vattn; const int C = a.x.c, nb = a.x.n, pix = a.x.h * a.x.w; const long long M = a.x.rows();
                 auto W2 = [&](const std::string& n) { return (const __half*)params[pindex[a.pre + n]].dst2; };   // transposed copies [in][out]
                 // out = x + ao Wo^T + b
                 __half* dao = alloc16(M * C);
                 linear(dh.p, M, C, W2(".to_out.0.weight"), C, dao);
-                // dV = P^T dao ; dP = dao V^T
-                __half* PT = alloc16((size_t)M * M); transpose(a.P, PT, 1, (int)M, (int)M);
-                __half* daoT = alloc16(M * C); transpose(dao, daoT, 1, (int)M, C);
+                // per image: dV = P^T dao ; dP = dao V^T
+                __half* PT = alloc16((size_t)M * pix); transpose(a.P, PT, nb, pix, pix);
+                __half* daoT = alloc16(M * C); transpose(dao, daoT, nb, pix, C);
                 __half* dV = alloc16(M * C);
-                { Mat A{PT, M, M, (int)M}; Mat Bm{daoT, M, C, (int)M}; Out oo; oo.p16 = dV; oo.ldc = C; Epi e; gemm(A, Bm, C, oo, e); }
-                __half* dP = alloc16((size_t)M * M);
-                { Mat A{dao, C, M, C}; Mat Bm{a.v, C, M, C}; Out oo; oo.p16 = dP; oo.ldc = M; Epi e; gemm(A, Bm, (int)M, oo, e); }
+                per_image_gemm(PT, pix, pix, pix, daoT, pix, C, dV, C, nb);
+                __half* dP = alloc16((size_t)M * pix);
+                per_image_gemm(dao, C, pix, C, a.v, C, pix, dP, pix, nb);
                 const float scale = 1.0f / sqrtf((float)C);
-                softmax_bwd(a.P, dP, (size_t)M, (int)M, scale);
+                softmax_bwd(a.P, dP, (size_t)M, pix, scale);
                 // dQ = dS K ; dK = dS^T Q
-                __half* kT = alloc16(M * C); transpose(a.k, kT, 1, (int)M, C);
-                __half* qT = alloc16(M * C); transpose(a.q, qT, 1, (int)M, C);
-                __half* dST = alloc16((size_t)M * M); transpose(dP, dST, 1, (int)M, (int)M);
+                __half* kT = alloc16(M * C); transpose(a.k, kT, nb, pix, C);
+                __half* qT = alloc16(M * C); transpose(a.q, qT, nb, pix, C);
+                __half* dST = alloc16((size_t)M * pix); transpose(dP, dST, nb, pix, pix);
                 __half* dQ = alloc16(M * C); __half* dK = alloc16(M * C);
-                { Mat A{dP, M, M, (int)M}; Mat Bm{kT, M, C, (int)M}; Out oo; oo.p16 = dQ; oo.ldc = C; Epi e; gemm(A, Bm, C, oo, e); }
-                { Mat A{dST, M, M, (int)M}; Mat Bm{qT, M, C, (int)M}; Out oo; oo.p16 = dK; oo.ldc = C; Epi e; gemm(A, Bm, C, oo, e); }
+                per_image_gemm(dP, pix, pix, pix, kT, pix, C, dQ, C, nb);
+                per_image_gemm(dST, pix, pix, pix, qT, pix, C, dK, C, nb);
                 // dn = dQ Wq + dK Wk + dV Wv
                 __half* dn1 = alloc16(M * C); __half* dn2 = alloc16(M * C); __half* dn3 = alloc16(M * C);
                 linear(dQ, M, C, W2(".to_q.weight"), C, dn1);
@@ -631,7 +643,18 @@ struct Engine : Builder {
         cur = nullptr;
     }
 
+    // images per encode (mi3d_vae_cfg.batch; 0 means one)
+    int vae_images() const { return std::max(1, vcfg.batch); }
+
+    // a measuring pass (host only) records each list's GroupNorm-statistics need, then the plan is built for real (or sized)
     int build(bool dry_run) {
+        if (vcfg.batch < 0) return MI3D_ERR_ARG;
+        measuring = true; pool_need.clear();
+        const int r = build_pass(true);
+        measuring = false;
+        return r ? r : build_pass(dry_run);
+    }
+    int build_pass(bool dry_run) {
         dry = dry_run; off = 0; err = 0; params.clear(); pindex.clear(); unet_ops.clear(); enc_ops.clear(); enc_bwd_ops.clear(); dec_ops.clear();
         sample_ops.clear(); vres.clear(); vdown.clear(); vorder.clear(); named.clear();
         splitk_elems = (size_t)2048 * 2560; splitk_ws = alloc32(splitk_elems);       // covers M <= 2048 rows x N <= 2560
@@ -732,10 +755,12 @@ __global__ void k_dec_out(const float* __restrict__ o, float* __restrict__ imgs,
     for (int c = 0; c < 3; c++) imgs[(size_t)c * pix + i] = fminf(fmaxf(o[4 * (size_t)i + c] / 2.f + 0.5f, 0.f), 1.f);
 }
 
+// Each API kernel below handles view blockIdx.y of a batch: view v's image, latents, noise and gradients are the v-th [C,h,w] slice.
 // bilinear resize (align_corners=False, F.interpolate semantics) of pred_rgb [3,H,W] fp32 NCHW to S x S, then 2x-1, NHWC fp16 (4 ch)
 __global__ void k_interp_in(const float* __restrict__ rgb, int H, int W, __half* __restrict__ out, int S) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= S * S) return;
+    rgb += (size_t)blockIdx.y * 3 * H * W; out += (size_t)blockIdx.y * S * S * 4;
     const int ox = i % S, oy = i / S;
     const float sx = (float)W / S, sy = (float)H / S;
     float fx = fmaxf((ox + 0.5f) * sx - 0.5f, 0.f), fy = fmaxf((oy + 0.5f) * sy - 0.5f, 0.f);
@@ -756,6 +781,7 @@ __global__ void k_interp_in(const float* __restrict__ rgb, int H, int W, __half*
 __global__ void k_interp_bwd(const float* __restrict__ g /*[S*S][4]*/, int S, float* __restrict__ grad_rgb, int H, int W) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= H * W) return;
+    g += (size_t)blockIdx.y * S * S * 4; grad_rgb += (size_t)blockIdx.y * 3 * H * W;
     const int x = i % W, y = i / W;
     const float sx = (float)W / S, sy = (float)H / S;
     // output pixels whose source footprint can touch (x, y): fx in (x-1, x+1)
@@ -784,6 +810,8 @@ __global__ void k_sample_latents(const float* __restrict__ conv_out /*[pix][8]*/
                                  const float* __restrict__ eps /*[4,h,w]*/, float* __restrict__ latents, int pix) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= pix) return;
+    const size_t v = blockIdx.y;
+    conv_out += v * pix * 8; eps += v * pix * 4; latents += v * pix * 4;
     float m[8];
     #pragma unroll
     for (int o = 0; o < 8; o++) { float a = qb[o]; for (int k = 0; k < 8; k++) a = fmaf(qw[o * 8 + k], conv_out[(size_t)i * 8 + k], a); m[o] = a; }
@@ -798,6 +826,8 @@ __global__ void k_sample_latents_bwd(const float* __restrict__ conv_out, const f
                                      const float* __restrict__ eps, const float* __restrict__ g_lat, float* __restrict__ g_conv_out, int pix) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= pix) return;
+    const size_t v = blockIdx.y;
+    conv_out += v * pix * 8; eps += v * pix * 4; g_lat += v * pix * 4; g_conv_out += v * pix * 8;
     float m[8], gm[8];
     #pragma unroll
     for (int o = 0; o < 8; o++) { float a = qb[o]; for (int k = 0; k < 8; k++) a = fmaf(qw[o * 8 + k], conv_out[(size_t)i * 8 + k], a); m[o] = a; }
@@ -812,17 +842,21 @@ __global__ void k_sample_latents_bwd(const float* __restrict__ conv_out, const f
     #pragma unroll
     for (int k = 0; k < 8; k++) { float a = 0.f; for (int o = 0; o < 8; o++) a = fmaf(qw[o * 8 + k], gm[o], a); g_conv_out[(size_t)i * 8 + k] = a; }
 }
-// DDIM add_noise + duplicate for CFG + NCHW fp32 -> NHWC fp16 : x_in[b][p][c] = sqrt(a_t) z[c][p] + sqrt(1-a_t) eps[c][p]
+// DDIM add_noise + duplicate for CFG + NCHW fp32 -> NHWC fp16 : x_in[b][p][c] = sqrt(a_t) z[c][p] + sqrt(1-a_t) eps[c][p] for the U-Net rows
+// b = v (uncond) and b = G + v (text) of view v
 __global__ void k_add_noise(const float* __restrict__ lat, const float* __restrict__ noise, const float* __restrict__ alphas, const long long* __restrict__ t,
-                            __half* __restrict__ xin, int pix, int B) {
+                            __half* __restrict__ xin, int pix, int G) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= pix) return;
+    const int v = blockIdx.y;
+    lat += (size_t)v * pix * 4; noise += (size_t)v * pix * 4;
     const float a = alphas[t[0]];
     const float sa = sqrtf(a), sb = sqrtf(1.f - a);
     __align__(8) __half o[4];
     #pragma unroll
     for (int c = 0; c < 4; c++) o[c] = __float2half_rn(sa * lat[(size_t)c * pix + i] + sb * noise[(size_t)c * pix + i]);
-    for (int b = 0; b < B; b++) *reinterpret_cast<uint2*>(xin + ((size_t)b * pix + i) * 4) = *reinterpret_cast<const uint2*>(o);
+    *reinterpret_cast<uint2*>(xin + ((size_t)v * pix + i) * 4) = *reinterpret_cast<const uint2*>(o);
+    *reinterpret_cast<uint2*>(xin + ((size_t)(G + v) * pix + i) * 4) = *reinterpret_cast<const uint2*>(o);
 }
 // ctx fp32 [B][L][D] -> fp16 [B][Lpad][D], zero rows beyond L
 __global__ void k_ctx_pad(const float* __restrict__ ctx, __half* __restrict__ out, int B, int L, int Lpad, int D) {
@@ -832,15 +866,21 @@ __global__ void k_ctx_pad(const float* __restrict__ ctx, __half* __restrict__ ou
         out[i] = __float2half_rn(l < L ? ctx[((size_t)b * L + l) * D + d] : 0.f);
     }
 }
-// CFG (sd.py:150-151: text + gs*(text - uncond)), SDS weight w = 1 - alpha_t, grad = nan_to_num(w (eps_hat - eps)); NHWC fp32 in, NCHW fp32 out
-__global__ void k_cfg_sds(const float* __restrict__ unet_out /*[2][pix][4]*/, const float* __restrict__ noise, const float* __restrict__ alphas,
-                          const long long* __restrict__ t, float gs, float* __restrict__ noise_pred, float* __restrict__ grad, int pix) {
+// CFG (sd.py:150-151: text + gs*(text - uncond)), SDS weight w = 1 - alpha_t, grad = nan_to_num(w (eps_hat - eps)); NHWC fp32 in, NCHW fp32 out.
+// View v pairs U-Net rows v (uncond) and G + v (text).
+__global__ void k_cfg_sds(const float* __restrict__ unet_out /*[2G][pix][4]*/, const float* __restrict__ noise, const float* __restrict__ alphas,
+                          const long long* __restrict__ t, float gs, float* __restrict__ noise_pred, float* __restrict__ grad, int pix, int G) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= pix) return;
+    const size_t v = blockIdx.y;
+    const float* un_p = unet_out + v * pix * 4; const float* tx_p = unet_out + (G + v) * pix * 4;
+    noise += v * pix * 4;
+    if (noise_pred) noise_pred += v * pix * 4;
+    if (grad) grad += v * pix * 4;
     const float w = 1.f - alphas[t[0]];
     #pragma unroll
     for (int c = 0; c < 4; c++) {
-        const float un = unet_out[(size_t)i * 4 + c], tx = unet_out[((size_t)pix + i) * 4 + c];
+        const float un = un_p[(size_t)i * 4 + c], tx = tx_p[(size_t)i * 4 + c];
         const float np = tx + gs * (tx - un);
         if (noise_pred) noise_pred[(size_t)c * pix + i] = np;
         float g = w * (np - noise[(size_t)c * pix + i]);
@@ -883,30 +923,31 @@ int mi3d_sd_profile_dump(mi3d_engine_t h, int enable, float* gemm_ms, int* launc
     return MI3D_OK;
 }
 
-// nerf/sd.py:124,133,212-220 : pred_rgb [1,3,H,W] fp32 -> bilinear to image_hw -> VAE encode -> posterior sample * 0.18215
+// nerf/sd.py:124,133,212-220 : pred_rgb [G,3,H,W] fp32 -> bilinear to image_hw -> VAE encode -> posterior sample * 0.18215, G = the planned
+// images per encode
 int mi3d_sd_encode(mi3d_engine_t h, const float* pred_rgb, int H, int W, const float* eps_posterior, float* latents, mi3d_stream_t stream) {
     sd::Engine* ep = plan::engine_of<sd::Engine>(h);
     if (!ep || ep->vcfg.n_levels == 0) return MI3D_ERR_ARG;
     cudaStream_t st = (cudaStream_t)stream; sd::Engine& e = *ep;
-    const int S = e.vcfg.image_hw;
-    sd::k_interp_in<<<(S * S + 255) / 256, 256, 0, st>>>(pred_rgb, H, W, e.vae_in.p, S);
+    const int S = e.vcfg.image_hw, G = e.vae_images();
+    sd::k_interp_in<<<dim3((S * S + 255) / 256, G), 256, 0, st>>>(pred_rgb, H, W, e.vae_in.p, S);
     int r = e.run(e.enc_ops, st); if (r) return r;
-    const int pix = (int)e.v_h_last.rows();
+    const int pix = (int)e.v_h_last.rows() / G;
     const float* qw = (const float*)e.params[e.pindex["quant_conv.weight"]].dst; const float* qb = (const float*)e.params[e.pindex["quant_conv.bias"]].dst;
-    sd::k_sample_latents<<<(pix + 127) / 128, 128, 0, st>>>(e.vae_moments, qw, qb, eps_posterior, latents, pix);
+    sd::k_sample_latents<<<dim3((pix + 127) / 128, G), 128, 0, st>>>(e.vae_moments, qw, qb, eps_posterior, latents, pix);
     return (int)cudaGetLastError();
 }
 
-// backward of mi3d_sd_encode w.r.t. pred_rgb (weights frozen): grad_pred_rgb [1,3,H,W] fp32 (overwritten)
+// backward of mi3d_sd_encode w.r.t. pred_rgb (weights frozen): grad_pred_rgb [G,3,H,W] fp32 (overwritten)
 int mi3d_sd_encode_backward(mi3d_engine_t h, const float* grad_latents, const float* eps_posterior, int H, int W, float* grad_pred_rgb, mi3d_stream_t stream) {
     sd::Engine* ep = plan::engine_of<sd::Engine>(h);
     if (!ep || ep->vcfg.n_levels == 0) return MI3D_ERR_ARG;
     cudaStream_t st = (cudaStream_t)stream; sd::Engine& e = *ep;
-    const int pix = (int)e.v_h_last.rows(), S = e.vcfg.image_hw;
+    const int G = e.vae_images(), pix = (int)e.v_h_last.rows() / G, S = e.vcfg.image_hw;
     const float* qw = (const float*)e.params[e.pindex["quant_conv.weight"]].dst; const float* qb = (const float*)e.params[e.pindex["quant_conv.bias"]].dst;
-    sd::k_sample_latents_bwd<<<(pix + 127) / 128, 128, 0, st>>>(e.vae_moments, qw, qb, eps_posterior, grad_latents, e.vae_gmoments, pix);
+    sd::k_sample_latents_bwd<<<dim3((pix + 127) / 128, G), 128, 0, st>>>(e.vae_moments, qw, qb, eps_posterior, grad_latents, e.vae_gmoments, pix);
     int r = e.run(e.enc_bwd_ops, st); if (r) return r;
-    sd::k_interp_bwd<<<(H * W + 127) / 128, 128, 0, st>>>(e.vae_grad_img, S, grad_pred_rgb, H, W);
+    sd::k_interp_bwd<<<dim3((H * W + 127) / 128, G), 128, 0, st>>>(e.vae_grad_img, S, grad_pred_rgb, H, W);
     return (int)cudaGetLastError();
 }
 
@@ -931,19 +972,21 @@ int mi3d_sd_decode(mi3d_engine_t h, const float* latents, float* imgs, mi3d_stre
     return (int)cudaGetLastError();
 }
 
-// nerf/sd.py:138-171 : add_noise -> U-Net on [uncond, text] -> CFG -> SDS gradient.  t: device int64 scalar; alphas: device [1000] fp32
+// nerf/sd.py:138-171 : add_noise -> U-Net on [uncond_0..uncond_{G-1}, text_0..text_{G-1}] -> CFG -> SDS gradient, G = batch / 2 views at one
+// timestep.  t: device int64 scalar; alphas: device [1000] fp32
 int mi3d_sd_unet_sds(mi3d_engine_t h, const float* latents, const float* noise, const long long* t, const float* alphas_cumprod,
                      const float* text_embeddings, float guidance_scale, float* noise_pred, float* grad, mi3d_stream_t stream) {
     sd::Engine* ep = plan::engine_of<sd::Engine>(h);
     if (!ep || ep->ucfg.n_levels == 0) return MI3D_ERR_ARG;
     cudaStream_t st = (cudaStream_t)stream; sd::Engine& e = *ep;
     const int pix = e.ucfg.latent_hw * e.ucfg.latent_hw, B = e.ucfg.batch;
-    if (B != 2 || e.ucfg.in_ch != 4) return MI3D_ERR_ARG;
+    if (B < 2 || B % 2 || e.ucfg.in_ch != 4) return MI3D_ERR_ARG;
+    const int G = B / 2;
     MI3D_CHECK(cudaMemcpyAsync(e.t_dev, t, sizeof(long long), cudaMemcpyDeviceToDevice, st));
-    sd::k_add_noise<<<(pix + 127) / 128, 128, 0, st>>>(latents, noise, alphas_cumprod, e.t_dev, e.unet_in.p, pix, B);
+    sd::k_add_noise<<<dim3((pix + 127) / 128, G), 128, 0, st>>>(latents, noise, alphas_cumprod, e.t_dev, e.unet_in.p, pix, G);
     sd::k_ctx_pad<<<sd::Engine::blocks_for((size_t)B * e.ctx_pad * e.ucfg.cross_dim), 256, 0, st>>>(text_embeddings, e.ctx16, B, e.ucfg.ctx_len, e.ctx_pad, e.ucfg.cross_dim);
     int r = e.run(e.unet_ops, st); if (r) return r;
-    sd::k_cfg_sds<<<(pix + 127) / 128, 128, 0, st>>>(e.unet_out, noise, alphas_cumprod, e.t_dev, guidance_scale, noise_pred, grad, pix);
+    sd::k_cfg_sds<<<dim3((pix + 127) / 128, G), 128, 0, st>>>(e.unet_out, noise, alphas_cumprod, e.t_dev, guidance_scale, noise_pred, grad, pix, G);
     return (int)cudaGetLastError();
 }
 

@@ -8,8 +8,13 @@ nerf/utils.py:461-574, :947-1027) on libmi3d.so.
   gradient enters as `StableDiffusion.train_step(defer=True)`'s surrogate instead of a second walk of the render graph), then one
   `Adan.step()` or `Adam.step()` (`--optim adan` / `adam|adamw`) with the Trainer's `clip_grad_norm(10)` folded in.  It returns
   the loss terms as device scalars and never synchronises the host.
-* `train_step(trainer, data)` / `train_one_epoch(trainer, loader)`: drop-ins for the two Trainer methods.  Swap them together:
-  `train_step` already runs the backward and the update, so the reference's `train_one_epoch` must not run them again.
+* `CoarseStep.step_views(datas, global_step, ...)`: one iteration over G (<= 8) novel views: one multi-view render, the loss kernel per
+  view, one batched guidance call (`StableDiffusion.train_step` on [G,3,H,W], U-Net at batch 2G), one backward, one optimizer step.
+* `train_step(trainer, data)` / `train_one_epoch(trainer, loader, views_per_step=1)`: drop-ins for the two Trainer methods.  Swap them
+  together: `train_step` already runs the backward and the update, so the reference's `train_one_epoch` must not run them again.
+  `views_per_step` G > 1 groups consecutive novel-view items up to G per `step_views`; front items still run alone.  Memory stays
+  bounded by G: StableDiffusion keeps one multi-view engine, at G, and a group with another number of guided views (cut short by a
+  front item, the end of the epoch or diff_iters) runs its guidance view by view on the single-view engine.
 
 What the iteration computes is the reference's: the render at data's H x W; bilinear upsampling (align_corners=True) of the image and
 depth to 512^2; the gt composite on a random background; opacity (x10 on large views), entropy (x1 before diff_iters, x10 after),
@@ -23,6 +28,16 @@ Differences, by design:
 * `train_one_epoch` accumulates the loss on the device and reads it once per epoch (the reference reads it every step), and prints
   nothing per step;
 * `--fp16`, multi-GPU, CPU tensors and reference images other than 512^2 are refused with `Mi3dError`.
+
+Several views per iteration (`step_views`, `views_per_step` G > 1).  View v of a group started at global_step counts as step
+global_step + 1 + v for every per-step rule (opacity x10 on large views, entropy / orientation x1 or x10 around diff_iters, the guidance
+skipped before diff_iters, text_z[1] / tokens[1] on large views).  The iteration's loss and gradient are the sum of the G single-view
+iterations' (the definition SURVEY 8e uses for G ranks), followed by ONE optimizer step.  Where it departs from G reference iterations:
+* one shading draw per group, at the first view's step (each view keeps the reference's marginal distribution, but the views of a
+  group share it);
+* one timestep t shared by the group's guidance;
+* one optimizer step (and one gradient clip) instead of G;
+* the density grid is refreshed at most once per group, when the group crosses a multiple of update_extra_interval.
 """
 import ctypes as C
 import os
@@ -141,11 +156,15 @@ class CoarseStep:
         self.mask = (depth_mask.reshape(REF_HW, REF_HW) == 0).to(torch.uint8).contiguous()      # ~depth_mask (utils.py:556)
         self.text_z, self.tokens = text_z, tokens.contiguous()
         self.last = None
+        # step_views: the number of guided views whose guidance runs as one batch (the size StableDiffusion keeps its one multi-view
+        # engine at; train_one_epoch sets views_per_step); other sizes run view by view.  None: every size is batched.
+        self.guidance_views = None
 
-    def step(self, data, global_step, *, shading=None, bg_color=None, t=None, noise=None, eps_posterior=None, noises=None, light_d=None):
+    def step(self, data, global_step, *, shading=None, bg_color=None, t=None, noise=None, eps_posterior=None, noises=None, light_d=None,
+             step_seed=None):
         """one iteration on the loader batch `data` (rays_o, rays_d, depth_scale, H, W, is_front, is_large) at global_step.  The
         keyword arguments inject the random draws (shading name, background [3], guidance t / noise / eps_posterior, march jitter
-        noises [N], light direction [3]).  Returns {'loss', 'opacity', 'entropy', 'orient', 'smooth', and 'l1', 'depth' (front) or
+        noises [N], light direction [3]; step_seed keys the smoothness perturbation by sample position, as in step_views).  Returns {'loss', 'opacity', 'entropy', 'orient', 'smooth', and 'l1', 'depth' (front) or
         'clip', 'guidance'} as device scalars (l1 = lambda_img L1, depth = lambda_depth (1 - pearson), clip = lambda_clip (img + text),
         guidance = the denoise branch's CLIP value, 0 otherwise).  `last` keeps pred512, gt512, the depth, weights_sum and the
         denoised image of this iteration for the PNG dumps."""
@@ -167,6 +186,8 @@ class CoarseStep:
         kw = dict(vars(opt))
         kw.update(depth_scale=data['depth_scale'], bg_color=bg_color, staged=False, perturb=True, ambient_ratio=ambient_ratio,
                   shading=shading, force_all_rays=True, light_d=light_d, noises=noises)
+        if step_seed is not None:
+            kw.update(step_seed=step_seed)
         out = self.model.render(rays_o, rays_d, **kw)
         terms, pred512, gt512 = coarse_losses(out['image'], out['depth'], out['weights_sum'], H, W, self.ref, bg_color, self.prior,
                                               self.mask, is_front)
@@ -216,6 +237,113 @@ class CoarseStep:
                          weights_sum=out['weights_sum'].detach().reshape(1, 1, H, W), denoised=de_imgs)
         return res
 
+    def step_views(self, datas, global_step, *, shading=None, bg_color=None, t=None, noise=None, eps_posterior=None, noises=None,
+                   light_d=None, step_seed=None):
+        """one iteration over the G novel-view loader batches `datas` (same H x W, none is_front); view v counts as step
+        global_step + 1 + v (see the module docstring).  Injectable draws as in `step`, batched: bg_color [G,3], light_d [G,3], noises
+        [G*H*W], noise / eps_posterior [G,4,h,w]; one shading and one t for the group.  Returns the same keys as `step`, each the sum
+        over the views; `last_views` keeps each view's `last` dict (`last` is the final view's).  G = 1 is `step`."""
+        G = len(datas)
+        if G == 1:
+            pick = lambda x: x[0] if x is not None else None
+            return self.step(datas[0], global_step + 1, shading=shading, bg_color=pick(bg_color), t=t, noise=noise, eps_posterior=eps_posterior,
+                             noises=noises, light_d=pick(light_d), step_seed=step_seed)
+        opt, gd = self.opt, self.guidance
+        H, W = int(datas[0]['H']), int(datas[0]['W'])
+        if not 1 <= G <= L.MAX_VIEWS or any(bool(d['is_front']) or (int(d['H']), int(d['W'])) != (H, W) for d in datas):
+            raise L.Mi3dError(f"step_views takes 1..{L.MAX_VIEWS} novel (not is_front) views of one size; got {G}")
+        steps = [global_step + 1 + v for v in range(G)]
+        large = [bool(d['is_large']) for d in datas]
+        if shading is None:
+            shading, ambient_ratio = pick_shading(steps[0], False, opt.albedo_iters)
+        else:
+            ambient_ratio = 1.0 if shading == 'albedo' else 0.1
+        rays_o = torch.cat([d['rays_o'].reshape(1, H * W, 3) for d in datas])
+        rays_d = torch.cat([d['rays_d'].reshape(1, H * W, 3) for d in datas])
+        depth_scale = torch.cat([d['depth_scale'].reshape(1, H * W) for d in datas])
+        L.require_cuda(rays_o, rays_d)
+        dev = rays_o.device
+        self.optimizer.zero_grad()
+        if bg_color is None:
+            bg_color = torch.rand(G, 3, device=dev)
+        if light_d is None:
+            light_d = safe_normalize(rays_o[:, 0] + torch.randn(G, 3, device=dev))
+        kw = dict(vars(opt))
+        kw.update(depth_scale=depth_scale, bg_color=bg_color, staged=False, perturb=True, ambient_ratio=ambient_ratio, shading=shading,
+                  force_all_rays=True, light_d=light_d, noises=noises)
+        if step_seed is not None:
+            kw.update(step_seed=step_seed)
+        out = self.model.render(rays_o, rays_d, **kw)
+        per_view = [coarse_losses(out['image'][v], out['depth'][v], out['weights_sum'][v], H, W, self.ref, bg_color[v], self.prior, self.mask, False)
+                    for v in range(G)]
+        zero = out['image'].new_zeros(())
+        # guidance: one batched call over the views at or past diff_iters
+        gv = [v for v in range(G) if steps[v] >= opt.diff_iters]
+        surrogate, gval, de_imgs = None, zero, [None] * G
+        if gv:
+            if t is None:
+                t = int(torch.randint(gd.min_step, gd.max_step + 1, [1]).item())      # train_step's draw, CPU generator: no sync
+            # views picked by slices (a list index would copy the index to the device and synchronise)
+            sub = lambda x: (x if len(gv) == G else torch.cat([x[v:v + 1] for v in gv])) if x is not None else None
+            pred_rgb = sub(out['image']).reshape(len(gv), H, W, 3).permute(0, 3, 1, 2)
+            ks = [1 if large[v] else 0 for v in gv]
+            gkw = dict(ref_rgb=torch.cat([per_view[v][2] for v in gv]), noise=sub(noise), ref_text=torch.cat([self.tokens[k:k + 1] for k in ks]),
+                       clip_model=self.clip, guidance_scale=opt.guidance_scale, t=t, eps_posterior=sub(eps_posterior))
+            if len(gv) > 1 and self.guidance_views in (None, len(gv)):
+                te = self.text_z[ks[0]] if len(set(ks)) == 1 else torch.cat([self.text_z[k][:1] for k in ks] + [self.text_z[k][1:] for k in ks])
+                surrogate, imgs = gd.train_step(te, pred_rgb, islarge=[large[v] for v in gv], defer=True, **gkw)
+                g = gd.last['denoise']
+                gval = g if torch.is_tensor(g) else zero + float(g)
+                for i, v in enumerate(gv):
+                    de_imgs[v] = imgs[i]
+            else:
+                # view by view on the constructor's engine, exactly as `step` calls it (one guided view, or a group size the multi-view
+                # engine is not kept at: planning one per size would hold a 10-34 GiB engine for every size met)
+                for i, v in enumerate(gv):
+                    one = dict(gkw, ref_rgb=gkw['ref_rgb'][i:i + 1], ref_text=gkw['ref_text'][i:i + 1],
+                               noise=gkw['noise'][i:i + 1] if noise is not None else None,
+                               eps_posterior=gkw['eps_posterior'][i:i + 1] if eps_posterior is not None else None)
+                    if not large[v] and t / gd.num_train_timesteps <= 0.4:
+                        with torch.no_grad():
+                            g, de_imgs[v] = gd.train_step(self.text_z[ks[i]], pred_rgb[i:i + 1].detach(), islarge=False, **one)
+                        gval = gval + (g if torch.is_tensor(g) else float(g))
+                    else:
+                        sv, _ = gd.train_step(self.text_z[ks[i]], pred_rgb[i:i + 1], islarge=large[v], defer=True, **one)
+                        surrogate = sv if surrogate is None else surrogate + sv
+        loss, res, clip_surrogate = gval, dict(clip=zero, opacity=zero, entropy=zero, orient=zero, smooth=zero), zero
+        self.last_views = []
+        for v in range(G):
+            terms, pred512, gt512 = per_view[v]
+            before = steps[v] < opt.diff_iters
+            if opt.lambda_opacity > 0:
+                loss = loss + (opt.lambda_opacity * terms[0] * 10 if large[v] else opt.lambda_opacity * terms[0])
+            if opt.lambda_entropy > 0:
+                loss = loss + (opt.lambda_entropy * terms[1] if before else opt.lambda_entropy * terms[1] * 10)
+            orient = out['loss_orient'][v] if 'loss_orient' in out else zero
+            smooth = out['loss_smooth'][v] if 'loss_smooth' in out else zero
+            if opt.lambda_orient > 0 and 'loss_orient' in out:
+                loss = loss + opt.lambda_orient * orient
+                loss = loss + (opt.lambda_orient * orient if before else opt.lambda_orient * orient * 10)
+            if opt.lambda_smooth > 0 and 'loss_smooth' in out:
+                loss = loss + opt.lambda_smooth * smooth
+            k = 1 if large[v] else 0
+            img_l, text_l = self.clip.losses(pred512, gt512, self.tokens[k:k + 1])
+            loss_ref = opt.lambda_clip * img_l + opt.lambda_clip * text_l
+            # the CLIP backward runs now, while this view's tape is the CLIP engine's: in the one backward below the G views' image
+            # towers would each have to be run forward again first.  Its gradient joins as a surrogate, like the SDS gradient.
+            (g_pred,) = torch.autograd.grad(loss_ref, pred512)
+            clip_surrogate = clip_surrogate + (g_pred * pred512).sum()
+            loss = loss + loss_ref.detach()
+            for name, val in (('clip', loss_ref), ('opacity', terms[0]), ('entropy', terms[1]), ('orient', orient), ('smooth', smooth)):
+                res[name] = res[name] + val.detach()
+            self.last_views.append(dict(pred512=pred512.detach(), gt512=gt512, depth=out['depth'][v].detach(), H=H, W=W,
+                                        weights_sum=out['weights_sum'][v].detach().reshape(1, 1, H, W), denoised=de_imgs[v]))
+        (loss + clip_surrogate if surrogate is None else loss + clip_surrogate + surrogate).backward()
+        self.optimizer.step()
+        res.update(loss=loss.detach(), guidance=gval.detach())
+        self.last = self.last_views[-1]
+        return res
+
 
 def _coarse_step(trainer):
     cs = getattr(trainer, "_coarse_step", None)
@@ -232,9 +360,10 @@ def _coarse_step(trainer):
     return cs
 
 
-def _save_pngs(trainer, cs):
-    """the reference's dumps at global_step % 100 == 0 or == 1 (utils.py:565-571); save_image clamps to [0, 1]"""
-    last, step, path = cs.last, trainer.global_step, trainer.img_path
+def _save_pngs(trainer, cs, last=None, step=None):
+    """the reference's dumps at global_step % 100 == 0 or == 1 (utils.py:565-571); save_image clamps to [0, 1].  last / step: a view
+    of a multi-view iteration and its step number (default: cs.last at trainer.global_step)"""
+    last, step, path = last or cs.last, trainer.global_step if step is None else step, trainer.img_path
     os.makedirs(path, exist_ok=True)
     with torch.no_grad():
         # the upsampled depth only feeds this dump (the loss kernel keeps its own copy), once per 100 steps
@@ -256,24 +385,62 @@ def train_step(trainer, data):
     return cs.last['pred512'], cs.last['weights_sum'], res['loss']
 
 
-def train_one_epoch(trainer, loader):
+def _dump_due(step):
+    return step % 100 == 0 or step == 1
+
+
+def train_one_epoch(trainer, loader, views_per_step=1):
     """drop-in for Trainer.train_one_epoch (nerf/utils.py:947-1027): density-grid update every update_extra_interval steps, one
-    coarse iteration per batch, the scheduler step; the loss is summed on the device and read once, for stats["loss"] and the log"""
+    coarse iteration per batch, the scheduler step; the loss is summed on the device and read once, for stats["loss"] and the log.
+    views_per_step G > 1: consecutive novel-view batches run G at a time through `CoarseStep.step_views` (a shorter group where a front
+    view or the end of the epoch cuts it), front views alone through `step`; global_step, the scheduler and the density-grid refresh
+    advance by views, so the step numbers and schedules are those of the one-view loop."""
     if getattr(trainer, "world_size", 1) > 1:
         raise L.Mi3dError("the coarse step is single-GPU (multi-GPU coarse training is not built)")
+    G = int(views_per_step)
+    if not 1 <= G <= L.MAX_VIEWS:
+        raise L.Mi3dError(f"views_per_step must be in 1..{L.MAX_VIEWS}; got {views_per_step}")
+    if G > 1:
+        _coarse_step(trainer).guidance_views = G
     trainer.log(f"==> Start Training {trainer.workspace} Epoch {trainer.epoch}, lr={trainer.optimizer.param_groups[0]['lr']:.6f} ...")
     trainer.model.train()
     trainer.local_step = 0
     total = None
-    for data in loader:
-        if trainer.model.cuda_ray and trainer.global_step % trainer.opt.update_extra_interval == 0:
+
+    def run(group):
+        nonlocal total
+        n, start = len(group), trainer.global_step
+        if trainer.model.cuda_ray and any((start + v) % trainer.opt.update_extra_interval == 0 for v in range(n)):
             trainer.model.update_extra_state()
-        trainer.local_step += 1
-        trainer.global_step += 1
-        _, _, loss = train_step(trainer, data)
+        trainer.local_step += n
+        trainer.global_step += n
+        if n == 1:
+            _, _, loss = train_step(trainer, group[0])
+        else:
+            cs = _coarse_step(trainer)
+            loss = cs.step_views(group, start)['loss']
+            due = [v for v in range(n) if _dump_due(start + 1 + v)]
+            if due:
+                _save_pngs(trainer, cs, cs.last_views[due[0]], start + 1 + due[0])
         total = loss if total is None else total + loss
         if trainer.scheduler_update_every_step:
-            trainer.lr_scheduler.step()
+            for _ in range(n):
+                trainer.lr_scheduler.step()
+
+    group = []
+    for data in loader:
+        if G > 1 and not data['is_front']:
+            group.append(data)
+            if len(group) == G:
+                run(group)
+                group = []
+            continue
+        if group:
+            run(group)
+            group = []
+        run([data])
+    if group:
+        run(group)
     if getattr(trainer, "ema", None) is not None:
         trainer.ema.update()
     average_loss = float(total) / trainer.local_step if trainer.local_step else 0.0

@@ -65,8 +65,12 @@ class NeRFRenderer(nn.Module):
         key = (N, max_steps, str(device), n_views)
         ws = self._workspaces.get(key)
         if ws is None:
+            # keep one workspace per shape, two shapes at most: a training loop alternates single views (front views) with one
+            # multi-view batch size (coarse.train_one_epoch's views_per_step), and re-carving on every switch costs a large allocation
             ws = field_ops.RenderWorkspace(N, max_steps, device, max_samples=getattr(self.opt, "max_samples", None), n_views=n_views)
-            self._workspaces = {key: ws}        # keep one (shapes are fixed during training)
+        # most recently used first (callers read the current one as list(_workspaces.values())[0]), then at most one other
+        others = [(k, w) for k, w in self._workspaces.items() if k != key][:1]
+        self._workspaces = dict([(key, ws)] + others)
         return ws
 
     def run_cuda(self, rays_o, rays_d, depth_scale=None, bg_color=None, dt_gamma=0, light_d=None, ambient_ratio=1.0,
@@ -79,7 +83,8 @@ class NeRFRenderer(nn.Module):
           cam_table [G,16]              the same, as the ready device table of nerf/utils.py::camera_table (instead of cam_poses)
           ray_parallel                  parallel.RayParallel: this rank renders every world-th pixel of each of `world` views and
                                         returns the complete image of ITS OWN view (rank r owns cam_poses[r]); needs step_seed
-          step_seed                     int shared by all ranks of a step (march jitter, smoothness perturbation, light directions)"""
+          step_seed                     int shared by all ranks of a step (march jitter, smoothness perturbation, light directions)
+        Explicit rays_o / rays_d [G,H*W,3] (depth_scale [G,H*W]) with G > 1 are a multi-view batch in training, as cam_poses are."""
         device = self.density_bitfield.device
         cam_poses = kwargs.get('cam_poses')
         cam_table = kwargs.get('cam_table')
@@ -106,6 +111,11 @@ class NeRFRenderer(nn.Module):
                 raise L.Mi3dError("ray_parallel needs step_seed (a value shared by all ranks, e.g. parallel.shared_seed(base, step))")
             seed = int(step_seed) if step_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())   # CPU generator: no device sync
             G, raygen, origins = 1, None, None
+            if cam_poses is None and len(prefix) == 2 and prefix[0] > 1:
+                G = prefix[0]
+                if G > L.MAX_VIEWS or par is not None:
+                    raise L.Mi3dError(f"a multi-view batch of explicit rays takes 2..{L.MAX_VIEWS} views on one rank; got {G}")
+                origins = rays_o.view(G, -1, 3)[:, 0]
             if cam_poses is not None:
                 from . import utils as U
                 Hc, Wc = kwargs['cam_hw']

@@ -22,6 +22,9 @@ Without text-encoder weights it returns a deterministic stand-in keyed by the pr
 `produce_latents` / `prompt_to_img` (nerf/sd.py:176-238) sample with DDIM (eta 0) and classifier-free guidance on the device
 (`mi3d_sd_sample`); `from_pretrained(local_dir, device)` loads a local diffusers directory; `python -m mi3d_b200.nerf.sd PROMPT --ckpt DIR`
 is the reference's demo.
+Batches of G views (2 <= G <= 8; the coarse stage's several views per iteration): `encode_imgs`, `unet_sds` and `train_step` take
+pred_rgb / latents [G,...] and run on a second engine planned for G views (U-Net batch 2G, VAE encoder batch G) on first use; its
+weights are the same parameter tensors.  ONE such engine is kept (33.5 GiB at G = 8, full size): a batch of another size replaces it.  The G views share one timestep; each takes the SDS or the denoise branch on its own.
 """
 import ctypes as C
 import hashlib
@@ -46,7 +49,7 @@ class UNetCfg(C.Structure):
 
 class VaeCfg(C.Structure):
     _fields_ = [("in_ch", C.c_int), ("latent_ch", C.c_int), ("n_levels", C.c_int), ("block_out", C.c_int * 4), ("layers_per_block", C.c_int),
-                ("groups", C.c_int), ("image_hw", C.c_int), ("decoder", C.c_int)]
+                ("groups", C.c_int), ("image_hw", C.c_int), ("decoder", C.c_int), ("batch", C.c_int)]
 
 
 def sd20_unet_cfg(latent_hw=64):
@@ -70,7 +73,7 @@ def sd_vae_cfg(image_hw=512):
     return dict(in_channels=3, latent_channels=4, block_out=(128, 256, 512, 512), layers_per_block=2, groups=32, image_hw=image_hw)
 
 
-def _unet_struct(cfg):
+def _unet_struct(cfg, views=1):
     u = UNetCfg()
     u.in_ch, u.out_ch, u.n_levels = cfg["in_channels"], cfg["out_channels"], len(cfg["block_out"])
     for i, v in enumerate(cfg["block_out"]):
@@ -78,18 +81,19 @@ def _unet_struct(cfg):
     for i, v in enumerate(cfg["heads"]):
         u.heads[i] = v
     u.layers_per_block, u.cross_dim, u.ctx_len, u.groups = cfg["layers_per_block"], cfg["cross_dim"], cfg["ctx_len"], cfg["groups"]
-    u.latent_hw, u.batch = cfg["latent_hw"], 2
+    u.latent_hw, u.batch = cfg["latent_hw"], 2 * views
     u.proj_conv = 1 if cfg.get("proj_conv", False) else 0
     return u
 
 
-def _vae_struct(cfg):
+def _vae_struct(cfg, views=1):
     v = VaeCfg()
     v.in_ch, v.latent_ch, v.n_levels = cfg["in_channels"], cfg["latent_channels"], len(cfg["block_out"])
     for i, c in enumerate(cfg["block_out"]):
         v.block_out[i] = c
     v.layers_per_block, v.groups, v.image_hw = cfg["layers_per_block"], cfg["groups"], cfg["image_hw"]
     v.decoder = 1 if cfg.get("decoder", True) else 0
+    v.batch = views
     return v
 
 
@@ -238,11 +242,13 @@ def _read_json(path):
 
 
 class SDEngine(L.Engine):
-    """The SD engine (mi3d_sd_create): U-Net and VAE launch lists planned in one workspace."""
+    """The SD engine (mi3d_sd_create): U-Net and VAE launch lists planned in one workspace, for `views` views per SDS step (U-Net
+    batch 2 * views, VAE encoder batch views)."""
 
-    def __init__(self, unet_cfg, vae_cfg, device, graph_replay=True):
-        self.u = _unet_struct(unet_cfg) if unet_cfg else None
-        self.v = _vae_struct(vae_cfg) if vae_cfg else None
+    def __init__(self, unet_cfg, vae_cfg, device, graph_replay=True, views=1):
+        self.views = views
+        self.u = _unet_struct(unet_cfg, views) if unet_cfg else None
+        self.v = _vae_struct(vae_cfg, views) if vae_cfg else None
         # graph_replay=False keeps plain launches on the caller's stream (used by the parity tests as the A/B arm)
         super().__init__("sd", (C.byref(self.u) if self.u else None, C.byref(self.v) if self.v else None), device, graph_replay,
                          f"SD configuration unet={unet_cfg} vae={vae_cfg}")
@@ -277,10 +283,10 @@ class _EncodeImgs(torch.autograd.Function):
         pred_rgb = L.f32c(pred_rgb)
         L.require_cuda(pred_rgb, eps)
         B, Cc, H, W = pred_rgb.shape
-        if B != 1 or Cc != 3:
-            raise L.Mi3dError("encode_imgs expects pred_rgb [1,3,H,W]")
+        if B != engine.views or Cc != 3:
+            raise L.Mi3dError(f"encode_imgs expects pred_rgb [{engine.views},3,H,W]")
         hw = engine.v.image_hw // 8
-        latents = torch.empty(1, 4, hw, hw, dtype=torch.float32, device=pred_rgb.device)
+        latents = torch.empty(B, 4, hw, hw, dtype=torch.float32, device=pred_rgb.device)
         with engine.on_stream():
             L.check(L.lib().mi3d_sd_encode(engine.h, L.ptr(pred_rgb), C.c_int(H), C.c_int(W), L.ptr(eps), L.ptr(latents), L.stream()), "sd_encode")
         ctx.engine, ctx.hw_in = engine, (H, W)
@@ -292,7 +298,7 @@ class _EncodeImgs(torch.autograd.Function):
         (eps,) = ctx.saved_tensors
         H, W = ctx.hw_in
         g = L.f32c(g)
-        grad = torch.empty(1, 3, H, W, dtype=torch.float32, device=g.device)
+        grad = torch.empty(g.shape[0], 3, H, W, dtype=torch.float32, device=g.device)
         with ctx.engine.on_stream():
             L.check(L.lib().mi3d_sd_encode_backward(ctx.engine.h, L.ptr(g), L.ptr(eps), C.c_int(H), C.c_int(W), L.ptr(grad), L.stream()),
                     "sd_encode_backward")
@@ -371,6 +377,7 @@ class StableDiffusion(nn.Module):
             setattr(self, k, v)
         self._schedules = {}          # (n, scheduler settings) -> device mi3d_sd_schedule table
         self._size_engines = {}       # image size -> SDEngine planned on first use by produce_latents / decode_latents
+        self._view_engine = None      # the one SDEngine for G > 1 views per SDS step, planned on first use (views_engine)
 
     def load_diffusers_state_dict(self, unet_state=None, vae_state=None, text_encoder_state=None):
         """copy tensors named like diffusers' UNet2DConditionModel / AutoencoderKL state_dict()s and push them to the engine;
@@ -396,7 +403,7 @@ class StableDiffusion(nn.Module):
     def reload(self):
         """push the current parameter values into the engine again (after load_state_dict)."""
         tensors = self._tensors()
-        for eng in [self.engine] + list(self._size_engines.values()):
+        for eng in [self.engine] + list(self._size_engines.values()) + ([self._view_engine] if self._view_engine else []):
             eng.load(tensors)
 
     def _tensors(self):
@@ -416,6 +423,23 @@ class StableDiffusion(nn.Module):
             eng.load(self._tensors())
             self._size_engines[size] = eng
         return eng
+
+    def views_engine(self, G):
+        """the engine of G-view SDS steps: the constructor's for G = 1, else the one multi-view engine (U-Net batch 2G, VAE encoder batch
+        G, no decoder: denoise-branch views decode one at a time on the constructor's engine), loaded from the same tensors.  Only one is
+        kept, so memory stays bounded by the largest batch in use: asking for another G frees the current one (an autograd node that still
+        holds it keeps it until its backward ran) and plans the new one.  Callers that mix batch sizes should run the odd ones view by
+        view instead (CoarseStep.step_views does)."""
+        if G == 1:
+            return self.engine
+        if not 1 <= G <= L.MAX_VIEWS:
+            raise L.Mi3dError(f"a batched SDS step takes 1..{L.MAX_VIEWS} views; got {G}")
+        if self._view_engine is None or self._view_engine.views != G:
+            self._view_engine = None                      # released before the new workspace is allocated
+            eng = SDEngine(self.unet_cfg, dict(self.vae_cfg, decoder=False), self.device, graph_replay=self.graph_replay, views=G)
+            eng.load(self._tensors())
+            self._view_engine = eng
+        return self._view_engine
 
     def _schedule(self, n):
         key = (n, self.timestep_spacing, self.steps_offset, self.set_alpha_to_one)
@@ -538,11 +562,13 @@ class StableDiffusion(nn.Module):
         return ids.reshape(1, T).to(self.device)
 
     def encode_imgs(self, imgs, eps=None):
-        """nerf/sd.py:212-220 (the 512x512 interpolation of :124 is folded in: pass the render-resolution image)."""
+        """nerf/sd.py:212-220 (the 512x512 interpolation of :124 is folded in: pass the render-resolution image).  imgs [G,3,H,W]:
+        G images at once on the G-view engine."""
         hw = self.vae_cfg["image_hw"] // 8
+        G = imgs.shape[0]
         if eps is None:
-            eps = torch.randn(1, 4, hw, hw, device=self.device)
-        return _EncodeImgs.apply(imgs, L.f32c(eps), self.engine)
+            eps = torch.randn(G, 4, hw, hw, device=self.device)
+        return _EncodeImgs.apply(imgs, L.f32c(eps), self.views_engine(G))
 
     def decode_latents(self, latents):
         """nerf/sd.py:201-210: (vae.decode(latents / 0.18215).sample / 2 + 0.5).clamp(0, 1) -> [B,3,S,S]; no gradient, like the reference.
@@ -599,12 +625,18 @@ class StableDiffusion(nn.Module):
         return loss, imgs
 
     def unet_sds(self, latents, noise, t, text_embeddings, guidance_scale):
-        """add_noise -> U-Net -> CFG -> SDS gradient (nerf/sd.py:138-170). t: device int64 [1]. Returns (noise_pred, grad)."""
+        """add_noise -> U-Net -> CFG -> SDS gradient (nerf/sd.py:138-170). t: device int64 [1]. Returns (noise_pred, grad).
+        latents / noise [G,4,h,w] of G views at the one timestep t; text_embeddings [2G,77,D] laid out [uncond x G, cond x G]."""
         latents, noise, text_embeddings = L.f32c(latents.detach()), L.f32c(noise), L.f32c(text_embeddings)
+        G = latents.shape[0]
+        if noise.numel() != latents.numel() or text_embeddings.dim() != 3 or text_embeddings.shape[0] != 2 * G:
+            raise L.Mi3dError(f"unet_sds: latents and noise [G,4,h,w] and text_embeddings [2G,77,D] expected; got {tuple(latents.shape)}, "
+                              f"{tuple(noise.shape)}, {tuple(text_embeddings.shape)}")
+        eng = self.views_engine(G)
         noise_pred = torch.empty_like(latents)
         grad = torch.empty_like(latents)
-        with self.engine.on_stream():
-            L.check(L.lib().mi3d_sd_unet_sds(self.engine.h, L.ptr(latents), L.ptr(noise), L.ptr(t), L.ptr(self.alphas), L.ptr(text_embeddings),
+        with eng.on_stream():
+            L.check(L.lib().mi3d_sd_unet_sds(eng.h, L.ptr(latents), L.ptr(noise), L.ptr(t), L.ptr(self.alphas), L.ptr(text_embeddings),
                                              C.c_float(float(guidance_scale)), L.ptr(noise_pred), L.ptr(grad), L.stream()), "sd_unet_sds")
         return noise_pred, grad
 
@@ -614,6 +646,9 @@ class StableDiffusion(nn.Module):
         (additive test hook: t, eps_posterior, noise make the step deterministic).  `defer` overrides the constructor's
         defer_backward for this call (None keeps it)."""
         defer = self.defer_backward if defer is None else bool(defer)
+        if pred_rgb.shape[0] > 1:
+            return self._train_step_views(text_embeddings, pred_rgb, ref_rgb, noise, islarge, ref_text, clip_model, guidance_scale, t,
+                                          eps_posterior, defer)
         loss, imgs = 0, None
         if t is None:
             t_host = int(torch.randint(self.min_step, self.max_step + 1, [1]).item())     # CPU generator: no device sync
@@ -637,7 +672,7 @@ class StableDiffusion(nn.Module):
                 with self.engine.on_stream():
                     L.check(L.lib().mi3d_sd_encode_backward(self.engine.h, L.ptr(grad), L.ptr(eps), C.c_int(H), C.c_int(W), L.ptr(grad_rgb), L.stream()),
                             "sd_encode_backward")
-            self.last = dict(latents=latents, noise_pred=noise_pred, grad=grad, t=t_host)
+            self.last = dict(latents=latents, noise_pred=noise_pred, grad=grad, t=t_host, grad_rgb=grad_rgb)
             return (grad_rgb * pred_rgb).sum(), None
         latents = self.encode_imgs(pred_rgb, eps_posterior)
         if noise is None:
@@ -653,6 +688,68 @@ class StableDiffusion(nn.Module):
                 return self._denoise_branch(noise_pred, latents_noisy, ref_rgb, ref_text, clip_model)
         latents.backward(gradient=grad, retain_graph=True)
         self.last = dict(latents=latents.detach(), noise_pred=noise_pred, grad=grad, t=t_host)
+        return loss, imgs
+
+    def _train_step_views(self, text_embeddings, pred_rgb, ref_rgb, noise, islarge, ref_text, clip_model, guidance_scale, t, eps_posterior,
+                          defer):
+        """train_step on G = pred_rgb.shape[0] views at one timestep: one encode, one U-Net pass at batch 2G and one encode backward on
+        the G-view engine.  text_embeddings [2,77,D] (shared) or [2G,77,D] ([uncond x G, cond x G]); islarge a bool or G bools; noise /
+        eps_posterior [G,4,h,w]; ref_rgb / ref_text one shared row or one per view.  Each view takes the reference's branch on its own:
+        large views, or t > 0.4 T, the SDS gradient; the others the denoise branch (DDIM step, decode, CLIP), without a gradient.
+        Returns (loss, imgs): loss = the denoise views' summed CLIP value (+ the SDS surrogate summed over the SDS views with defer),
+        imgs = a list of G decoded images, None for SDS views.  Without defer the SDS gradient is back-propagated here, as at G = 1."""
+        G, hw = pred_rgb.shape[0], self.vae_cfg["image_hw"] // 8
+        large = [bool(islarge)] * G if isinstance(islarge, (bool, int)) else [bool(x) for x in islarge]
+        te = L.f32c(text_embeddings)
+        if len(large) != G or te.dim() != 3 or te.shape[0] not in (2, 2 * G):
+            raise L.Mi3dError(f"train_step on {G} views: islarge takes a bool or {G} of them, text_embeddings [2,77,D] or [{2 * G},77,D]; got "
+                              f"{len(large)} flags and {tuple(te.shape)}")
+        if te.shape[0] == 2:
+            te = torch.cat([te[:1].expand(G, -1, -1), te[1:].expand(G, -1, -1)]).contiguous()
+        if t is None:
+            t_host = int(torch.randint(self.min_step, self.max_step + 1, [1]).item())     # CPU generator: no device sync
+            noise = None
+        else:
+            t_host = int(t)
+        self._t.fill_(t_host)
+        sds = [lg or t_host / self.num_train_timesteps > 0.4 for lg in large]
+        eng = self.views_engine(G)
+        rgb = L.f32c(pred_rgb.detach())
+        H, W = rgb.shape[-2:]
+        with torch.no_grad():
+            eps = L.f32c(eps_posterior) if eps_posterior is not None else torch.randn(G, 4, hw, hw, device=self.device)
+            latents = torch.empty(G, 4, hw, hw, dtype=torch.float32, device=rgb.device)
+            with eng.on_stream():
+                L.check(L.lib().mi3d_sd_encode(eng.h, L.ptr(rgb), C.c_int(H), C.c_int(W), L.ptr(eps), L.ptr(latents), L.stream()), "sd_encode")
+            if noise is None:
+                noise = torch.randn_like(latents)
+            noise = L.f32c(noise)
+            noise_pred, grad = self.unet_sds(latents, noise, self._t, te, guidance_scale)
+            loss, imgs = 0, [None] * G
+            if not all(sds):
+                a = self.alphas[t_host]
+                for v in range(G):
+                    if sds[v]:
+                        continue
+                    grad[v].zero_()
+                    if not self.vae_cfg.get("decoder", True):
+                        continue
+                    latents_noisy = a.sqrt() * latents[v:v + 1] + (1 - a).sqrt() * noise[v:v + 1]     # scheduler.add_noise (nerf/sd.py:141)
+                    pick = lambda x: x[v:v + 1] if torch.is_tensor(x) and x.dim() > 0 and x.shape[0] == G else x
+                    lv, imgs[v] = self._denoise_branch(noise_pred[v:v + 1], latents_noisy, pick(ref_rgb), pick(ref_text), clip_model)
+                    loss = loss + lv
+            grad_rgb = None
+            if any(sds):
+                grad_rgb = torch.empty_like(rgb)
+                with eng.on_stream():
+                    L.check(L.lib().mi3d_sd_encode_backward(eng.h, L.ptr(grad), L.ptr(eps), C.c_int(H), C.c_int(W), L.ptr(grad_rgb), L.stream()),
+                            "sd_encode_backward")
+        self.last = dict(latents=latents, noise_pred=noise_pred, grad=grad, t=t_host, sds=sds, denoise=loss, grad_rgb=grad_rgb)
+        if grad_rgb is not None and pred_rgb.requires_grad:
+            if defer:
+                loss = loss + (grad_rgb * pred_rgb).sum()
+            else:
+                torch.autograd.backward(pred_rgb, grad_rgb, retain_graph=True)
         return loss, imgs
 
 
