@@ -39,6 +39,10 @@ template <int BLOCK_N> struct Cfg {
     static constexpr int kStageBytes = kABytes + kBBytes;
     static constexpr size_t kSmemBytes = 1024 /*align slack*/ + (size_t)kStages * kStageBytes + 256;
     static constexpr int kMinBlocks = BLOCK_N == 64 ? 2 : 1;
+    // 8-column groups whose epilogue inputs are loaded together: as many as the register budget holds without spilling
+    // (BN = 256: the accumulator takes 128 of 168 registers; BN = 64: two CTAs per SM cap a thread at 85).  The QuickGELU
+    // instantiation at BN = 256 holds one group (with two it spills).
+    template <bool kQuickGelu> static constexpr int kEpiChunk = (BLOCK_N == 128 || BLOCK_N == 160) ? 4 : (kQuickGelu && BLOCK_N == 256 ? 1 : 2);
 };
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
@@ -163,47 +167,67 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUt
                 const bool row_ok = m < p.m_valid;
                 if (!row_ok) continue;
                 const float* rb = p.row_bias ? p.row_bias + (size_t)(((long long)z * p.M + m) / p.rows_per_group) * p.N : nullptr;
+                if (p.splits > 1) {
+                    // split-K partial: fp32 RED into the workspace; bias / residual / conversion happen in k_splitk_finish
+                    #pragma unroll
+                    for (int j = 0; j < BLOCK_N / 8; j++)
+                        atomicAdd(reinterpret_cast<float2*>(p.splitk_ws + (size_t)m * p.N + n_blk * BLOCK_N + 8 * j + 2 * (lane & 3)),
+                                  make_float2(acc[4 * j + 2 * hh], acc[4 * j + 2 * hh + 1]));
+                    continue;
+                }
+                // the epilogue's bias and fp16 input (residual / aux) of kEpiChunk 8-column groups are loaded before any of their outputs
+                // is stored: a load placed after a store waits for it (the pointers may alias), which made every group pay a full load
+                // latency (the row bias, on the deep-K time-embedding convs only, is still read in place)
+                const __half* in16 = nullptr;                  // the fp16 input of the mode, same row / column as the output
+                long long ld_in = p.ldc;
+                if (p.epi_mode == EPI_PLAIN && p.residual) { in16 = p.residual; ld_in = p.ld_res; }
+                else if ((kQuickGelu && p.epi_mode == EPI_QUICKGELU_BWD) || (kVgg && p.epi_mode == EPI_RELU_BWD)) in16 = p.aux;
+                constexpr int kChunk = C::template kEpiChunk<kQuickGelu>;
                 #pragma unroll
-                for (int j = 0; j < BLOCK_N / 8; j++) {
-                    const int n = n_blk * BLOCK_N + 8 * j + 2 * (lane & 3);
-                    float f0 = acc[4 * j + 2 * hh], f1 = acc[4 * j + 2 * hh + 1];
-                    if (p.splits > 1) {
-                        // split-K partial: fp32 RED into the workspace; bias / residual / conversion happen in k_splitk_finish
-                        atomicAdd(reinterpret_cast<float2*>(p.splitk_ws + (size_t)m * p.N + n), make_float2(f0, f1));
-                        continue;
+                for (int j0 = 0; j0 < BLOCK_N / 8; j0 += kChunk) {
+                    float2 bias_v[kChunk];
+                    __half2 in_v[kChunk];
+                    #pragma unroll
+                    for (int c = 0; c < kChunk; c++) {
+                        const int n = n_blk * BLOCK_N + 8 * (j0 + c) + 2 * (lane & 3);
+                        if (p.bias) bias_v[c] = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+                        if (in16) in_v[c] = *reinterpret_cast<const __half2*>(in16 + zoff + (size_t)m * ld_in + n);
                     }
-                    f0 *= p.alpha; f1 *= p.alpha;
-                    if (p.bias) { const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + n)); f0 += bv.x; f1 += bv.y; }
-                    if (rb) { const float2 bv = __ldg(reinterpret_cast<const float2*>(rb + n)); f0 += bv.x; f1 += bv.y; }
-                    if (p.epi_mode == EPI_GEGLU) {
-                        // weight rows were interleaved (value, gate) at plan time: out[:, n/2] = value * gelu(gate)
-                        p.out[zoff + (size_t)m * p.ldc + (n >> 1)] = __float2half_rn(f0 * gelu_erf(f1));
-                    } else if (p.epi_mode == EPI_TRANSPOSED) {
-                        __half* o = p.out + zoff + (size_t)n * p.ldc + m;
-                        o[0] = __float2half_rn(f0); o[p.ldc] = __float2half_rn(f1);
-                    } else if (kQuickGelu && p.epi_mode == EPI_QUICKGELU) {
-                        const size_t o = zoff + (size_t)m * p.ldc + n;
-                        if (p.aux) *reinterpret_cast<__half2*>(p.aux + o) = __floats2half2_rn(f0, f1);
-                        *reinterpret_cast<__half2*>(p.out + o) = __floats2half2_rn(quick_gelu(f0), quick_gelu(f1));
-                    } else if (kQuickGelu && p.epi_mode == EPI_QUICKGELU_BWD) {
-                        const size_t o = zoff + (size_t)m * p.ldc + n;
-                        const __half2 pre = *reinterpret_cast<const __half2*>(p.aux + o);
-                        *reinterpret_cast<__half2*>(p.out + o) = __floats2half2_rn(f0 * quick_gelu_grad(__low2float(pre)), f1 * quick_gelu_grad(__high2float(pre)));
-                    } else if (kVgg && p.epi_mode == EPI_RELU) {
-                        *reinterpret_cast<__half2*>(p.out + zoff + (size_t)m * p.ldc + n) = __floats2half2_rn(fmaxf(f0, 0.f), fmaxf(f1, 0.f));
-                    } else if (kVgg && p.epi_mode == EPI_RELU_BWD) {
-                        const size_t o = zoff + (size_t)m * p.ldc + n;
-                        const __half2 a = *reinterpret_cast<const __half2*>(p.aux + o);
-                        *reinterpret_cast<__half2*>(p.out + o) = __floats2half2_rn(__low2float(a) > 0.f ? f0 : 0.f, __high2float(a) > 0.f ? f1 : 0.f);
-                    } else if (kGelu && p.epi_mode == EPI_GELU) {
-                        *reinterpret_cast<__half2*>(p.out + zoff + (size_t)m * p.ldc + n) = __floats2half2_rn(gelu_erf(f0), gelu_erf(f1));
-                    } else {
-                        if (p.residual) {
-                            const __half2 rv = *reinterpret_cast<const __half2*>(p.residual + zoff + (size_t)m * p.ld_res + n);
-                            f0 += __low2float(rv); f1 += __high2float(rv);
+                    #pragma unroll
+                    for (int c = 0; c < kChunk; c++) {
+                        const int j = j0 + c;
+                        const int n = n_blk * BLOCK_N + 8 * j + 2 * (lane & 3);
+                        float f0 = acc[4 * j + 2 * hh], f1 = acc[4 * j + 2 * hh + 1];
+                        f0 *= p.alpha; f1 *= p.alpha;
+                        if (p.bias) { f0 += bias_v[c].x; f1 += bias_v[c].y; }
+                        if (rb) { const float2 bv = __ldg(reinterpret_cast<const float2*>(rb + n)); f0 += bv.x; f1 += bv.y; }
+                        if (p.epi_mode == EPI_GEGLU) {
+                            // weight rows were interleaved (value, gate) at plan time: out[:, n/2] = value * gelu(gate)
+                            p.out[zoff + (size_t)m * p.ldc + (n >> 1)] = __float2half_rn(f0 * gelu_erf(f1));
+                        } else if (p.epi_mode == EPI_TRANSPOSED) {
+                            __half* o = p.out + zoff + (size_t)n * p.ldc + m;
+                            o[0] = __float2half_rn(f0); o[p.ldc] = __float2half_rn(f1);
+                        } else if (kQuickGelu && p.epi_mode == EPI_QUICKGELU) {
+                            const size_t o = zoff + (size_t)m * p.ldc + n;
+                            if (p.aux) *reinterpret_cast<__half2*>(p.aux + o) = __floats2half2_rn(f0, f1);
+                            *reinterpret_cast<__half2*>(p.out + o) = __floats2half2_rn(quick_gelu(f0), quick_gelu(f1));
+                        } else if (kQuickGelu && p.epi_mode == EPI_QUICKGELU_BWD) {
+                            const __half2 pre = in_v[c];
+                            *reinterpret_cast<__half2*>(p.out + zoff + (size_t)m * p.ldc + n) =
+                                __floats2half2_rn(f0 * quick_gelu_grad(__low2float(pre)), f1 * quick_gelu_grad(__high2float(pre)));
+                        } else if (kVgg && p.epi_mode == EPI_RELU) {
+                            *reinterpret_cast<__half2*>(p.out + zoff + (size_t)m * p.ldc + n) = __floats2half2_rn(fmaxf(f0, 0.f), fmaxf(f1, 0.f));
+                        } else if (kVgg && p.epi_mode == EPI_RELU_BWD) {
+                            const __half2 a = in_v[c];
+                            *reinterpret_cast<__half2*>(p.out + zoff + (size_t)m * p.ldc + n) =
+                                __floats2half2_rn(__low2float(a) > 0.f ? f0 : 0.f, __high2float(a) > 0.f ? f1 : 0.f);
+                        } else if (kGelu && p.epi_mode == EPI_GELU) {
+                            *reinterpret_cast<__half2*>(p.out + zoff + (size_t)m * p.ldc + n) = __floats2half2_rn(gelu_erf(f0), gelu_erf(f1));
+                        } else {
+                            if (in16) { f0 += __low2float(in_v[c]); f1 += __high2float(in_v[c]); }
+                            if (p.out_f32) *reinterpret_cast<float2*>(p.out_f32 + zoff + (size_t)m * p.ldc + n) = make_float2(f0, f1);
+                            else *reinterpret_cast<__half2*>(p.out + zoff + (size_t)m * p.ldc + n) = __floats2half2_rn(f0, f1);
                         }
-                        if (p.out_f32) *reinterpret_cast<float2*>(p.out_f32 + zoff + (size_t)m * p.ldc + n) = make_float2(f0, f1);
-                        else *reinterpret_cast<__half2*>(p.out + zoff + (size_t)m * p.ldc + n) = __floats2half2_rn(f0, f1);
                     }
                 }
             }
