@@ -420,6 +420,16 @@ int mi3d_op_gemm(const mi3d_op_gemm_args* g, void* splitk_ws, size_t splitk_byte
 /* Builder::conv3: x [Nimg,H,W,Cin], w [Cout][3][3][Cin], y [Nimg,H,W,Cout]; row_bias [Nimg][Cout] (one row per image) */
 int mi3d_op_conv3(const void* x, const void* w, void* y, int Nimg, int H, int W, int Cin, int Cout, const float* bias, const float* row_bias,
                   const void* residual, void* splitk_ws, size_t splitk_bytes, int* plan, mi3d_stream_t stream);
+/* Builder::conv3_s2 (3x3 stride 2 as im2col + GEMM): x [Nimg,H,W,C], w [Cout][3][3][C], y [Nimg,Ho,Wo,Cout]; pad_lo 1 (padding 1) or 0
+ * (padding (0, 1, 0, 1)).  col: at least Nimg*Ho*Wo*9*C fp16 for the im2col matrix, which is left there. */
+int mi3d_op_conv3_s2(const void* x, const void* w, void* y, int Nimg, int H, int W, int C, int Ho, int Wo, int Cout, const float* bias, int pad_lo,
+                     void* col, size_t col_bytes, void* splitk_ws, size_t splitk_bytes, int* plan, mi3d_stream_t stream);
+/* Builder::conv_small_cin: x fp16 [Nimg,H,W,Cin] (Cin 4 or 8), w fp32 [Cout][3][3][Cin], y fp16 [Nimg,H,W,Cout] (Cout % 8 == 0).
+ * Builder::conv_small_cout: x fp16 [Nimg,H,W,Cin] (Cin % 8 == 0), w fp16 [Cout][3][3][Cin] (Cout 4 or 8), y fp32 [Nimg,H,W,Cout].
+ * Both 3x3 stride 1 padding 1; bias nullable. */
+int mi3d_op_conv_small_cin(const void* x, const float* w, const float* bias, void* y, int Nimg, int H, int W, int Cin, int Cout, mi3d_stream_t stream);
+int mi3d_op_conv_small_cout(const void* x, const void* w, const float* bias, float* y, int Nimg, int H, int W, int Cin, int Cout,
+                            mi3d_stream_t stream);
 /* Builder::conv3_block (any H x W): mode 0 plain (+ residual), 5 ReLU, 6 ReLU input gradient masked by aux > 0 */
 int mi3d_op_conv3_block(const void* x, const void* w, void* y, int Nimg, int H, int W, int Cin, int Cout, const float* bias, int mode,
                         const void* aux, const void* residual, int* plan, mi3d_stream_t stream);
@@ -441,6 +451,37 @@ int mi3d_op_layernorm_bwd(const void* x, const void* dy, const float* gamma, con
 int mi3d_op_softmax(void* s, size_t rows, int cols, int valid, int causal_tq, float scale, mi3d_stream_t stream);
 int mi3d_op_softmax_bwd(const void* p, void* dp, size_t rows, int cols, float scale, mi3d_stream_t stream);
 int mi3d_op_transpose(const void* in, void* out, int Z, int R, int C, mi3d_stream_t stream);
+/* The SD engine's own kernels with the launch geometry it plans (sd_engine.cu).
+ * mi3d_op_groupnorm: y = GroupNorm(+SiLU when silu) of x fp16 NHWC [N][HW][C] in G groups; stats: [N][G][2] doubles, zeroed by the caller,
+ * left holding each group's (sum, sum of squares).  mi3d_op_groupnorm_bwd: dx = the input gradient of dy (+ add, nullable) given the
+ * forward's stats; bstats: [N][G][2] zeroed doubles, left holding each group's sums of dg and dg * xhat (dg = dy * silu'(z) * gamma).
+ * geom (nullable, int[3]): the planned CTAs per image, pixels per CTA and pixel lanes per CTA. */
+int mi3d_op_groupnorm(const void* x, void* y, double* stats, const float* gamma, const float* beta, int N, int HW, int C, int G, float eps,
+                      int silu, int* geom, mi3d_stream_t stream);
+int mi3d_op_groupnorm_bwd(const void* x, const void* dy, const double* stats, double* bstats, const float* gamma, const float* beta,
+                          const void* add, void* dx, int N, int HW, int C, int G, float eps, int silu, int* geom, mi3d_stream_t stream);
+/* dx [N,H,W,C] of Builder::conv3_s2 from the gradient dcol [N*Ho*Wo][9*C] of its im2col matrix */
+int mi3d_op_col2im_s2(const void* dcol, void* dx, int N, int H, int W, int C, int Ho, int Wo, int pad_lo, mi3d_stream_t stream);
+/* The time-embedding linears: y_i[b][n] = bias_i[n] + sum_k act(x[b][k]) W_i[n][k] for b < B, x fp32 [B][K], W_i fp16 [N_i][K], y_i fp32
+ * [B][N_i], bias_i nullable.  grouped 0: one layer (layers = 1) with optional SiLU on x and on y; grouped 1: the per-ResBlock projections,
+ * `layers` of them in one launch, SiLU on x (silu_in = 1, silu_out = 0).  w, bias, y, N: host arrays of `layers` entries. */
+int mi3d_op_linear_small(const float* x, const void* const* w, const float* const* bias, float* const* y, const int* N, int layers, int B, int K,
+                         int silu_in, int silu_out, int grouped, mi3d_stream_t stream);
+/* The per-view latent kernels of mi3d_sd_encode / _backward and mi3d_sd_unet_sds, for G views (view v: the v-th slice of every per-view
+ * tensor): bilinear resize of rgb [G][3][H][W] to out fp16 [G][S][S][4] (2x - 1) and its input gradient from g fp32 [G][S*S][4];
+ * the posterior sample latents [G][4][pix] from conv_out [G][pix][8] through quant_conv (qw [8][8], qb [8]) and eps [G][4][pix], and
+ * its gradient g_conv_out [G][pix][8]; the noised U-Net input xin fp16 [2G][pix][4] (rows v and G + v of view v); CFG and the SDS
+ * gradient from unet_out [2G][pix][4] into noise_pred / grad [G][4][pix] (each nullable).  t: device int64 timestep. */
+int mi3d_op_interp_in(const float* rgb, int H, int W, void* out, int S, int G, mi3d_stream_t stream);
+int mi3d_op_interp_bwd(const float* g, int S, float* grad_rgb, int H, int W, int G, mi3d_stream_t stream);
+int mi3d_op_sample_latents(const float* conv_out, const float* qw, const float* qb, const float* eps, float* latents, int pix, int G,
+                           mi3d_stream_t stream);
+int mi3d_op_sample_latents_bwd(const float* conv_out, const float* qw, const float* qb, const float* eps, const float* g_lat, float* g_conv_out,
+                               int pix, int G, mi3d_stream_t stream);
+int mi3d_op_add_noise(const float* latents, const float* noise, const float* alphas_cumprod, const long long* t, void* xin, int pix, int G,
+                      mi3d_stream_t stream);
+int mi3d_op_cfg_sds(const float* unet_out, const float* noise, const float* alphas_cumprod, const long long* t, float guidance_scale,
+                    float* noise_pred, float* grad, int pix, int G, mi3d_stream_t stream);
 
 /* Stable-Diffusion engine: a statically planned launch list over the tile kernel above + memory-bound kernels.
  * Configuration mirrors diffusers' UNet2DConditionModel / AutoencoderKL config.json fields that nerf/sd.py:41,53 load. */

@@ -128,7 +128,9 @@ SYMBOLS = [
     "mi3d_sumsq_workspace_bytes", "mi3d_sumsq", "mi3d_adan_step", "mi3d_adam_step",
     "mi3d_tf32_tile_test",
     "mi3d_op_gemm", "mi3d_op_conv3", "mi3d_op_conv3_block", "mi3d_op_attention", "mi3d_op_attention_core", "mi3d_op_layernorm", "mi3d_op_layernorm_bwd",
-    "mi3d_op_softmax", "mi3d_op_softmax_bwd", "mi3d_op_transpose",
+    "mi3d_op_softmax", "mi3d_op_softmax_bwd", "mi3d_op_transpose", "mi3d_op_conv3_s2", "mi3d_op_conv_small_cin", "mi3d_op_conv_small_cout",
+    "mi3d_op_groupnorm", "mi3d_op_groupnorm_bwd", "mi3d_op_col2im_s2", "mi3d_op_linear_small", "mi3d_op_interp_in", "mi3d_op_interp_bwd",
+    "mi3d_op_sample_latents", "mi3d_op_sample_latents_bwd", "mi3d_op_add_noise", "mi3d_op_cfg_sds",
     "mi3d_engine_destroy", "mi3d_engine_num_params", "mi3d_engine_param_name", "mi3d_engine_param_shape", "mi3d_engine_load_param",
     "mi3d_engine_set_graph_replay", "mi3d_engine_graph_replays", "mi3d_engine_debug_tensor",
     "mi3d_sd_workspace_bytes", "mi3d_sd_create", "mi3d_sd_encode", "mi3d_sd_encode_backward", "mi3d_sd_unet_sds", "mi3d_sd_profile",

@@ -75,6 +75,12 @@ __global__ void __launch_bounds__(1024) k_sample_step(const float* __restrict__ 
     if (threadIdx.x == 0) s->step = step + 1;
 }
 
+// dx of Builder::conv3_s2 from the gradient of its im2col matrix (grid-stride over dx's 8-channel vectors)
+int col2im_s2(const __half* dcol, __half* dx, int N, int H, int W, int C, int Ho, int Wo, int pad_lo, cudaStream_t st) {
+    sdk::k_col2im_s2<<<Builder::blocks_for((size_t)N * H * W * C / 8), 256, 0, st>>>(dcol, dx, N, H, W, C, Ho, Wo, pad_lo);
+    return (int)cudaGetLastError();
+}
+
 struct Engine : Builder {
     mi3d_unet_cfg ucfg; mi3d_vae_cfg vcfg;
     // either part may be absent (NULL); a VAE-only engine takes its GroupNorm group count from the VAE
@@ -113,17 +119,10 @@ struct Engine : Builder {
         g.stats = pool_stats((size_t)x.n * g.G * 2);
         if (dry) return g;
         const int HW = x.h * x.w, C = x.c, G = g.G, N = x.n;
-        const int VPP = C / 8, PL = std::max(1, 256 / VPP), threads = PL * VPP;
-        if (G > 64 || threads > 1024 || C % 8) { err = MI3D_ERR_ARG; return g; }
-        // enough CTAs to fill the machine twice, at least PL*8 pixels each (more CTAs would only add partial sums to fold)
-        int chunks = std::max(1, std::min((HW + PL * 8 - 1) / (PL * 8), (2 * num_sms + N - 1) / N));
-        const int ppc = (HW + chunks - 1) / chunks; chunks = (HW + ppc - 1) / ppc;
+        sdk::GnGrid q;
+        if (!sdk::gn_grid(N, HW, C, G, num_sms, &q)) { err = MI3D_ERR_ARG; return g; }
         const __half* xp = x.p; __half* yp = y.p; const GN gg = g;
-        push([=](cudaStream_t st) {
-            sdk::k_gn_stats<<<dim3(chunks, N), threads, sdk::gn_smem_bytes(PL, C, G), st>>>(xp, HW, C, G, ppc, gg.stats);
-            sdk::k_gn_apply<<<dim3(chunks, N), threads, 0, st>>>(xp, yp, gg.stats, gg.gamma, gg.beta, HW, C, G, gg.eps, gg.silu, ppc);
-            return (int)cudaGetLastError();
-        });
+        push([=](cudaStream_t st) { return sdk::gn_forward(q, xp, yp, gg.stats, gg.gamma, gg.beta, N, HW, C, G, gg.eps, gg.silu, st); });
         return g;
     }
     // dx = GN(+SiLU) backward of dy (+ add)
@@ -131,21 +130,13 @@ struct Engine : Builder {
         double* bstats = pool_stats((size_t)g.x.n * g.G * 2);
         if (dry) return;
         const int HW = g.x.h * g.x.w, C = g.x.c, G = g.G, N = g.x.n;
-        const int VPP = C / 8, PL = std::max(1, 256 / VPP), threads = PL * VPP;
-        int chunks = std::max(1, std::min((HW + PL * 8 - 1) / (PL * 8), (2 * num_sms + N - 1) / N));
-        const int ppc = (HW + chunks - 1) / chunks; chunks = (HW + ppc - 1) / ppc;
+        sdk::GnGrid q;
+        if (!sdk::gn_grid(N, HW, C, G, num_sms, &q)) { err = MI3D_ERR_ARG; return; }
         const GN gg = g;
-        push([=](cudaStream_t st) {
-            sdk::k_gn_bwd_stats<<<dim3(chunks, N), threads, sdk::gn_smem_bytes(PL, C, G), st>>>(gg.x.p, dy, gg.stats, gg.gamma, gg.beta, HW, C, G, gg.eps, gg.silu, ppc, bstats);
-            sdk::k_gn_bwd_apply<<<dim3(chunks, N), threads, 0, st>>>(gg.x.p, dy, gg.stats, bstats, gg.gamma, gg.beta, HW, C, G, gg.eps, gg.silu, add, dx, ppc);
-            return (int)cudaGetLastError();
-        });
+        push([=](cudaStream_t st) { return sdk::gn_backward(q, gg.x.p, dy, gg.stats, bstats, gg.gamma, gg.beta, add, dx, N, HW, C, G, gg.eps, gg.silu, st); });
     }
     void linear_small(const float* x, const __half* w, const float* bias, float* y, int B, int N, int K, int silu_in, int silu_out) {
-        push([=](cudaStream_t st) {
-            sdk::k_linear_small<<<(N + 7) / 8, 256, 0, st>>>(x, w, bias, y, B, N, K, silu_in, silu_out);
-            return (int)cudaGetLastError();
-        });
+        push([=](cudaStream_t st) { return sdk::linear_small(x, w, bias, y, B, N, K, silu_in, silu_out, st); });
     }
 
     // ------------------------------------------------------------------------------------------------------
@@ -326,8 +317,7 @@ struct Engine : Builder {
             const float* te = temb;
             push([this, te, B, tdim](cudaStream_t st) {
                 if (temb_jobs.empty()) return 0;
-                sdk::k_linear_small_grouped<<<dim3((temb_max_n + 7) / 8, (unsigned)temb_jobs.size()), 256, 0, st>>>(te, temb_jobs_dev, B, tdim);
-                return (int)cudaGetLastError();
+                return sdk::linear_small_grouped(te, temb_jobs_dev, (int)temb_jobs.size(), temb_max_n, B, tdim, st);
             });
         }
         // conv_in (Cin = 4): direct
@@ -572,10 +562,7 @@ struct Engine : Builder {
                 linear(dh.p, Mo, C, (const __half*)w.dst2, 9 * C, dcol);
                 T4 dx = act(d.x.n, d.x.h, d.x.w, C);
                 const T4 xx = d.x, yy = d.y;
-                push([=](cudaStream_t st) {
-                    sdk::k_col2im_s2<<<blocks_for(dx.numel() / 8), 256, 0, st>>>(dcol, dx.p, xx.n, xx.h, xx.w, C, yy.h, yy.w, 0);
-                    return (int)cudaGetLastError();
-                });
+                push([=](cudaStream_t st) { return col2im_s2(dcol, dx.p, xx.n, xx.h, xx.w, C, yy.h, yy.w, 0, st); });
                 dh = dx;
             } else {
                 const AttnTape& a = vattn; const int C = a.x.c, nb = a.x.n, pix = a.x.h * a.x.w; const long long M = a.x.rows();
@@ -889,6 +876,34 @@ __global__ void k_cfg_sds(const float* __restrict__ unet_out /*[2G][pix][4]*/, c
     }
 }
 
+// The per-view launches: grid (pixel blocks, G views).  The API entry points below and the mi3d_op_* test entry points both call these.
+int interp_in(const float* rgb, int H, int W, __half* out, int S, int G, cudaStream_t st) {
+    k_interp_in<<<dim3((S * S + 255) / 256, G), 256, 0, st>>>(rgb, H, W, out, S);
+    return (int)cudaGetLastError();
+}
+int interp_bwd(const float* g, int S, float* grad_rgb, int H, int W, int G, cudaStream_t st) {
+    k_interp_bwd<<<dim3((H * W + 127) / 128, G), 128, 0, st>>>(g, S, grad_rgb, H, W);
+    return (int)cudaGetLastError();
+}
+int sample_latents(const float* conv_out, const float* qw, const float* qb, const float* eps, float* latents, int pix, int G, cudaStream_t st) {
+    k_sample_latents<<<dim3((pix + 127) / 128, G), 128, 0, st>>>(conv_out, qw, qb, eps, latents, pix);
+    return (int)cudaGetLastError();
+}
+int sample_latents_bwd(const float* conv_out, const float* qw, const float* qb, const float* eps, const float* g_lat, float* g_conv_out, int pix,
+                       int G, cudaStream_t st) {
+    k_sample_latents_bwd<<<dim3((pix + 127) / 128, G), 128, 0, st>>>(conv_out, qw, qb, eps, g_lat, g_conv_out, pix);
+    return (int)cudaGetLastError();
+}
+int add_noise(const float* lat, const float* noise, const float* alphas, const long long* t, __half* xin, int pix, int G, cudaStream_t st) {
+    k_add_noise<<<dim3((pix + 127) / 128, G), 128, 0, st>>>(lat, noise, alphas, t, xin, pix, G);
+    return (int)cudaGetLastError();
+}
+int cfg_sds(const float* unet_out, const float* noise, const float* alphas, const long long* t, float gs, float* noise_pred, float* grad, int pix,
+            int G, cudaStream_t st) {
+    k_cfg_sds<<<dim3((pix + 127) / 128, G), 128, 0, st>>>(unet_out, noise, alphas, t, gs, noise_pred, grad, pix, G);
+    return (int)cudaGetLastError();
+}
+
 }  // namespace sd
 
 extern "C" {
@@ -930,12 +945,11 @@ int mi3d_sd_encode(mi3d_engine_t h, const float* pred_rgb, int H, int W, const f
     if (!ep || ep->vcfg.n_levels == 0) return MI3D_ERR_ARG;
     cudaStream_t st = (cudaStream_t)stream; sd::Engine& e = *ep;
     const int S = e.vcfg.image_hw, G = e.vae_images();
-    sd::k_interp_in<<<dim3((S * S + 255) / 256, G), 256, 0, st>>>(pred_rgb, H, W, e.vae_in.p, S);
-    int r = e.run(e.enc_ops, st); if (r) return r;
+    int r = sd::interp_in(pred_rgb, H, W, e.vae_in.p, S, G, st); if (r) return r;
+    r = e.run(e.enc_ops, st); if (r) return r;
     const int pix = (int)e.v_h_last.rows() / G;
     const float* qw = (const float*)e.params[e.pindex["quant_conv.weight"]].dst; const float* qb = (const float*)e.params[e.pindex["quant_conv.bias"]].dst;
-    sd::k_sample_latents<<<dim3((pix + 127) / 128, G), 128, 0, st>>>(e.vae_moments, qw, qb, eps_posterior, latents, pix);
-    return (int)cudaGetLastError();
+    return sd::sample_latents(e.vae_moments, qw, qb, eps_posterior, latents, pix, G, st);
 }
 
 // backward of mi3d_sd_encode w.r.t. pred_rgb (weights frozen): grad_pred_rgb [G,3,H,W] fp32 (overwritten)
@@ -945,10 +959,9 @@ int mi3d_sd_encode_backward(mi3d_engine_t h, const float* grad_latents, const fl
     cudaStream_t st = (cudaStream_t)stream; sd::Engine& e = *ep;
     const int G = e.vae_images(), pix = (int)e.v_h_last.rows() / G, S = e.vcfg.image_hw;
     const float* qw = (const float*)e.params[e.pindex["quant_conv.weight"]].dst; const float* qb = (const float*)e.params[e.pindex["quant_conv.bias"]].dst;
-    sd::k_sample_latents_bwd<<<dim3((pix + 127) / 128, G), 128, 0, st>>>(e.vae_moments, qw, qb, eps_posterior, grad_latents, e.vae_gmoments, pix);
-    int r = e.run(e.enc_bwd_ops, st); if (r) return r;
-    sd::k_interp_bwd<<<dim3((H * W + 127) / 128, G), 128, 0, st>>>(e.vae_grad_img, S, grad_pred_rgb, H, W);
-    return (int)cudaGetLastError();
+    int r = sd::sample_latents_bwd(e.vae_moments, qw, qb, eps_posterior, grad_latents, e.vae_gmoments, pix, G, st); if (r) return r;
+    r = e.run(e.enc_bwd_ops, st); if (r) return r;
+    return sd::interp_bwd(e.vae_grad_img, S, grad_pred_rgb, H, W, G, st);
 }
 
 // nerf/sd.py:154-155: one DDIM step t -> t-1 on the noisy latents with the CFG-combined noise prediction.  All fp32 [1,4,h,w].
@@ -983,11 +996,10 @@ int mi3d_sd_unet_sds(mi3d_engine_t h, const float* latents, const float* noise, 
     if (B < 2 || B % 2 || e.ucfg.in_ch != 4) return MI3D_ERR_ARG;
     const int G = B / 2;
     MI3D_CHECK(cudaMemcpyAsync(e.t_dev, t, sizeof(long long), cudaMemcpyDeviceToDevice, st));
-    sd::k_add_noise<<<dim3((pix + 127) / 128, G), 128, 0, st>>>(latents, noise, alphas_cumprod, e.t_dev, e.unet_in.p, pix, G);
+    int r = sd::add_noise(latents, noise, alphas_cumprod, e.t_dev, e.unet_in.p, pix, G, st); if (r) return r;
     sd::k_ctx_pad<<<sd::Engine::blocks_for((size_t)B * e.ctx_pad * e.ucfg.cross_dim), 256, 0, st>>>(text_embeddings, e.ctx16, B, e.ucfg.ctx_len, e.ctx_pad, e.ucfg.cross_dim);
-    int r = e.run(e.unet_ops, st); if (r) return r;
-    sd::k_cfg_sds<<<dim3((pix + 127) / 128, G), 128, 0, st>>>(e.unet_out, noise, alphas_cumprod, e.t_dev, guidance_scale, noise_pred, grad, pix, G);
-    return (int)cudaGetLastError();
+    r = e.run(e.unet_ops, st); if (r) return r;
+    return sd::cfg_sds(e.unet_out, noise, alphas_cumprod, e.t_dev, guidance_scale, noise_pred, grad, pix, G, st);
 }
 
 // nerf/sd.py:176-199 produce_latents: n DDIM steps with CFG on the device; the text context is padded once, before the loop
@@ -1005,6 +1017,94 @@ int mi3d_sd_sample(mi3d_engine_t h, float* latents, const mi3d_sd_schedule* sche
     for (int i = 0; i < n; i++) { int r = e.run(e.sample_ops, st); if (r) return r; }
     MI3D_CHECK(cudaMemcpyAsync(latents, e.sample_lat, (size_t)count * sizeof(float), cudaMemcpyDeviceToDevice, st));
     return (int)cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Test entry points: one kernel of this engine with the launch geometry the engine plans (include/mi3d.h, the mi3d_op_* section)
+// ------------------------------------------------------------------------------------------------------------
+static int sms_of_device() {
+    int dev = 0, n = 0;
+    cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    return n;
+}
+
+int mi3d_op_groupnorm(const void* x, void* y, double* stats, const float* gamma, const float* beta, int N, int HW, int C, int G, float eps,
+                      int silu, int* geom, mi3d_stream_t stream) {
+    sdk::GnGrid q;
+    if (!x || !y || !stats || !gamma || !beta || !sdk::gn_grid(N, HW, C, G, sms_of_device(), &q)) return MI3D_ERR_ARG;
+    if (geom) { geom[0] = q.chunks; geom[1] = q.ppc; geom[2] = q.PL; }
+    return sdk::gn_forward(q, (const __half*)x, (__half*)y, stats, gamma, beta, N, HW, C, G, eps, silu, (cudaStream_t)stream);
+}
+
+int mi3d_op_groupnorm_bwd(const void* x, const void* dy, const double* stats, double* bstats, const float* gamma, const float* beta,
+                          const void* add, void* dx, int N, int HW, int C, int G, float eps, int silu, int* geom, mi3d_stream_t stream) {
+    sdk::GnGrid q;
+    if (!x || !dy || !stats || !bstats || !gamma || !beta || !dx || !sdk::gn_grid(N, HW, C, G, sms_of_device(), &q)) return MI3D_ERR_ARG;
+    if (geom) { geom[0] = q.chunks; geom[1] = q.ppc; geom[2] = q.PL; }
+    return sdk::gn_backward(q, (const __half*)x, (const __half*)dy, stats, bstats, gamma, beta, (const __half*)add, (__half*)dx, N, HW, C, G,
+                            eps, silu, (cudaStream_t)stream);
+}
+
+int mi3d_op_col2im_s2(const void* dcol, void* dx, int N, int H, int W, int C, int Ho, int Wo, int pad_lo, mi3d_stream_t stream) {
+    if (N < 1 || H < 1 || W < 1 || C % 8 || Ho < 1 || Wo < 1 || (pad_lo != 0 && pad_lo != 1)) return MI3D_ERR_ARG;
+    return sd::col2im_s2((const __half*)dcol, (__half*)dx, N, H, W, C, Ho, Wo, pad_lo, (cudaStream_t)stream);
+}
+
+int mi3d_op_linear_small(const float* x, const void* const* w, const float* const* bias, float* const* y, const int* N, int layers, int B, int K,
+                         int silu_in, int silu_out, int grouped, mi3d_stream_t stream) {
+    if (!x || !w || !bias || !y || !N || layers < 1 || layers > 64 || B < 1 || K < 8 || K % 8) return MI3D_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (!grouped) {
+        if (layers != 1 || N[0] < 1) return MI3D_ERR_ARG;
+        return sdk::linear_small(x, (const __half*)w[0], bias[0], y[0], B, N[0], K, silu_in, silu_out, st);
+    }
+    if (!silu_in || silu_out) return MI3D_ERR_ARG;          // the grouped kernel applies SiLU to x and nothing to y
+    sdk::SmallLinearJob jobs[64]; int max_n = 0;
+    for (int i = 0; i < layers; i++) {
+        if (N[i] < 1) return MI3D_ERR_ARG;
+        jobs[i] = {(const __half*)w[i], bias[i], y[i], N[i]}; max_n = std::max(max_n, N[i]);
+    }
+    sdk::SmallLinearJob* dev = nullptr;
+    MI3D_CHECK(cudaMallocAsync((void**)&dev, layers * sizeof(sdk::SmallLinearJob), st));
+    MI3D_CHECK(cudaMemcpyAsync(dev, jobs, layers * sizeof(sdk::SmallLinearJob), cudaMemcpyHostToDevice, st));
+    const int r = sdk::linear_small_grouped(x, dev, layers, max_n, B, K, st);
+    const int f = (int)cudaFreeAsync(dev, st);
+    MI3D_CHECK(cudaStreamSynchronize(st));                   // the job table is host memory of this frame
+    return r ? r : f;
+}
+
+int mi3d_op_interp_in(const float* rgb, int H, int W, void* out, int S, int G, mi3d_stream_t stream) {
+    if (!rgb || !out || H < 1 || W < 1 || S < 1 || G < 1) return MI3D_ERR_ARG;
+    return sd::interp_in(rgb, H, W, (__half*)out, S, G, (cudaStream_t)stream);
+}
+
+int mi3d_op_interp_bwd(const float* g, int S, float* grad_rgb, int H, int W, int G, mi3d_stream_t stream) {
+    if (!g || !grad_rgb || H < 1 || W < 1 || S < 1 || G < 1) return MI3D_ERR_ARG;
+    return sd::interp_bwd(g, S, grad_rgb, H, W, G, (cudaStream_t)stream);
+}
+
+int mi3d_op_sample_latents(const float* conv_out, const float* qw, const float* qb, const float* eps, float* latents, int pix, int G,
+                           mi3d_stream_t stream) {
+    if (!conv_out || !qw || !qb || !eps || !latents || pix < 1 || G < 1) return MI3D_ERR_ARG;
+    return sd::sample_latents(conv_out, qw, qb, eps, latents, pix, G, (cudaStream_t)stream);
+}
+
+int mi3d_op_sample_latents_bwd(const float* conv_out, const float* qw, const float* qb, const float* eps, const float* g_lat, float* g_conv_out,
+                               int pix, int G, mi3d_stream_t stream) {
+    if (!conv_out || !qw || !qb || !eps || !g_lat || !g_conv_out || pix < 1 || G < 1) return MI3D_ERR_ARG;
+    return sd::sample_latents_bwd(conv_out, qw, qb, eps, g_lat, g_conv_out, pix, G, (cudaStream_t)stream);
+}
+
+int mi3d_op_add_noise(const float* latents, const float* noise, const float* alphas_cumprod, const long long* t, void* xin, int pix, int G,
+                      mi3d_stream_t stream) {
+    if (!latents || !noise || !alphas_cumprod || !t || !xin || pix < 1 || G < 1) return MI3D_ERR_ARG;
+    return sd::add_noise(latents, noise, alphas_cumprod, t, (__half*)xin, pix, G, (cudaStream_t)stream);
+}
+
+int mi3d_op_cfg_sds(const float* unet_out, const float* noise, const float* alphas_cumprod, const long long* t, float guidance_scale,
+                    float* noise_pred, float* grad, int pix, int G, mi3d_stream_t stream) {
+    if (!unet_out || !noise || !alphas_cumprod || !t || pix < 1 || G < 1) return MI3D_ERR_ARG;
+    return sd::cfg_sds(unet_out, noise, alphas_cumprod, t, guidance_scale, noise_pred, grad, pix, G, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -6,6 +6,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
+
 #include "warp_reduce.cuh"
 
 namespace sdk {
@@ -44,13 +46,21 @@ __device__ __forceinline__ void gn_group_consts(const double* __restrict__ stats
 // Fold the per-thread partial sums sm[PL][C][2] of one CTA into its (group) totals and add them to out[G][2], in a FIXED order (run-to-run
 // deterministic): thread (g, q) first sums the group's channels of pixel lane q, then thread g sums the PL lanes (one thread per group
 // walking all cpg x PL slots serially would be a long dependent chain of double-precision adds).
+// pivot (nullable): the sums were taken of x - k with k = pivot[c] per channel; lane q's cnt terms give back, in fp64,
+// sum x = s + cnt k and sum x^2 = ss + 2 k s + cnt k^2.  p0, p1: the CTA's pixel range.
 // Dynamic shared memory: 2 * PL * C floats + 2 * G * PL doubles (gn_smem_bytes).
-__device__ __forceinline__ void gn_fold(const float* sm, int C, int G, int cpg, int PL, double* __restrict__ out) {
+__device__ __forceinline__ void gn_fold(const float* sm, int C, int G, int cpg, int PL, const __half* __restrict__ pivot, int p0, int p1,
+                                        double* __restrict__ out) {
     double* part = reinterpret_cast<double*>(const_cast<float*>(sm) + (((size_t)2 * PL * C + 1) & ~(size_t)1));
     for (int t = threadIdx.x; t < G * PL; t += blockDim.x) {
         const int g = t / PL, q = t - g * PL;
+        const double cnt = p1 - p0 > q ? (p1 - p0 - q + PL - 1) / PL : 0;
         double a = 0, b = 0;
-        for (int c = g * cpg; c < (g + 1) * cpg; c++) { a += sm[2 * (q * C + c)]; b += sm[2 * (q * C + c) + 1]; }
+        for (int c = g * cpg; c < (g + 1) * cpg; c++) {
+            double s = sm[2 * (q * C + c)], ss = sm[2 * (q * C + c) + 1];
+            if (pivot) { const double k = __half2float(pivot[c]); ss += k * (2 * s + cnt * k); s += cnt * k; }
+            a += s; b += ss;
+        }
         part[2 * t] = a; part[2 * t + 1] = b;
     }
     __syncthreads();
@@ -62,16 +72,41 @@ __device__ __forceinline__ void gn_fold(const float* sm, int C, int G, int cpg, 
 }
 inline size_t gn_smem_bytes(int PL, int C, int G) { return ((((size_t)2 * PL * C + 1) & ~(size_t)1) * sizeof(float)) + (size_t)2 * G * PL * sizeof(double); }
 
+// Launch geometry of the four GroupNorm kernels over N images of HW pixels, C channels in G groups: PL = max(1, 256 / VPP) pixel lanes of
+// VPP = C / 8 channel vectors per CTA, and per image `chunks` CTAs of ppc pixels each -- enough CTAs to fill the machine twice, at least
+// PL * 8 pixels each (more CTAs would only add partial sums to fold).  False for a shape the kernels cannot take.
+struct GnGrid { int chunks = 0, ppc = 0, PL = 0, threads = 0; };
+inline bool gn_grid(int N, int HW, int C, int G, int num_sms, GnGrid* q) {
+    if (N < 1 || HW < 1 || G < 1 || G > 64 || C % 8 || C % G) return false;
+    const int VPP = C / 8;
+    q->PL = std::max(1, 256 / VPP); q->threads = q->PL * VPP;
+    if (q->threads > 1024) return false;
+    const int chunks = std::max(1, std::min((HW + q->PL * 8 - 1) / (q->PL * 8), (2 * num_sms + N - 1) / N));
+    q->ppc = (HW + chunks - 1) / chunks; q->chunks = (HW + q->ppc - 1) / q->ppc;
+    return true;
+}
+
+// Statistics of x - k, k = the image's pixel 0 per channel (a shift by a value of the data): the fp32 sums then carry the rounding of
+// terms of the size of the group's spread, not of its mean, and E[x^2] - mean^2 does not cancel away the variance of groups whose |mean|
+// is large against their standard deviation.  gn_fold adds the shift back in fp64.
 __global__ void k_gn_stats(const __half* __restrict__ x, int HW, int C, int G, int pix_per_cta, double* __restrict__ stats /*[N][G][2]*/) {
     extern __shared__ float sm[];                 // [PL][C][2]: one slot per thread, folded in a FIXED order (run-to-run deterministic)
     const int n = blockIdx.y, cpg = C / G, VPP = C / 8, PL = blockDim.x / VPP;
     const int pl = threadIdx.x / VPP, cv = threadIdx.x % VPP;
     const int p0 = blockIdx.x * pix_per_cta, p1 = min(HW, p0 + pix_per_cta);
+    const __half* img = x + ((size_t)n * HW) * C;
     float s[8], ss[8];
     #pragma unroll
     for (int k = 0; k < 8; k++) { s[k] = 0.f; ss[k] = 0.f; }
     if (pl < PL) {
-        const __half* base = x + ((size_t)n * HW) * C + (size_t)cv * 8;
+        const __half* base = img + (size_t)cv * 8;
+        float piv[8];
+        {
+            const uint4 raw = __ldg(reinterpret_cast<const uint4*>(base));
+            const __half* h = reinterpret_cast<const __half*>(&raw);
+            #pragma unroll
+            for (int k = 0; k < 8; k++) piv[k] = __half2float(h[k]);
+        }
         // 4 independent 16-byte loads in flight per thread: with 2 CTAs x 8 warps per SM a single load per iteration leaves the
         // kernel latency-bound (Little's law); the pixel order of the sums is unchanged (still deterministic)
         int p = p0 + pl;
@@ -83,20 +118,20 @@ __global__ void k_gn_stats(const __half* __restrict__ x, int HW, int C, int G, i
             for (int u = 0; u < 4; u++) {
                 const __half* h = reinterpret_cast<const __half*>(&raw[u]);
                 #pragma unroll
-                for (int k = 0; k < 8; k++) { const float v = __half2float(h[k]); s[k] += v; ss[k] = fmaf(v, v, ss[k]); }
+                for (int k = 0; k < 8; k++) { const float v = __half2float(h[k]) - piv[k]; s[k] += v; ss[k] = fmaf(v, v, ss[k]); }
             }
         }
         for (; p < p1; p += PL) {
             const uint4 raw = __ldg(reinterpret_cast<const uint4*>(base + (size_t)p * C));
             const __half* h = reinterpret_cast<const __half*>(&raw);
             #pragma unroll
-            for (int k = 0; k < 8; k++) { const float v = __half2float(h[k]); s[k] += v; ss[k] = fmaf(v, v, ss[k]); }
+            for (int k = 0; k < 8; k++) { const float v = __half2float(h[k]) - piv[k]; s[k] += v; ss[k] = fmaf(v, v, ss[k]); }
         }
         #pragma unroll
         for (int k = 0; k < 8; k++) { sm[2 * (pl * C + cv * 8 + k)] = s[k]; sm[2 * (pl * C + cv * 8 + k) + 1] = ss[k]; }
     }
     __syncthreads();
-    gn_fold(sm, C, G, cpg, PL, stats + (size_t)n * G * 2);
+    gn_fold(sm, C, G, cpg, PL, img, p0, p1, stats + (size_t)n * G * 2);
 }
 
 // y = act((x - mean) * rstd * gamma + beta); same (chunks, N) grid and thread mapping as k_gn_stats
@@ -180,7 +215,7 @@ __global__ void k_gn_bwd_stats(const __half* __restrict__ x, const __half* __res
         for (int k = 0; k < 8; k++) { sm[2 * (pl * C + cv * 8 + k)] = s1[k]; sm[2 * (pl * C + cv * 8 + k) + 1] = s2[k]; }
     }
     __syncthreads();
-    gn_fold(sm, C, G, cpg, PL, bstats + (size_t)n * G * 2);
+    gn_fold(sm, C, G, cpg, PL, nullptr, 0, 0, bstats + (size_t)n * G * 2);
 }
 // pass 2: dx = rstd * (dg - mean(dg) - xhat * mean(dg*xhat)) (+ add, optional accumulation of another gradient branch)
 __global__ void k_gn_bwd_apply(const __half* __restrict__ x, const __half* __restrict__ dy, const double* __restrict__ stats,
@@ -235,6 +270,21 @@ __global__ void k_gn_bwd_apply(const __half* __restrict__ x, const __half* __res
     }
 }
 
+// y = GroupNorm(+SiLU)(x): statistics into the zeroed stats [N][G][2], then the normalisation
+inline int gn_forward(const GnGrid& q, const __half* x, __half* y, double* stats, const float* gamma, const float* beta, int N, int HW, int C,
+                      int G, float eps, int do_silu, cudaStream_t st) {
+    k_gn_stats<<<dim3(q.chunks, N), q.threads, gn_smem_bytes(q.PL, C, G), st>>>(x, HW, C, G, q.ppc, stats);
+    k_gn_apply<<<dim3(q.chunks, N), q.threads, 0, st>>>(x, y, stats, gamma, beta, HW, C, G, eps, do_silu, q.ppc);
+    return (int)cudaGetLastError();
+}
+// dx = GroupNorm(+SiLU) input gradient of dy (+ add): the forward's stats, the gradient sums into the zeroed bstats [N][G][2]
+inline int gn_backward(const GnGrid& q, const __half* x, const __half* dy, const double* stats, double* bstats, const float* gamma,
+                       const float* beta, const __half* add, __half* dx, int N, int HW, int C, int G, float eps, int do_silu, cudaStream_t st) {
+    k_gn_bwd_stats<<<dim3(q.chunks, N), q.threads, gn_smem_bytes(q.PL, C, G), st>>>(x, dy, stats, gamma, beta, HW, C, G, eps, do_silu, q.ppc, bstats);
+    k_gn_bwd_apply<<<dim3(q.chunks, N), q.threads, 0, st>>>(x, dy, stats, bstats, gamma, beta, HW, C, G, eps, do_silu, add, dx, q.ppc);
+    return (int)cudaGetLastError();
+}
+
 // channel concat: out[p][0:Ca] = a[p], out[p][Ca:Ca+Cb] = b[p]   (8-channel vectors)
 __global__ void k_concat(const __half* __restrict__ a, const __half* __restrict__ b, __half* __restrict__ out, size_t pixels, int Ca, int Cb) {
     const int va = Ca / 8, vb = Cb / 8, vt = va + vb;
@@ -287,23 +337,33 @@ __global__ void k_col2im_s2(const __half* __restrict__ dcol, __half* __restrict_
 }
 // dx[n,h,w] = sum of the 4 upsampled children (backward of nearest 2x) -- not needed by the frozen U-Net (no grad), kept out.
 
-// y[b][n] = bias[n] + sum_k act(x[b][k]) * W[n][k]   (B <= 8 rows; time embedding MLP and per-ResBlock temb projections)
+// y[b][n] = bias[n] + sum_k act(x[b][k]) * W[n][k]  (time embedding MLP and per-ResBlock temb projections; B = the U-Net batch, 2G)
+// One warp per output n.  The rows are taken in blocks of 8, each with its accumulators in registers (fully unrolled over the block, so
+// the row index is a constant); a block's rows keep the k order of the lanes' FMA chains and the warp tree whatever B is.
 __global__ void k_linear_small(const float* __restrict__ x, const __half* __restrict__ w, const float* __restrict__ bias, float* __restrict__ y,
                                int B, int N, int K, int silu_in, int silu_out) {
     const int n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (n >= N) return;
-    float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    for (int k = lane * 8; k < K; k += 256) {
-        const uint4 rw = *reinterpret_cast<const uint4*>(w + (size_t)n * K + k);
-        const __half* hw = reinterpret_cast<const __half*>(&rw);
-        for (int b = 0; b < B; b++) {
+    for (int b0 = 0; b0 < B; b0 += 8) {
+        const int nb = min(8, B - b0);
+        const float* xb = x + (size_t)b0 * K;
+        float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        for (int k = lane * 8; k < K; k += 256) {
+            const uint4 rw = *reinterpret_cast<const uint4*>(w + (size_t)n * K + k);
+            const __half* hw = reinterpret_cast<const __half*>(&rw);
             #pragma unroll
-            for (int j = 0; j < 8; j++) { float v = x[(size_t)b * K + k + j]; if (silu_in) v = silu(v); acc[b] = fmaf(v, __half2float(hw[j]), acc[b]); }
+            for (int b = 0; b < 8; b++) {
+                if (b >= nb) break;
+                #pragma unroll
+                for (int j = 0; j < 8; j++) { float v = xb[(size_t)b * K + k + j]; if (silu_in) v = silu(v); acc[b] = fmaf(v, __half2float(hw[j]), acc[b]); }
+            }
         }
-    }
-    for (int b = 0; b < B; b++) {
-        float v = warp_sum(acc[b]);
-        if (lane == 0) { v += bias ? bias[n] : 0.f; if (silu_out) v = silu(v); y[(size_t)b * N + n] = v; }
+        #pragma unroll
+        for (int b = 0; b < 8; b++) {
+            if (b >= nb) break;
+            float v = warp_sum(acc[b]);
+            if (lane == 0) { v += bias ? bias[n] : 0.f; if (silu_out) v = silu(v); y[(size_t)(b0 + b) * N + n] = v; }
+        }
     }
 }
 
@@ -313,19 +373,37 @@ __global__ void k_linear_small_grouped(const float* __restrict__ x, const SmallL
     const SmallLinearJob jb = jobs[blockIdx.y];
     const int n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (n >= jb.N) return;
-    float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    for (int k = lane * 8; k < K; k += 256) {
-        const uint4 rw = *reinterpret_cast<const uint4*>(jb.w + (size_t)n * K + k);
-        const __half* hw = reinterpret_cast<const __half*>(&rw);
-        for (int b = 0; b < B; b++) {
+    for (int b0 = 0; b0 < B; b0 += 8) {
+        const int nb = min(8, B - b0);
+        const float* xb = x + (size_t)b0 * K;
+        float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        for (int k = lane * 8; k < K; k += 256) {
+            const uint4 rw = *reinterpret_cast<const uint4*>(jb.w + (size_t)n * K + k);
+            const __half* hw = reinterpret_cast<const __half*>(&rw);
             #pragma unroll
-            for (int j = 0; j < 8; j++) acc[b] = fmaf(silu(x[(size_t)b * K + k + j]), __half2float(hw[j]), acc[b]);
+            for (int b = 0; b < 8; b++) {
+                if (b >= nb) break;
+                #pragma unroll
+                for (int j = 0; j < 8; j++) acc[b] = fmaf(silu(xb[(size_t)b * K + k + j]), __half2float(hw[j]), acc[b]);
+            }
+        }
+        #pragma unroll
+        for (int b = 0; b < 8; b++) {
+            if (b >= nb) break;
+            const float v = warp_sum(acc[b]);
+            if (lane == 0) jb.y[(size_t)(b0 + b) * jb.N + n] = v + (jb.bias ? jb.bias[n] : 0.f);
         }
     }
-    for (int b = 0; b < B; b++) {
-        const float v = warp_sum(acc[b]);
-        if (lane == 0) jb.y[(size_t)b * jb.N + n] = v + (jb.bias ? jb.bias[n] : 0.f);
-    }
+}
+
+// one warp per output feature, 8 features per CTA; the grouped form: one grid row per layer of the job table, max_n the widest layer
+inline int linear_small(const float* x, const __half* w, const float* bias, float* y, int B, int N, int K, int silu_in, int silu_out, cudaStream_t st) {
+    k_linear_small<<<(N + 7) / 8, 256, 0, st>>>(x, w, bias, y, B, N, K, silu_in, silu_out);
+    return (int)cudaGetLastError();
+}
+inline int linear_small_grouped(const float* x, const SmallLinearJob* jobs, int layers, int max_n, int B, int K, cudaStream_t st) {
+    k_linear_small_grouped<<<dim3((max_n + 7) / 8, (unsigned)layers), 256, 0, st>>>(x, jobs, B, K);
+    return (int)cudaGetLastError();
 }
 
 // sinusoidal timestep embedding (diffusers Timesteps, flip_sin_to_cos=True, freq_shift=0): out[b] = [cos | sin]

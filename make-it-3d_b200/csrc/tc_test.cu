@@ -51,6 +51,29 @@ int mi3d_op_conv3(const void* x, const void* w, void* y, int Nimg, int H, int W,
     return op.run(stream, plan);
 }
 
+// the im2col matrix of Builder::conv3_s2 is carved out of `col` (the builder's workspace)
+int mi3d_op_conv3_s2(const void* x, const void* w, void* y, int Nimg, int H, int W, int C, int Ho, int Wo, int Cout, const float* bias, int pad_lo,
+                     void* col, size_t col_bytes, void* splitk_ws, size_t splitk_bytes, int* plan, mi3d_stream_t stream) {
+    if (!col || (pad_lo != 0 && pad_lo != 1) || C % 8 || Ho < 1 || Wo < 1) return MI3D_ERR_ARG;
+    OneOp op(splitk_ws, splitk_bytes);
+    op.b.base = (uint8_t*)col; op.b.cap = col_bytes;
+    op.b.conv3_s2(t4(x, Nimg, H, W, C), (const __half*)w, t4(y, Nimg, Ho, Wo, Cout), bias, pad_lo);
+    return op.run(stream, plan);
+}
+
+int mi3d_op_conv_small_cin(const void* x, const float* w, const float* bias, void* y, int Nimg, int H, int W, int Cin, int Cout, mi3d_stream_t stream) {
+    OneOp op;
+    op.b.conv_small_cin(t4(x, Nimg, H, W, Cin), w, bias, t4(y, Nimg, H, W, Cout));
+    return op.run(stream);
+}
+
+int mi3d_op_conv_small_cout(const void* x, const void* w, const float* bias, float* y, int Nimg, int H, int W, int Cin, int Cout,
+                            mi3d_stream_t stream) {
+    OneOp op;
+    op.b.conv_small_cout(t4(x, Nimg, H, W, Cin), (const __half*)w, bias, y, Cout);
+    return op.run(stream);
+}
+
 int mi3d_op_conv3_block(const void* x, const void* w, void* y, int Nimg, int H, int W, int Cin, int Cout, const float* bias, int mode,
                         const void* aux, const void* residual, int* plan, mi3d_stream_t stream) {
     OneOp op;

@@ -48,17 +48,25 @@ class ColourClip:
 
 
 def test_batched_sds_matches_single_views_and_the_oracle(tiny):
+    """G = 3, and G = 8, the most nerf/sd.py plans: there the U-Net runs at batch 16, and the text rows G + v cross batch row 8 (the
+    time-embedding linears hold their rows in blocks of 8)"""
+    for views in (G, 8):
+        _check_batched_sds(tiny, views)
+
+
+def _check_batched_sds(tiny, views):
+    print(f"G = {views}")
     sdm, g, unet, vae = tiny
-    rgb, eps, noise, ctx = _inputs(31)
-    large = [False, True, False]
+    rgb, eps, noise, ctx = _inputs(31, views)
+    large = [v % 3 == 1 for v in range(views)]
     rb = rgb.clone().requires_grad_()
     loss, imgs = g.train_step(ctx, rb, islarge=large, guidance_scale=10, t=500, eps_posterior=eps, noise=noise)
-    assert loss == 0 and imgs == [None] * G and g.last["sds"] == [True] * G
+    assert loss == 0 and imgs == [None] * views and g.last["sds"] == [True] * views
     batch = {k: g.last[k].clone() for k in ("latents", "noise_pred", "grad")}
-    assert g.views_engine(G).views == G and g.views_engine(G) is not g.engine
-    for v in range(G):
+    assert g.views_engine(views).views == views and g.views_engine(views) is not g.engine
+    for v in range(views):
         rv = rgb[v:v + 1].clone().requires_grad_()
-        g.train_step(_one(ctx, v), rv, islarge=large[v], guidance_scale=10, t=500, eps_posterior=eps[v:v + 1], noise=noise[v:v + 1])
+        g.train_step(_one(ctx, v, views), rv, islarge=large[v], guidance_scale=10, t=500, eps_posterior=eps[v:v + 1], noise=noise[v:v + 1])
         torch.cuda.synchronize()
         # CFG amplifies the U-Net's (text - uncond) by the guidance scale: noise_pred and grad are compared at that scale, as
         # test_sd_gpu compares them with the oracle; the U-Net's own output is held to 1e-2 below
@@ -72,16 +80,18 @@ def test_batched_sds_matches_single_views_and_the_oracle(tiny):
         # guidance scale 0: noise_pred is the U-Net's text-row output, row G + v of the batch-2G pass against row 1 of the batch-2 pass
         tt = torch.tensor([500], dtype=torch.long, device="cuda")
         raw_b, _ = g.unet_sds(batch["latents"], noise, tt, ctx, 0.0)
-        raw_1, _ = g.unet_sds(batch["latents"][v:v + 1], noise[v:v + 1], tt, _one(ctx, v), 0.0)
+        raw_1, _ = g.unet_sds(batch["latents"][v:v + 1], noise[v:v + 1], tt, _one(ctx, v, views), 0.0)
         e, c = _rel(raw_b[v], raw_1[0])
         print(f"view {v} U-Net out   batch vs single rel_l2={e:.3e} cos={c:.6f}")
         assert e < 1e-2 and c > 0.9999, (v, "U-Net output", e, c)
         # each view against the fp32 oracle (the bounds of test_sd_gpu's oracle comparisons)
         rr = rgb[v:v + 1].cpu().clone().requires_grad_()
-        ref = sd_ref.sds_train_step_ref_at(unet, vae, _one(ctx, v).cpu(), rr, 500, eps[v:v + 1].cpu(), noise[v:v + 1].cpu(), 256, guidance_scale=10.0)
+        ref = sd_ref.sds_train_step_ref_at(unet, vae, _one(ctx, v, views).cpu(), rr, 500, eps[v:v + 1].cpu(), noise[v:v + 1].cpu(), 256, guidance_scale=10.0)
         e, c = _rel(batch["latents"][v], ref["latents"][0])
+        print(f"view {v} latents    batch vs oracle rel_l2={e:.3e} cos={c:.6f}")
         assert e < 1e-2 and c > 0.9999, (v, "oracle latents", e, c)
         e, c = _rel(batch["noise_pred"][v], ref["noise_pred"][0])
+        print(f"view {v} noise_pred batch vs oracle rel_l2={e:.3e} cos={c:.6f}")
         assert e < 3e-2 and c > 0.999, (v, "oracle noise_pred", e, c)
         e, c = _rel(rb.grad[v], rr.grad[0])
         print(f"view {v} d pred_rgb  batch vs oracle rel_l2={e:.3e} cos={c:.6f}")
